@@ -11,7 +11,7 @@ extern "C" {
 #endif
 
 enum { FILT_SHUFFLE = 0, FILT_UNSHUFFLE = 1, FILT_BITSHUFFLE = 2, FILT_BITUNSHUFFLE = 3 };
-enum { B2_CODEC_BLOSCLZ = 0, B2_CODEC_LZ4 = 1, B2_CODEC_ZLIB = 2, B2_CODEC_ZSTD = 3 /* the last two: decode only */ };
+enum { B2_CODEC_BLOSCLZ = 0, B2_CODEC_LZ4 = 1, B2_CODEC_ZLIB = 2 /* decode only */, B2_CODEC_ZSTD = 3 };
 
 typedef struct FilterArgs {
   const uint8_t* src;
@@ -109,6 +109,11 @@ typedef struct FastArgs {
   int* done;
   int fold_scan;
   ScanArgs scan;
+  /* zstd encoder (dev_zstdenc.cuh): the same index and windows, sequence records instead of LZ4 bytes, then one warp
+   * per stream writes its zstd frame; segs / seg_done / ptail are not used */
+  int zstd;
+  uint32_t* recs;                  /* 64 records per segment, segment-major as segs */
+  uint32_t* nrec;                  /* records per segment */
 } FastArgs;
 
 typedef struct CompactArgs {

@@ -60,6 +60,8 @@ extern "C" int b2_device_prepare(void) {
   CK(cudaFuncSetAttribute(decode_kernel<B2_CODEC_ZSTD>, cudaFuncAttributeMaxDynamicSharedMemorySize, DECODE_WARPS * LZ4D_SMEM));
   CK(cudaFuncSetAttribute(index_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, INDEX_WARPS * FAST_TAB_BYTES));
   CK(cudaFuncSetAttribute(parse_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, B2_FAST_WIN_MAX + 64));
+  CK(cudaFuncSetAttribute(zparse_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, B2_FAST_WIN_MAX + 64));
+  CK(cudaFuncSetAttribute(zenc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, ZE_WARPS * ZE_SMEM_BYTES));
   CK(cudaFuncSetAttribute(filter_kernel<0>, cudaFuncAttributeMaxDynamicSharedMemorySize, FILT_WARPS * 16 * FILT_TILE));
   CK(cudaFuncSetAttribute(filter_kernel<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, FILT_WARPS * 16 * FILT_TILE));
   CK(cudaFuncSetAttribute(filter_kernel<4>, cudaFuncAttributeMaxDynamicSharedMemorySize, FILT_WARPS * 16 * FILT_TILE));
@@ -233,7 +235,8 @@ extern "C" int b2_launch_encode(const EncodeArgs* a, b2_stream_t s) {
   return 0;
 }
 
-/* segment-parallel LZ4: the hash-chain index of every stream, then one lane per segment */
+/* segment-parallel LZ4: the hash-chain index of every stream, then one lane per segment; a->zstd: the same index and
+ * parse into zstd sequence records, then one warp per zstd frame (dev_zstdenc.cuh) */
 extern "C" int b2_launch_fast(const FastArgs* a, b2_stream_t s) {
   if (a->map.nstreams <= 0) return 0;
   {
@@ -256,8 +259,16 @@ extern "C" int b2_launch_fast(const FastArgs* a, b2_stream_t s) {
     FastArgs args = *a;
     args.queue_base = *a->queue_base_host;
     *a->queue_base_host += (unsigned)njobs + (unsigned)ctas;      /* one ticket-drawing thread per CTA */
-    parse_kernel<<<(unsigned)ctas, threads, smem, s->s>>>(args);
+    if (a->zstd) zparse_kernel<<<(unsigned)ctas, threads, smem, s->s>>>(args);
+    else parse_kernel<<<(unsigned)ctas, threads, smem, s->s>>>(args);
     CK(cudaGetLastError());
+  }
+  if (a->zstd) {                                                  /* one warp per zstd frame */
+    const int ctas = (a->map.nstreams + ZE_WARPS - 1) / ZE_WARPS;
+    ProfScope ps(B2_K_ZENC, s->s);
+    zenc_kernel<<<ctas, ZE_WARPS * 32, ZE_WARPS * ZE_SMEM_BYTES, s->s>>>(*a);
+    CK(cudaGetLastError());
+    return 0;
   }
   {
     const int ctas = (a->map.nstreams + FSCAN_WARPS - 1) / FSCAN_WARPS;

@@ -280,12 +280,20 @@ int blosc_free_resources(void) {                              /* blosc.h:411 */
 /* ------------------------------------------------------------------------- */
 /* names                                                                      */
 /* ------------------------------------------------------------------------- */
+/* BLOSC_B200_ZSTD=1 (read on every call) makes the library behave like a reference built with zstd: "zstd" chunks
+ * are then written (dev_zstdenc.cuh).  Unset, it is a reference built without zstd, which still reads them. */
+static int zstd_enabled(void) {
+  const char* e = getenv("BLOSC_B200_ZSTD");
+  return e && *e && atoi(e) != 0;
+}
+
 int blosc_compcode_to_compname(int compcode, const char** compname) {    /* blosc.c:329-374 */
   static const char* names[6] = {BLOSC_BLOSCLZ_COMPNAME, BLOSC_LZ4_COMPNAME, BLOSC_LZ4HC_COMPNAME,
                                  BLOSC_SNAPPY_COMPNAME, BLOSC_ZLIB_COMPNAME, BLOSC_ZSTD_COMPNAME};
   *compname = (compcode >= 0 && compcode < 6) ? names[compcode] : NULL;
   /* codecs this build can ENCODE; like a reference built without the others */
   if (compcode == BLOSC_BLOSCLZ || compcode == BLOSC_LZ4 || compcode == BLOSC_LZ4HC) return compcode;
+  if (compcode == BLOSC_ZSTD && zstd_enabled()) return compcode;
   return -1;
 }
 
@@ -293,10 +301,14 @@ int blosc_compname_to_compcode(const char* compname) {                    /* blo
   if (strcmp(compname, BLOSC_BLOSCLZ_COMPNAME) == 0) return BLOSC_BLOSCLZ;
   if (strcmp(compname, BLOSC_LZ4_COMPNAME) == 0) return BLOSC_LZ4;
   if (strcmp(compname, BLOSC_LZ4HC_COMPNAME) == 0) return BLOSC_LZ4HC;
+  if (strcmp(compname, BLOSC_ZSTD_COMPNAME) == 0 && zstd_enabled()) return BLOSC_ZSTD;
   return -1;
 }
 
-const char* blosc_list_compressors(void) { return BLOSC_BLOSCLZ_COMPNAME "," BLOSC_LZ4_COMPNAME "," BLOSC_LZ4HC_COMPNAME; }   /* blosc.c:2033-2056 */
+const char* blosc_list_compressors(void) {                                  /* blosc.c:2033-2056 */
+  if (zstd_enabled()) return BLOSC_BLOSCLZ_COMPNAME "," BLOSC_LZ4_COMPNAME "," BLOSC_LZ4HC_COMPNAME "," BLOSC_ZSTD_COMPNAME;
+  return BLOSC_BLOSCLZ_COMPNAME "," BLOSC_LZ4_COMPNAME "," BLOSC_LZ4HC_COMPNAME;
+}
 const char* blosc_get_version_string(void) { return BLOSC_VERSION_STRING; }
 
 int blosc_get_complib_info(const char* compname, char** complib, char** version) {   /* blosc.c:2063-2124 */
@@ -305,6 +317,8 @@ int blosc_get_complib_info(const char* compname, char** complib, char** version)
   if (strcmp(compname, BLOSC_BLOSCLZ_COMPNAME) == 0) { code = BLOSC_BLOSCLZ_LIB; lib = "BloscLZ"; ver = "2.5.1"; }
   else if (strcmp(compname, BLOSC_LZ4_COMPNAME) == 0 || strcmp(compname, BLOSC_LZ4HC_COMPNAME) == 0) {
     code = BLOSC_LZ4_LIB; lib = "LZ4"; ver = "1.10.0";
+  } else if (strcmp(compname, BLOSC_ZSTD_COMPNAME) == 0 && zstd_enabled()) {
+    code = BLOSC_ZSTD_LIB; lib = "Zstd"; ver = "1.5.6";         /* the zstd release the frames are checked against */
   }
   if (code < 0) {
     if (complib) *complib = NULL;
@@ -575,6 +589,7 @@ static int compress_impl(int clevel, int doshuffle, size_t typesize, size_t nbyt
   if (compcode == BLOSC_BLOSCLZ) compformat = BLOSC_BLOSCLZ_FORMAT;
   else if (compcode == BLOSC_LZ4) compformat = BLOSC_LZ4_FORMAT;
   else if (compcode == BLOSC_LZ4HC) compformat = BLOSC_LZ4HC_FORMAT;     /* blosc.c:1170-1172: the LZ4 format */
+  else if (compcode == BLOSC_ZSTD) compformat = BLOSC_ZSTD_FORMAT;       /* blosc.c:1190-1196 */
   else {
     fprintf(stderr, "Blosc has not been compiled with '%s' ", compressor ? compressor : "(null)");
     fprintf(stderr, "compression support.  Please use one having it.");
@@ -657,7 +672,36 @@ static int compress_impl(int clevel, int doshuffle, size_t typesize, size_t nbyt
     ea.scan = sa;
     launched = 1;
     memset(&ca, 0, sizeof ca);
-    if (ea.codec == B2_CODEC_LZ4 && (compcode == BLOSC_LZ4HC || lz4_fast_wanted())) {
+    if (compcode == BLOSC_ZSTD) {
+      /* the zstd encoder (dev_zstdenc.cuh): the index and windows of the segment-parallel parse, sequence records
+       * instead of LZ4 bytes, then one warp per zstd frame */
+      FastArgs fx;
+      const int neblock = bs / nsplits;
+      const int longest = neblock > leftover ? neblock : leftover;
+      int win = (longest + 32 * B2_FAST_SEG - 1) / (32 * B2_FAST_SEG) * (32 * B2_FAST_SEG);
+      long long nsegs;
+      b2_buf* recs;
+      memset(&fx, 0, sizeof fx);
+      if (win > B2_FAST_WIN_MAX) win = B2_FAST_WIN_MAX;
+      fx.map = ea.map; fx.in = ea.in; fx.slots = ea.slots; fx.csizes = ea.csizes; fx.needs = ea.needs;
+      fx.segs_full = (neblock + B2_FAST_SEG - 1) / B2_FAST_SEG; fx.segs_left = (leftover + B2_FAST_SEG - 1) / B2_FAST_SEG;
+      fx.win_bytes = win; fx.threads = win / B2_FAST_SEG;
+      fx.groups_full = (neblock + win - 1) / win; fx.groups_left = (leftover + win - 1) / win;
+      /* effort: the chain depth and laziness of "lz4hc" (blosc.c:499-511 maps clevel to zstd levels 1..22) */
+      fx.depth = clevel <= 2 ? 4 : (clevel >= 8 ? 128 : (1 << (clevel - 1))); fx.accel = 1;
+      fx.hash_mask = 0xffff; fx.lazy = 64;
+      nsegs = (long long)nfull * nsplits * fx.segs_full + fx.segs_left;
+      /* the records need 256 bytes per segment; whichever of the staging / filter buffers does not hold the
+       * codec input is free for them */
+      recs = d_codec_in == (const uint8_t*)w->in.p ? &w->filt : &w->in;
+      if (buf_ensure(&w->prev, 2 * (size_t)nb + 64)) break;
+      if (buf_ensure(recs, (size_t)nsegs * B2_FAST_SEG + 64)) break;
+      if (buf_ensure(&w->segs, (size_t)nsegs * 4 + 64)) break;
+      fx.prev = (uint16_t*)w->prev.p; fx.zstd = 1; fx.recs = (uint32_t*)recs->p; fx.nrec = (uint32_t*)w->segs.p;
+      fx.queue = ea.queue; fx.queue_base_host = ea.queue_base_host; fx.done = ea.done;
+      fx.fold_scan = ea.fold_scan; fx.scan = sa;
+      if (b2_launch_fast(&fx, w->stream)) break;
+    } else if (ea.codec == B2_CODEC_LZ4 && (compcode == BLOSC_LZ4HC || lz4_fast_wanted())) {
       FastArgs fx;
       const int neblock = bs / nsplits;
       memset(&fx, 0, sizeof fx);

@@ -21,6 +21,7 @@
 #include "dev_lz4fast.cuh"
 #include "dev_lz4dpair.cuh"
 #include "dev_zstd.cuh"
+#include "dev_zstdenc.cuh"
 
 
 
@@ -243,12 +244,9 @@ __global__ void __launch_bounds__(INDEX_WARPS * 32) index_kernel(FastArgs a) {
 /* One CTA per window of a stream (at most B2_FAST_WIN_MAX bytes): the window's bytes are staged in shared memory, then every THREAD parses one segment of FAST_SEG bytes.
  * Candidate compares -- the random accesses of LZ matching -- hit shared memory; only the chain links (prev[]) and
  * candidates in front of the window come from L2. */
-__global__ void __launch_bounds__(B2_FAST_WIN_MAX / FAST_SEG, 3) parse_kernel(FastArgs a) {
-#ifdef SIMT_EMU
-  u8* smem = simt::g_dynsmem;
-#else
-  extern __shared__ __align__(16) u8 smem[];
-#endif
+/* ZSTD: the same windows and segments, parsed into zstd sequence records (dev_zstdenc.cuh) instead of LZ4 bytes */
+template <bool ZSTD>
+DEV void fast_parse_body(const FastArgs& a, u8* smem) {
   u32* sdata = (u32*)smem;
   int* sjob = (int*)(smem + a.win_bytes + 48);
   const int tid = (int)threadIdx.x, lane = lane_id();
@@ -274,7 +272,7 @@ __global__ void __launch_bounds__(B2_FAST_WIN_MAX / FAST_SEG, 3) parse_kernel(Fa
     int block, len, split;
     long long off;
     stream_locate(a.map, idx, &block, &off, &len, &split);
-    FastSeg* segs = a.segs + (long long)idx * a.segs_full;
+    FastSeg* segs = ZSTD ? nullptr : a.segs + (long long)idx * a.segs_full;
     FastView v = fast_view(a.in + off, len);
     const int wa = g * a.win_bytes, wb = wa + a.win_bytes < len ? wa + a.win_bytes : len;
     /* stage the 16-byte granules that overlap the window (they lie inside the buffer's allocation: device
@@ -303,16 +301,49 @@ __global__ void __launch_bounds__(B2_FAST_WIN_MAX / FAST_SEG, 3) parse_kernel(Fa
       const int k = g * spw + t;
       if (t >= spw || k >= K) break;
       const int sa = k * FAST_SEG, sb = sa + FAST_SEG < len ? sa + FAST_SEG : len;
-      lz4f_parse_lane(v, len, a.prev + off, sa, sb, a.slots + off + sa, &segs[k], a.depth, a.accel, a.lazy);
+      if (ZSTD) {
+        const long long gk = (long long)idx * a.segs_full + k;
+        a.nrec[gk] = (u32)zse_parse_lane(v, len, a.prev + off, sa, sb, a.recs + gk * ZE_SEG_RECS, a.depth, a.lazy);
+      } else {
+        lz4f_parse_lane(v, len, a.prev + off, sa, sb, a.slots + off + sa, &segs[k], a.depth, a.accel, a.lazy);
+      }
     }
     __syncthreads();                               /* shared memory may be reused */
   }
 }
 
+__global__ void __launch_bounds__(B2_FAST_WIN_MAX / FAST_SEG, 3) parse_kernel(FastArgs a) {
+#ifdef SIMT_EMU
+  u8* smem = simt::g_dynsmem;
+  if (a.zstd) { fast_parse_body<true>(a, smem); return; }     /* the emulator launches the zstd parse under this name */
+#else
+  extern __shared__ __align__(16) u8 smem[];
+#endif
+  fast_parse_body<false>(a, smem);
+}
+
+/* FastArgs.zstd: the zstd encoder's parse (the backend launches it instead of parse_kernel) */
+__global__ void __launch_bounds__(B2_FAST_WIN_MAX / FAST_SEG, 3) zparse_kernel(FastArgs a) {
+#ifdef SIMT_EMU
+  u8* smem = simt::g_dynsmem;
+#else
+  extern __shared__ __align__(16) u8 smem[];
+#endif
+  fast_parse_body<true>(a, smem);
+}
+
 /* One warp per stream: scan of its segment records (pending literals, continued matches, output offsets, compressed
  * size); the warp that finishes the last stream runs the block scan, exactly as in encode_kernel. */
 #define FSCAN_WARPS 4
+DEV void zenc_body(const FastArgs& a, ZeSm* S);
 __global__ void __launch_bounds__(FSCAN_WARPS * 32) fscan_kernel(FastArgs a) {
+#ifdef SIMT_EMU
+  if (a.zstd) {                                    /* the emulator launches the zstd entropy stage under this name */
+    __shared__ ZeSm ztab[FSCAN_WARPS];
+    zenc_body(a, &ztab[threadIdx.x >> 5]);
+    return;
+  }
+#endif
   const int lane = lane_id();
   const int nfs = a.map.nfull * a.map.nsplits;
   int mine = 0;
@@ -337,6 +368,48 @@ __global__ void __launch_bounds__(FSCAN_WARPS * 32) fscan_kernel(FastArgs a) {
   if (a.fold_scan) warp_scan_blocks(a.scan);
   __syncwarp();
   if (lane == 0) *a.done = 0;
+}
+
+
+/* ---- segment-parallel zstd (dev_zstdenc.cuh): index_kernel, zparse_kernel, then one warp per frame ---- */
+DEV void zenc_body(const FastArgs& a, ZeSm* S) {
+  const int lane = lane_id(), warp = (int)(threadIdx.x >> 5), nwarps = (int)(blockDim.x >> 5);
+  int mine = 0;
+  for (int idx = (int)blockIdx.x * nwarps + warp; idx < a.map.nstreams; idx += (int)gridDim.x * nwarps) {
+    int block, len, split;
+    long long off;
+    stream_locate(a.map, idx, &block, &off, &len, &split);
+    const long long gseg = (long long)idx * a.segs_full;
+    int c = 0;
+    if (lane == 0)
+      c = zse_frame_serial(*S, a.in + off, len, a.recs + gseg * ZE_SEG_RECS, a.nrec + gseg, (u8*)(a.prev + off), a.slots + off);
+    c = __shfl_sync(FULLMASK, c, 0);
+    if (c >= len) c = len;                         /* blosc.c:705-714: incompressible split is stored raw */
+    if (lane == 0) { a.csizes[idx] = c; a.needs[idx] = c; }
+    mine++;
+    __syncwarp();
+  }
+  /* whoever completes the stream count does the block scan, exactly as in encode_kernel */
+  if (mine == 0) return;
+  __threadfence();
+  int last = 0;
+  if (lane == 0) last = atomicAdd(a.done, mine) + mine == a.map.nstreams;
+  last = __shfl_sync(FULLMASK, last, 0);
+  if (!last) return;
+  __threadfence();
+  if (a.fold_scan) warp_scan_blocks(a.scan);
+  __syncwarp();
+  if (lane == 0) *a.done = 0;
+}
+
+/* One warp per stream: its frame, lane 0 codes it; the tables live in the warp's ZE_SMEM_BYTES of shared memory */
+__global__ void __launch_bounds__(ZE_WARPS * 32) zenc_kernel(FastArgs a) {
+#ifdef SIMT_EMU
+  u8* smem = simt::g_dynsmem;
+#else
+  extern __shared__ __align__(16) u8 smem[];
+#endif
+  zenc_body(a, (ZeSm*)(smem + (size_t)(threadIdx.x >> 5) * ZE_SMEM_BYTES));
 }
 
 

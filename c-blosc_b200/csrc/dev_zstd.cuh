@@ -4,7 +4,8 @@
  * SURVEY.md section 8 row (f4): chunks written with Blosc's "zstd" codec hold one zstd frame
  * per block (never split, reference blosc/blosc.c:929-934; zstd_wrap_decompress ->
  * ZSTD_decompress(), :517-529).  Decode-only companion of dev_inflate.cuh so that such chunks
- * (3 of the compat .cdata goldens) decode on the GPU; the encoder side stays out of scope.
+ * (3 of the compat .cdata goldens) decode on the GPU.  The encoder is dev_zstdenc.cuh, which shares the
+ * code tables and predefined distributions below.
  *
  * The format is entropy coded with backward bitstreams (Huffman literals, FSE sequences), which
  * is serial work: one lane of the warp walks the frame while the chunk's other frames run in

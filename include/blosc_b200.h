@@ -18,6 +18,10 @@
  *     bytes are not LZ4_compress_HC's; other compressors report -5 exactly like a reference built
  *     with -DDEACTIVATE_ZLIB/ZSTD/SNAPPY (blosc.c:573,1197-1208).  Decoding is wider: zlib and
  *     zstd chunks decode too (serial GPU decoders, one lane per stream); snappy chunks report -5;
+ *   - with the environment variable BLOSC_B200_ZSTD=1 (read on every call) the library behaves
+ *     like a reference built with zstd: "zstd" is listed, named and encoded (segment-parallel GPU
+ *     encoder, one zstd frame per block).  The header is the reference's and every reference build
+ *     with zstd decodes the chunks, but the frames are not ZSTD_compress's bytes;
  *   - there is no CPU codec: without a CUDA device every compress/decompress call
  *     prints a message on stderr and returns -1.
  */

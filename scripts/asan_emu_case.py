@@ -25,4 +25,16 @@ for parse in ("exact","fast"):
                     c=chunk.copy(); pos=rng.integers(16,r,3); c[pos]=rng.integers(0,256,3,dtype=np.uint8)
                     emu.blosc_decompress_ctx(c.ctypes.data_as(C.c_void_p),out.ctypes.data_as(C.c_void_p),C.c_size_t(n),C.c_int(1))
                 cases+=1
+os.environ.pop('BLOSC_B200_PARSE', None)
+os.environ['BLOSC_B200_ZSTD']='1'          # the zstd encoder: several zstd blocks per frame (forced blocksize), raw streams
+for kind in ("bench","text","lowent","mixed","zeros","rand"):
+    for n in (13, 1000, 70001, 300001):
+        src=gen(kind,n)
+        for ts,shuf,cl,bs in ((4,1,5,0),(1,0,9,0),(8,2,1,0),(3,1,5,200000)):
+            dest=np.full(n+16,0xAA,np.uint8)
+            r=emu.blosc_compress_ctx(C.c_int(cl),C.c_int(shuf),C.c_size_t(ts),C.c_size_t(n),src.ctypes.data_as(C.c_void_p),dest.ctypes.data_as(C.c_void_p),C.c_size_t(n+16),b"zstd",C.c_size_t(bs),C.c_int(1))
+            assert r>0
+            chunk=dest[:r].copy(); out=np.zeros(n,np.uint8)
+            assert emu.blosc_decompress_ctx(chunk.ctypes.data_as(C.c_void_p),out.ctypes.data_as(C.c_void_p),C.c_size_t(n),C.c_int(1))==n and (out==src).all()
+            cases+=1
 print("asan workload ok, cases", cases)
