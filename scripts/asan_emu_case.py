@@ -37,4 +37,14 @@ for kind in ("bench","text","lowent","mixed","zeros","rand"):
             chunk=dest[:r].copy(); out=np.zeros(n,np.uint8)
             assert emu.blosc_decompress_ctx(chunk.ctypes.data_as(C.c_void_p),out.ctypes.data_as(C.c_void_p),C.c_size_t(n),C.c_int(1))==n and (out==src).all()
             cases+=1
+os.environ.pop('BLOSC_B200_ZSTD', None)
+# the zstd entropy stage on chosen sequence records (emu_zstd_frame): the records-driven scenarios of
+# tests/test_zstd_encode_edges.py, each frame decoded by zstd_frame.py and by this library's decoder
+import test_zstd_encode_edges as edges
+emu.emu_zstd_frame.restype=C.c_int; emu.emu_zstd_frame.argtypes=[C.c_void_p,C.c_int,C.c_void_p,C.c_void_p,C.c_void_p]
+emu.emu_zstd_decode.restype=C.c_int; emu.emu_zstd_decode.argtypes=[C.c_void_p,C.c_int,C.c_void_p,C.c_int]
+for sc in edges.SCENARIOS:
+    for name,p in sc().items():
+        edges.encode_and_check(emu,None,p)
+        cases+=1
 print("asan workload ok, cases", cases)

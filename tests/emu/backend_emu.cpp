@@ -259,4 +259,22 @@ int emu_zstd_decode(const unsigned char* src, int csize, unsigned char* dst, int
   return result;
 }
 
+/* the zstd entropy stage alone (zse_frame_serial), driven by sequence records the caller chose in zse_parse_lane's
+ * format: rec[k * ZE_SEG_RECS + r] for segment k, cnt[k] records each.  Scratch of 2n (+8) bytes as in zenc_body
+ * (the stream's part of prev[]), out n bytes.  Returns the frame size, or n for "stored". */
+int emu_zstd_frame(const unsigned char* src, int n, const unsigned int* rec, const unsigned int* cnt, unsigned char* out) {
+  int result = 0;
+  ZeSm* S = new ZeSm;
+  unsigned char* scratch = (unsigned char*)malloc(2 * (size_t)n + 8);
+  simt::launch(simt::Dim3(1), simt::Dim3(32), 0, [&] {
+    int r = 0;
+    if ((threadIdx.x & 31) == 0) r = zse_frame_serial(*S, src, n, rec, cnt, scratch, out);
+    r = __shfl_sync(FULLMASK, r, 0);
+    if ((threadIdx.x & 31) == 11) result = r;
+  });
+  free(scratch);
+  delete S;
+  return result;
+}
+
 }  // extern "C"
