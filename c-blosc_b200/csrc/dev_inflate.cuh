@@ -12,10 +12,18 @@
  * stored blocks and the Adler-32 check.  Accept / reject rules follow zlib's inflate():
  * bad header, reserved block type, stored-length mismatch, over-subscribed or incomplete code
  * sets (a single 1-bit code is allowed), missing end-of-block code, distances before the start
- * of the output, output overrun and a wrong Adler-32 all fail.
+ * of the output, output overrun and a wrong Adler-32 all fail.  tests/test_zlib_decode_edges.py
+ * reaches every reject site on hand-written streams and holds each verdict to Python's zlib.
  */
 #pragma once
 #include "dev_common.cuh"
+
+#ifdef SIMT_EMU
+static int g_inf_fail_line = 0;              /* emulator builds remember the first check that rejected the stream */
+#define INF_FAIL (g_inf_fail_line = g_inf_fail_line ? g_inf_fail_line : __LINE__, -1)
+#else
+#define INF_FAIL (-1)
+#endif
 
 #define INF_MAXBITS 15
 #define INF_MAXLCODES 286
@@ -108,21 +116,21 @@ DEV int inf_deflate_serial(InfState& z, u16* sm) {
   do {
     last = (int)inf_bits(z, 1);
     const int type = (int)inf_bits(z, 2);
-    if (z.bad) return -1;
+    if (z.bad) return INF_FAIL;                              /* no block header */
     if (type == 0) {                                         /* stored */
       z.ip -= z.bitcnt >> 3;                                 /* RFC 1951 3.2.4: skip to a byte boundary -- whole bytes that were */
       z.bitbuf = 0; z.bitcnt = 0;                            /* fetched ahead go back, the rest of the current byte is dropped */
-      if (z.ip + 4 > z.iend) return -1;
+      if (z.ip + 4 > z.iend) return INF_FAIL;
       const u32 len = (u32)z.in[z.ip] | ((u32)z.in[z.ip + 1] << 8);
       const u32 nlen = (u32)z.in[z.ip + 2] | ((u32)z.in[z.ip + 3] << 8);
       z.ip += 4;
-      if (len != (~nlen & 0xffffu)) return -1;
-      if (z.ip + (int)len > z.iend || z.op + (int)len > z.oend) return -1;
+      if (len != (~nlen & 0xffffu)) return INF_FAIL;
+      if (z.ip + (int)len > z.iend || z.op + (int)len > z.oend) return INF_FAIL;
       for (u32 k = 0; k < len; k++) z.out[z.op + k] = z.in[z.ip + k];
       z.ip += (int)len; z.op += (int)len;
       continue;
     }
-    if (type == 3) return -1;
+    if (type == 3) return INF_FAIL;
     if (type == 1) {                                         /* fixed codes, RFC 1951 3.2.6 */
       int s = 0;
       for (; s < 144; s++) lengths[s] = 8;
@@ -134,52 +142,52 @@ DEV int inf_deflate_serial(InfState& z, u16* sm) {
       inf_construct(dcount, dsym, lengths, INF_MAXDCODES);
     } else {                                                 /* dynamic codes, RFC 1951 3.2.7 */
       const int nlen = (int)inf_bits(z, 5) + 257, ndist = (int)inf_bits(z, 5) + 1, ncode = (int)inf_bits(z, 4) + 4;
-      if (z.bad || nlen > INF_MAXLCODES || ndist > INF_MAXDCODES) return -1;
+      if (z.bad || nlen > INF_MAXLCODES || ndist > INF_MAXDCODES) return INF_FAIL;
       int idx = 0;
       for (; idx < ncode; idx++) lengths[k_inf_order[idx]] = (u16)inf_bits(z, 3);
       for (; idx < 19; idx++) lengths[k_inf_order[idx]] = 0;
-      if (z.bad) return -1;
-      if (inf_construct(lcount, lsym, lengths, 19) != 0) return -1;   /* the code-length code must be complete */
+      if (z.bad) return INF_FAIL;                            /* code-length code cut */
+      if (inf_construct(lcount, lsym, lengths, 19) != 0) return INF_FAIL;   /* the code-length code must be complete */
       idx = 0;
       while (idx < nlen + ndist) {
         int sym = inf_decode(z, lcount, lsym);
-        if (sym < 0) return -1;
+        if (sym < 0) return INF_FAIL;                        /* not a code-length code */
         if (sym < 16) lengths[idx++] = (u16)sym;
         else {
           int rep, val = 0;
           if (sym == 16) {
-            if (idx == 0) return -1;                         /* nothing to repeat */
+            if (idx == 0) return INF_FAIL;                         /* nothing to repeat */
             val = lengths[idx - 1];
             rep = 3 + (int)inf_bits(z, 2);
           } else if (sym == 17) rep = 3 + (int)inf_bits(z, 3);
           else rep = 11 + (int)inf_bits(z, 7);
-          if (z.bad || idx + rep > nlen + ndist) return -1;
+          if (z.bad || idx + rep > nlen + ndist) return INF_FAIL;
           while (rep--) lengths[idx++] = (u16)val;
         }
       }
-      if (lengths[256] == 0) return -1;                      /* no end-of-block code */
+      if (lengths[256] == 0) return INF_FAIL;                      /* no end-of-block code */
       /* the distance lengths follow the literal/length ones; build dist first, it reads its slice */
       int err = inf_construct(dcount, dsym, lengths + nlen, ndist);
-      if (err && (err < 0 || ndist != dcount[0] + dcount[1])) return -1;
+      if (err && (err < 0 || ndist != dcount[0] + dcount[1])) return INF_FAIL;
       err = inf_construct(lcount, lsym, lengths, nlen);
-      if (err && (err < 0 || nlen != lcount[0] + lcount[1])) return -1;
+      if (err && (err < 0 || nlen != lcount[0] + lcount[1])) return INF_FAIL;
     }
     for (;;) {                                               /* the block's symbols */
       int sym = inf_decode(z, lcount, lsym);
-      if (sym < 0) return -1;
+      if (sym < 0) return INF_FAIL;                          /* not a literal/length code */
       if (sym < 256) {
-        if (z.op >= z.oend) return -1;
+        if (z.op >= z.oend) return INF_FAIL;
         z.out[z.op++] = (u8)sym;
         continue;
       }
       if (sym == 256) break;
       sym -= 257;
-      if (sym >= 29) return -1;
+      if (sym >= 29) return INF_FAIL;
       const int len = k_inf_lens[sym] + (int)inf_bits(z, k_inf_lext[sym]);
       const int ds = inf_decode(z, dcount, dsym);
-      if (ds < 0 || ds >= 30) return -1;
+      if (ds < 0 || ds >= 30) return INF_FAIL;
       const int dist = k_inf_dists[ds] + (int)inf_bits(z, k_inf_dext[ds]);
-      if (z.bad || dist > z.op || z.op + len > z.oend) return -1;
+      if (z.bad || dist > z.op || z.op + len > z.oend) return INF_FAIL;
       for (int k = 0; k < len; k++) z.out[z.op + k] = z.out[z.op + k - dist];
       z.op += len;
     }
@@ -195,20 +203,22 @@ DEV int zlib_decode_warp(const u8* __restrict__ in, const int csize, u8* out, co
   int n = -1, endpos = 0;
   if (lane == 0) {
     do {
-      if (csize < 2 + 4) break;                              /* header + Adler-32 at least */
+      if (csize < 2 + 4) { n = INF_FAIL; break; }            /* header + Adler-32 at least */
       const u32 cmf = in[0], flg = in[1];
-      if ((cmf & 15u) != 8u || (cmf >> 4) > 7u || ((cmf << 8) | flg) % 31u != 0u || (flg & 0x20u)) break;   /* RFC 1950 2.2; no preset dictionary */
+      if ((cmf & 15u) != 8u || (cmf >> 4) > 7u) { n = INF_FAIL; break; }                    /* RFC 1950 2.2: deflate, window <= 32 KiB */
+      if (((cmf << 8) | flg) % 31u != 0u) { n = INF_FAIL; break; }                         /* FCHECK */
+      if (flg & 0x20u) { n = INF_FAIL; break; }                                            /* FDICT: no preset dictionary */
       InfState z;
       z.in = in; z.ip = 2; z.iend = csize; z.bitbuf = 0; z.bitcnt = 0; z.out = out; z.op = 0; z.oend = cap; z.bad = false;
       n = inf_deflate_serial(z, (u16*)smem);
-      if (z.bad) n = -1;
+      if (z.bad) n = INF_FAIL;                               /* the input ended inside the last symbol */
       endpos = z.ip - (z.bitcnt >> 3);                       /* whole unread bytes go back: the trailer is byte aligned */
     } while (0);
   }
   n = __shfl_sync(FULLMASK, n, 0);
   endpos = __shfl_sync(FULLMASK, endpos, 0);
-  if (n < 0) return -1;
-  if (endpos + 4 > csize) return -1;
+  if (n < 0) return -1;                                      /* refused above, where the line was recorded */
+  if (endpos + 4 > csize) return INF_FAIL;
   __syncwarp();
   /* Adler-32 of the output by the whole warp: lane l sums a contiguous slice (a = 1 + sum of bytes,
    * b = sum of the running a), slices are combined with b_total = sum(b_i + len_after_i * (a_i - ...)) */
@@ -233,6 +243,6 @@ DEV int zlib_decode_warp(const u8* __restrict__ in, const int csize, u8* out, co
   for (int d = 16; d >= 1; d >>= 1) tb = (tb + __shfl_xor_sync(FULLMASK, tb, d)) % 65521u;
   const u32 ta = (__shfl_sync(FULLMASK, pa, 31) + 1u) % 65521u;
   const u32 want = ((u32)in[endpos] << 24) | ((u32)in[endpos + 1] << 16) | ((u32)in[endpos + 2] << 8) | (u32)in[endpos + 3];
-  if (((tb << 16) | ta) != want) return -1;
+  if (((tb << 16) | ta) != want) return INF_FAIL;
   return n;
 }

@@ -13,16 +13,22 @@
  * per-block literal buffer is needed; the tables live in the warp's shared-memory scratch.
  * Everything zstd's own decoder checks on the way is checked here as well: magic, reserved
  * bits, sizes against the input, table descriptions, offsets beyond the decoded data, exact
- * consumption of every bitstream, declared content size and the optional XXH64 checksum.
- * (On damaged input this is slightly stricter than zstd 1.5.6, whose fast Huffman loops do not
- * verify that a literal stream is used up exactly and then emit garbage; such frames fail here.)
+ * consumption of every bitstream, declared content size and the optional XXH64 checksum.  Like
+ * ZSTD_decompress, the input may hold several frames and skippable frames one after the other, and
+ * a compressed block and its literals are limited by min(window size, 128 KiB).
+ *
+ * Verdict rule: never accept a frame that zstd 1.5.6's ZSTD_decompress rejects, never reject an
+ * RFC 8878-valid frame that it accepts.  RFC-invalid frames that it accepts are refused here only for
+ * the STRICT list of tests/test_zstd_decode_edges.py (each entry pinned by a test): Huffman codes of
+ * 12 bits, raw / RLE blocks above 128 KiB, a compressed block that decodes to more than 128 KiB, and
+ * a literal stream with bits left over (zstd's fast Huffman loops do not check it).
  */
 #pragma once
 #include "dev_common.cuh"
 
 #ifdef SIMT_EMU
-static int g_zs_fail_line = 0;               /* emulator builds remember which check rejected the frame */
-#define ZS_FAIL (g_zs_fail_line = __LINE__, -1)
+static int g_zs_fail_line = 0;               /* emulator builds remember the first check that rejected the frame */
+#define ZS_FAIL (g_zs_fail_line = g_zs_fail_line ? g_zs_fail_line : __LINE__, -1)
 #else
 #define ZS_FAIL (-1)
 #endif
@@ -97,7 +103,7 @@ DEV void zs_fse_build(ZsFse* t, const short* norm, int nsym, int log, u16* next)
 
 /* FSE table description (RFC 8878 4.1.1): fills norm[0, *nsym) and *log; returns bytes used or -1 */
 DEV int zs_fse_header(const u8* p, int len, short* norm, int maxsym, int maxlog, int* nsym, int* log) {
-  if (len < 1) return ZS_FAIL;
+  if (len < 1) return ZS_FAIL;                                   /* no description */
   const int total = len * 8;
   int pos = 0;
   const int alog = 5 + (int)zs_bits_at(p, pos, 4);
@@ -164,7 +170,7 @@ DEV bool zs_lit_take(ZsLit& L, const u16* huf, u8* dst, int n) {
 DEV int zs_huf_table(const u8* p, int len, u8* sm, int* hlog) {
   u16* huf = (u16*)(sm + ZS_OFF_HUF);
   u8* w = sm + ZS_OFF_WEIGHT;
-  if (len < 1) return ZS_FAIL;
+  if (len < 1) return ZS_FAIL;                                   /* no tree description */
   const int hb = p[0];
   int n, used;
   if (hb >= 128) {                                           /* 4-bit weights */
@@ -187,11 +193,11 @@ DEV int zs_huf_table(const u8* p, int len, u8* sm, int* hlog) {
     if (b.pos < 0) return ZS_FAIL;
     n = 0;
     for (;;) {                                               /* at most 255 explicit weights */
-      if (n >= 254) return ZS_FAIL;
+      if (n >= 254) return ZS_FAIL;                          /* first state */
       w[n++] = t[s1].sym;
       s1 = t[s1].base + zs_back_read(b, t[s1].nbits);
       if (b.pos < 0) { w[n++] = t[s2].sym; break; }
-      if (n >= 254) return ZS_FAIL;
+      if (n >= 254) return ZS_FAIL;                          /* second state */
       w[n++] = t[s2].sym;
       s2 = t[s2].base + zs_back_read(b, t[s2].nbits);
       if (b.pos < 0) { w[n++] = t[s1].sym; break; }
@@ -275,17 +281,20 @@ DEV u64 zs_xxh64(const u8* p, int len) {                    /* XXH64, seed 0 */
   return h;
 }
 
-/* Runs on ONE lane: one frame, which must use up the whole input.  Returns bytes written or -1. */
-DEV int zs_frame_serial(const u8* in, int csize, u8* out, int cap, u8* sm) {
+/* Runs on ONE lane: the frame at the start of in[0, csize).  Returns bytes written or -1, and the frame's size in *used. */
+DEV int zs_frame_one(const u8* in, int csize, u8* out, int cap, u8* sm, int* used) {
   if (csize < 6) return ZS_FAIL;
   if (((u32)in[0] | ((u32)in[1] << 8) | ((u32)in[2] << 16) | ((u32)in[3] << 24)) != 0xFD2FB528u) return ZS_FAIL;
   const int fhd = in[4];
   const int fcs_flag = fhd >> 6, single = (fhd >> 5) & 1, checksum = (fhd >> 2) & 1, did_flag = fhd & 3;
   if (fhd & 0x08) return ZS_FAIL;                                 /* reserved bit */
   int ip = 5;
+  u32 window = ZS_BLOCKMAX;                                       /* min(window size, ZS_BLOCKMAX) */
   if (!single) {
     if (ip >= csize) return ZS_FAIL;
     if ((in[ip] >> 3) > 21) return ZS_FAIL;                       /* window above 2 GiB: more than ZSTD_decompress accepts (31 bits) */
+    const int wexp = (in[ip] >> 3) + 10;
+    if (wexp < 17) window = (1u << wexp) + ((1u << wexp) >> 3) * (in[ip] & 7u);   /* from 2^17 on, no block is limited by it */
     ip++;
   }
   const int did_bytes = did_flag == 3 ? 4 : did_flag;
@@ -299,6 +308,10 @@ DEV int zs_frame_serial(const u8* in, int csize, u8* out, int cap, u8* sm) {
   if (fcs_bytes == 2) fcs += 256;
   ip += fcs_bytes;
   if (fcs_bytes && fcs > (u64)cap) return ZS_FAIL;
+  if (single && fcs < (u64)window) window = (u32)fcs;             /* a single-segment frame's window is its content size */
+  /* RFC 8878 Block_Maximum_Size: a compressed block and its literals stay within min(window, 128 KiB), as in
+   * ZSTD_decompress.  Raw and RLE block sizes and a compressed block's output are held to 128 KiB only. */
+  const int bmax = (int)window;
 
   u16* huf = (u16*)(sm + ZS_OFF_HUF);
   ZsFse* tll = (ZsFse*)(sm + ZS_OFF_LL);
@@ -328,7 +341,7 @@ DEV int zs_frame_serial(const u8* in, int csize, u8* out, int cap, u8* sm) {
       op += bsize;
       continue;
     }
-    if (bsize > ZS_BLOCKMAX || bsize < 2 || ip + bsize > csize) return ZS_FAIL;   /* compressed block */
+    if (bsize > bmax || bsize < 2 || ip + bsize > csize) return ZS_FAIL;   /* compressed block */
     const u8* b = in + ip;
     const int bend = bsize;
     ip += bsize;
@@ -349,7 +362,7 @@ DEV int zs_frame_serial(const u8* in, int csize, u8* out, int cap, u8* sm) {
         else if (sf == 2) { hdr = 4; const u32 v = (u32)b[0] | ((u32)b[1] << 8) | ((u32)b[2] << 16) | ((u32)b[3] << 24); regen = (int)((v >> 4) & 0x3fffu); comp = (int)(v >> 18); }
         else { hdr = 5; const u64 v = (u64)b[0] | ((u64)b[1] << 8) | ((u64)b[2] << 16) | ((u64)b[3] << 24) | ((u64)b[4] << 32); regen = (int)((v >> 4) & 0x3ffffu); comp = (int)(v >> 22); }
       }
-      if (regen > ZS_BLOCKMAX) return ZS_FAIL;
+      if (regen > bmax) return ZS_FAIL;
       L.left = regen; L.cur = 0;
       if (ltype == 0) { if (hdr + regen > bend) return ZS_FAIL; L.type = 0; L.raw = b + hdr; lp = hdr + regen; }
       else if (ltype == 1) { if (hdr + 1 > bend) return ZS_FAIL; L.type = 1; L.raw = b + hdr; lp = hdr + 1; }
@@ -384,24 +397,24 @@ DEV int zs_frame_serial(const u8* in, int csize, u8* out, int cap, u8* sm) {
       }
     }
     /* ---- sequences section ---- */
-    if (lp >= bend) return ZS_FAIL;
+    if (lp >= bend) return ZS_FAIL;                          /* no sequence count */
     int nseq = b[lp++];
     if (nseq >= 128) {
       if (nseq == 255) { if (lp + 2 > bend) return ZS_FAIL; nseq = (b[lp] | (b[lp + 1] << 8)) + 0x7F00; lp += 2; }
       else { if (lp + 1 > bend) return ZS_FAIL; nseq = ((nseq - 128) << 8) + b[lp++]; }
     }
     if (nseq > 0) {
-      if (lp >= bend) return ZS_FAIL;
+      if (lp >= bend) return ZS_FAIL;                        /* no modes byte */
       const int modes = b[lp++];
       if (modes & 3) return ZS_FAIL;
       int u = zs_seq_table(modes >> 6, b + lp, bend - lp, tll, &ll_log, &have_ll, k_zs_ll_norm, 36, 6, 35, 9, sm);
-      if (u < 0) return ZS_FAIL;
+      if (u < 0) return ZS_FAIL;                             /* LL table */
       lp += u;
       u = zs_seq_table((modes >> 4) & 3, b + lp, bend - lp, tof, &of_log, &have_of, k_zs_of_norm, 29, 5, 31, 8, sm);
-      if (u < 0) return ZS_FAIL;
+      if (u < 0) return ZS_FAIL;                             /* OF table */
       lp += u;
       u = zs_seq_table((modes >> 2) & 3, b + lp, bend - lp, tml, &ml_log, &have_ml, k_zs_ml_norm, 53, 6, 52, 9, sm);
-      if (u < 0) return ZS_FAIL;
+      if (u < 0) return ZS_FAIL;                             /* ML table */
       lp += u;
       ZsBack sb;
       if (!zs_back_init(sb, b + lp, bend - lp)) return ZS_FAIL;
@@ -456,7 +469,31 @@ DEV int zs_frame_serial(const u8* in, int csize, u8* out, int cap, u8* sm) {
     if ((u32)zs_xxh64(out, op) != want) return ZS_FAIL;
     ip += 4;
   }
-  if (ip != csize) return ZS_FAIL;
+  *used = ip;
+  return op;
+}
+
+/* Runs on ONE lane: frames and skippable frames until the input is used up, as ZSTD_decompress does
+ * (ZSTD_decompressMultiFrame).  Each frame starts with fresh tables and repeat offsets, its content size is held
+ * to the room left and its checksum covers its own output.  Returns bytes written or -1; an input of skippable
+ * frames only gives 0. */
+DEV int zs_frame_serial(const u8* in, int csize, u8* out, int cap, u8* sm) {
+  int ip = 0, op = 0;
+  while (ip < csize) {
+    if (csize - ip < 5) return ZS_FAIL;                          /* 1 to 4 bytes after the last frame */
+    const u32 magic = (u32)in[ip] | ((u32)in[ip + 1] << 8) | ((u32)in[ip + 2] << 16) | ((u32)in[ip + 3] << 24);
+    if ((magic & 0xFFFFFFF0u) == 0x184D2A50u) {                  /* skippable frame: 4-byte size, then that many bytes */
+      if (csize - ip < 8) return ZS_FAIL;
+      const u32 fsz = (u32)in[ip + 4] | ((u32)in[ip + 5] << 8) | ((u32)in[ip + 6] << 16) | ((u32)in[ip + 7] << 24);
+      if (fsz > (u32)(csize - ip - 8)) return ZS_FAIL;
+      ip += 8 + (int)fsz;
+      continue;
+    }
+    int used = 0;
+    const int n = zs_frame_one(in + ip, csize - ip, out + op, cap - op, sm, &used);
+    if (n < 0) return -1;
+    ip += used; op += n;
+  }
   return op;
 }
 

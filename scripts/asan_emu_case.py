@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """Workload for the AddressSanitizer build of the emulated library (make -C tests/emu asan):
   LD_PRELOAD=$(gcc -print-file-name=libasan.so) ASAN_OPTIONS=detect_leaks=0 python scripts/asan_emu_case.py
-exact / fast / lz4hc / BloscLZ paths, exact-size buffers, damaged chunks."""
+exact / fast / lz4hc / BloscLZ paths, exact-size buffers, damaged chunks, crafted and damaged zstd frames and zlib streams."""
 import os, sys, ctypes as C, numpy as np
 sys.path.insert(0, os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), 'tests'))
 from datagen import gen, compress, decompress
@@ -47,4 +47,32 @@ for sc in edges.SCENARIOS:
     for name,p in sc().items():
         edges.encode_and_check(emu,None,p)
         cases+=1
+# the zstd decoder on crafted frames (tests/test_zstd_decode_edges.py): accepted, rejected, STRICT and damaged frames,
+# each in an input buffer of exactly its size, so that a read past the input shows; then the same frames as chunks
+import test_zstd_decode_edges as zedges
+frames=[(f,len(c)) for f,c,_ in zedges.ACCEPT.values()]+[(f,cap) for f,cap,_ in zedges.REJECT.values()]
+frames+=[(fc[0],len(fc[1])+16) for fc,_ in zedges.strict_frames().values()]+list(zedges._damage_corpus())
+for f,cap in frames:
+    src=np.frombuffer(f,np.uint8).copy(); out=np.zeros(max(cap,1),np.uint8)
+    emu.emu_zstd_decode(src.ctypes.data_as(C.c_void_p),C.c_int(len(f)),out.ctypes.data_as(C.c_void_p),C.c_int(cap))
+    cases+=1
+for name,ch,n,_ in zedges.chunk_corpus(damaged=True):
+    c=np.frombuffer(ch,np.uint8).copy(); out=np.zeros(n,np.uint8)
+    emu.blosc_decompress_ctx(c.ctypes.data_as(C.c_void_p),out.ctypes.data_as(C.c_void_p),C.c_size_t(n),C.c_int(1))
+    emu.blosc_getitem(c.ctypes.data_as(C.c_void_p),C.c_int(0),C.c_int(n),out.ctypes.data_as(C.c_void_p))
+    cases+=1
+# the inflate decoder on crafted streams (tests/test_zlib_decode_edges.py): accepted, rejected, Adler-32 sizes and
+# damaged streams, each in an input buffer of exactly its size; then the same streams as chunks
+import test_zlib_decode_edges as iedges
+emu.emu_zlib_decode.restype=C.c_int; emu.emu_zlib_decode.argtypes=[C.c_void_p,C.c_int,C.c_void_p,C.c_int]
+streams=[(st,len(iedges.zlib_verdict(st,1<<20))) for st in iedges.ACCEPT.values()]+[(st,cap) for st,cap,_ in iedges.REJECT.values()]
+streams+=[(st,len(d)) for _,st,d in iedges.adler_streams()]+list(iedges._damage_corpus())
+for st,cap in streams:
+    src=np.frombuffer(st,np.uint8).copy(); out=np.zeros(max(cap,1),np.uint8)
+    emu.emu_zlib_decode(src.ctypes.data_as(C.c_void_p),C.c_int(len(st)),out.ctypes.data_as(C.c_void_p),C.c_int(cap))
+    cases+=1
+for name,ch,n in iedges.chunk_corpus():
+    c=np.frombuffer(ch,np.uint8).copy(); out=np.zeros(n,np.uint8)
+    emu.blosc_decompress_ctx(c.ctypes.data_as(C.c_void_p),out.ctypes.data_as(C.c_void_p),C.c_size_t(n),C.c_int(1))
+    cases+=1
 print("asan workload ok, cases", cases)

@@ -240,8 +240,10 @@ int emu_blz_decode(const unsigned char* src, int csize, unsigned char* dst, int 
   return result;
 }
 
+int emu_zlib_fail_line(void) { return g_inf_fail_line; }
 int emu_zlib_decode(const unsigned char* src, int csize, unsigned char* dst, int cap) {
   int result = 0;
+  g_inf_fail_line = 0;
   simt::launch(simt::Dim3(1), simt::Dim3(32), INF_SMEM_BYTES, [&] {
     int r = zlib_decode_warp(src, csize, dst, cap, simt::g_dynsmem);
     if ((threadIdx.x & 31) == 17) result = r;
@@ -252,6 +254,7 @@ int emu_zlib_decode(const unsigned char* src, int csize, unsigned char* dst, int
 int emu_zstd_fail_line(void) { return g_zs_fail_line; }
 int emu_zstd_decode(const unsigned char* src, int csize, unsigned char* dst, int cap) {
   int result = 0;
+  g_zs_fail_line = 0;
   simt::launch(simt::Dim3(1), simt::Dim3(32), ZS_SMEM_BYTES, [&] {
     int r = zstd_decode_warp(src, csize, dst, cap, simt::g_dynsmem);
     if ((threadIdx.x & 31) == 9) result = r;

@@ -5,7 +5,10 @@ internal-complibs/ and absent from this repository), so parity is pinned on (1) 
 own golden chunks compat/blosc-*-zstd*.cdata and (2) frames written and judged by that very
 library (oracle/_ref is built with it): all levels, raw / RLE / compressed blocks, Huffman and
 FSE table modes, multi-block frames with repeat modes, checksums; damaged frames must get
-ZSTD_decompress()'s accept/reject verdict.  CPU: the device code inside the SIMT emulator."""
+ZSTD_decompress()'s accept/reject verdict.  CPU: the device code inside the SIMT emulator.
+
+The verdict rule and its STRICT exceptions (frames the RFC forbids but ZSTD_decompress accepts, refused here) are
+stated in tests/test_zstd_decode_edges.py, which tests the decoder branch by branch on frames written to order."""
 import ctypes as C
 import glob
 import os

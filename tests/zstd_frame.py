@@ -6,9 +6,11 @@ mistake shared by the library's encoder and decoder (which share dev_zstd.cuh's 
 than ZSTD_decompress where the RFC allows it: every Huffman and sequence bitstream must be used up exactly, FSE
 descriptions must sum exactly to 2^log within the RFC's accuracy limits, Huffman weights must give a complete tree,
 no block may produce more than 128 KiB, and the content size must equal the bytes produced, with nothing after the
-last block.  Checksums, dictionaries and skippable frames are not produced by the encoder and are rejected.
+last block.  A content checksum is verified with XXH64; a dictionary-ID field must be zero (no dictionary).
 
-decode_frame(data) -> (bytes, FrameInfo).  FrameInfo.blocks holds one dict per block:
+decode_frame(data) -> (bytes, FrameInfo) for one frame that fills `data`.  decode_stream(data) -> (bytes, [FrameInfo])
+decodes frames and skippable frames one after the other until `data` is used up, as ZSTD_decompress does.
+FrameInfo.blocks holds one dict per block:
   {"type": "raw" | "rle" | "compressed", "size": bytes in the frame, "last": bool, "out": bytes produced,
    "lit": {...}, "seq": {...}}   (lit / seq for compressed blocks only)
 lit: {"type": "raw" | "rle" | "compressed" | "treeless", "size_format": 0..3, "streams": 1 | 4, "regen": int,
@@ -43,6 +45,60 @@ MAX_SYM = {"ll": 35, "of": 31, "ml": 52}
 MODES = ("predefined", "rle", "fse", "repeat")
 
 
+M64 = (1 << 64) - 1
+
+
+# ---------------------------------------------------------------------------------------------------------------
+# XXH64 (seed 0 by default), for content checksums
+# ---------------------------------------------------------------------------------------------------------------
+_P1, _P2, _P3, _P4, _P5 = (11400714785074694791, 14029467366897019727, 1609587929392839161, 9650029242287828579,
+                           2870177450012600261)
+
+
+def _rotl(x, r):
+    return ((x << r) | (x >> (64 - r))) & M64
+
+
+def _round(acc, lane):
+    return (_rotl((acc + lane * _P2) & M64, 31) * _P1) & M64
+
+
+def xxh64(data, seed=0):
+    data = bytes(data)
+    n, p = len(data), 0
+    if n >= 32:
+        v = [(seed + _P1 + _P2) & M64, (seed + _P2) & M64, seed, (seed - _P1) & M64]
+        while p + 32 <= n:
+            for i in range(4):
+                v[i] = _round(v[i], int.from_bytes(data[p:p + 8], "little"))
+                p += 8
+        h = (_rotl(v[0], 1) + _rotl(v[1], 7) + _rotl(v[2], 12) + _rotl(v[3], 18)) & M64
+        for i in range(4):
+            h = ((h ^ _round(0, v[i])) * _P1 + _P4) & M64
+    else:
+        h = (seed + _P5) & M64
+    h = (h + n) & M64
+    while p + 8 <= n:
+        h ^= _round(0, int.from_bytes(data[p:p + 8], "little"))
+        h = (_rotl(h, 27) * _P1 + _P4) & M64
+        p += 8
+    if p + 4 <= n:
+        h ^= (int.from_bytes(data[p:p + 4], "little") * _P1) & M64
+        h = (_rotl(h, 23) * _P2 + _P3) & M64
+        p += 4
+    while p < n:
+        h ^= (data[p] * _P5) & M64
+        h = (_rotl(h, 11) * _P1) & M64
+        p += 1
+    h ^= h >> 33
+    h = (h * _P2) & M64
+    h ^= h >> 29
+    h = (h * _P3) & M64
+    h ^= h >> 32
+    return h
+
+
+
 class ZstdError(Exception):
     pass
 
@@ -62,6 +118,9 @@ class FrameInfo:
         self.fcs_bytes = 0
         self.fcs = None
         self.single_segment = False
+        self.checksum = False
+        self.window = None
+        self.did_bytes = 0
         self.blocks = []
 
 
@@ -449,22 +508,55 @@ def _sequences(data, p, end, st, lits, out, frame_start):
 def decode_frame(data):
     """one frame, which must fill `data` exactly -> (bytes, FrameInfo)"""
     data = bytes(data)
+    out, info, end = _frame(data, 0)
+    _check(end == len(data), f"{len(data) - end} bytes after the last block")
+    return out, info
+
+
+def decode_stream(data):
+    """frames and skippable frames until `data` is used up -> (bytes, [FrameInfo of each frame])"""
+    data = bytes(data)
+    out, infos, p = b"", [], 0
+    while p < len(data):
+        _check(len(data) - p >= 5, "1 to 4 bytes after the last frame")
+        magic = int.from_bytes(data[p:p + 4], "little")
+        if magic & 0xFFFFFFF0 == 0x184D2A50:
+            _check(len(data) - p >= 8, "skippable frame header past the data")
+            n = int.from_bytes(data[p + 4:p + 8], "little")
+            _check(p + 8 + n <= len(data), "skippable frame past the data")
+            p += 8 + n
+            continue
+        o, info, p = _frame(data, p)
+        out += o
+        infos.append(info)
+    return out, infos
+
+
+def _frame(data, start):
+    """the frame at data[start:] -> (bytes, FrameInfo, end of the frame)"""
     info = FrameInfo()
-    _check(len(data) >= 6 and int.from_bytes(data[:4], "little") == MAGIC, "no zstd frame magic")
-    fhd = data[4]
+    _check(len(data) - start >= 6 and int.from_bytes(data[start:start + 4], "little") == MAGIC, "no zstd frame magic")
+    fhd = data[start + 4]
     info.fhd = fhd
     fcs_flag, single, cks, dict_flag = fhd >> 6, bool(fhd & 0x20), bool(fhd & 4), fhd & 3
     _check(not fhd & 8, "reserved frame header bit set")
-    _check(not cks, "content checksums are not produced by this encoder")
-    _check(dict_flag == 0, "dictionaries are not produced by this encoder")
     info.single_segment = single
-    p = 5
+    info.checksum = cks
+    p = start + 5
     window = None
     if not single:
+        _check(p < len(data), "frame header past the data")
         wd = data[p]
         exp, mant = (wd >> 3) + 10, wd & 7
+        _check(exp <= 31, "window above 2 GiB")
         window = (1 << exp) + ((1 << exp) >> 3) * mant
+        info.window = window
         p += 1
+    did_bytes = (0, 1, 2, 4)[dict_flag]
+    info.did_bytes = did_bytes
+    _check(p + did_bytes <= len(data), "frame header past the data")
+    _check(not any(data[p:p + did_bytes]), "a dictionary is required")
+    p += did_bytes
     fcs_bytes = (1 if single else 0, 2, 4, 8)[fcs_flag]
     info.fcs_bytes = fcs_bytes
     _check(p + fcs_bytes <= len(data), "frame header past the data")
@@ -507,10 +599,13 @@ def decode_frame(data):
         info.blocks.append(blk)
         if last:
             break
-    _check(p == len(data), f"{len(data) - p} bytes after the last block")
     if info.fcs is not None:
         _check(info.fcs == len(out), f"content size {info.fcs} but {len(out)} bytes produced")
-    return bytes(out), info
+    if cks:
+        _check(p + 4 <= len(data), "checksum past the data")
+        _check(int.from_bytes(data[p:p + 4], "little") == xxh64(bytes(out)) & 0xFFFFFFFF, "wrong content checksum")
+        p += 4
+    return bytes(out), info, p
 
 
 def huffman_depth(literals):
