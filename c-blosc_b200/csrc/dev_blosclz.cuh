@@ -313,10 +313,22 @@ DEV int blz_encode_main(const int clevel, const u8* __restrict__ b, const int le
 #undef BLZ_LIMIT
 }
 
+/* branch ids of blz_decode_warp; emulator builds count them, and remember the first check that refused a stream */
+enum { BLZ_H_DENSE, BLZ_H_DENSE_FEW, BLZ_H_DENSE_BAD, BLZ_H_FAR, BLZ_H_LENEXT, BLZ_H_LITERAL, BLZ_H_DROPPED, BLZ_NHIT };
+#ifdef SIMT_EMU
+static int g_blz_fail_line = 0;
+#define BLZ_FAIL (g_blz_fail_line = g_blz_fail_line ? g_blz_fail_line : __LINE__, 0)
+static long long g_blz_hit[BLZ_NHIT];
+#define BLZ_HIT(id) do { if (lane_id() == 0) g_blz_hit[id]++; } while (0)
+#else
+#define BLZ_FAIL 0
+#define BLZ_HIT(id) do {} while (0)
+#endif
+
 /* blosclz_decompress for one stream (blosclz.c:679-789).  Returns bytes written, 0 on error. */
 DEV int blz_decode_warp(const u8* __restrict__ in, const int length, u8* out, const int maxout) {
   int ip = 0, op = 0;
-  if (length == 0) return 0;
+  if (length == 0) return BLZ_FAIL;
   u32 ctrl = in[ip++] & 31u;
   const int lane = lane_id();
   int dense_skip = 0, dense_back = 0;
@@ -337,6 +349,7 @@ DEV int blz_decode_warp(const u8* __restrict__ in, const int length, u8* out, co
       const unsigned okm = __ballot_sync(FULLMASK, simple);
       int cnt = okm == FULLMASK ? 32 : __ffs((int)~okm) - 1;
       if (cnt < 4) {                                                       /* not worth a step: straight to the token machine */
+        BLZ_HIT(BLZ_H_DENSE_FEW);
         dense_back = dense_back < 32 ? dense_back + dense_back / 2 + 1 : 32;
         dense_skip = dense_back;
         goto serial;
@@ -354,6 +367,7 @@ DEV int blz_decode_warp(const u8* __restrict__ in, const int length, u8* out, co
       if (bad) cnt = __ffs((int)bad) - 1;
       if (cnt >= 4) {
         const int total = __shfl_sync(FULLMASK, incl, cnt - 1);
+        BLZ_HIT(BLZ_H_DENSE);
         if (lane < cnt) {
           const u32 v0 = ld_u32(out + ref), v1 = ld_u32(out + ref + 4);
           u8* o = out + dst;
@@ -370,6 +384,7 @@ DEV int blz_decode_warp(const u8* __restrict__ in, const int length, u8* out, co
         dense_back = 0;
         continue;
       }
+      BLZ_HIT(BLZ_H_DENSE_BAD);
       dense_back = dense_back < 32 ? dense_back + dense_back / 2 + 1 : 32;   /* not that kind of data right here: back off */
       dense_skip = dense_back;
     }
@@ -380,24 +395,26 @@ DEV int blz_decode_warp(const u8* __restrict__ in, const int length, u8* out, co
       long long ref = (long long)op - ofs;
       u32 code;
       if (len == 6) {
+        BLZ_HIT(BLZ_H_LENEXT);
         do {
-          if (ip + 1 >= length) return 0;
+          if (ip + 1 >= length) return BLZ_FAIL;               /* length bytes run into the end */
           code = in[ip++];
           len += code;
         } while (code == 255);
-      } else if (ip + 1 >= length) return 0;
+      } else if (ip + 1 >= length) return BLZ_FAIL;
       code = in[ip++];
       len += 3;
       ref -= code;
       if (code == 255 && ofs == (31 << 8)) {                  /* 16-bit far distance (:717-726) */
-        if (ip + 1 >= length) return 0;
+        BLZ_HIT(BLZ_H_FAR);
+        if (ip + 1 >= length) return BLZ_FAIL;                 /* no room for the 16-bit distance */
         ofs = (int)in[ip++] << 8;
         ofs += in[ip++];
         ref = (long long)op - ofs - BLZ_MAX_DISTANCE;
       }
-      if (op + len > maxout) return 0;                        /* :728-730 */
-      if (ref - 1 < 0) return 0;                              /* :732-734 */
-      if (ip >= length) break;                                /* :736 ends without copying */
+      if (op + len > maxout) return BLZ_FAIL;                        /* :728-730 */
+      if (ref - 1 < 0) return BLZ_FAIL;                              /* :732-734 */
+      if (ip >= length) { BLZ_HIT(BLZ_H_DROPPED); break; }    /* :736 ends without copying */
       ctrl = in[ip++];
       ref--;
       __syncwarp();
@@ -406,8 +423,9 @@ DEV int blz_decode_warp(const u8* __restrict__ in, const int length, u8* out, co
       op += (int)len;
     } else {
       ctrl++;
-      if ((long long)op + ctrl > maxout) return 0;            /* :769-774 */
-      if ((long long)ip + ctrl > length) return 0;
+      BLZ_HIT(BLZ_H_LITERAL);
+      if ((long long)op + ctrl > maxout) return BLZ_FAIL;            /* :769-774 */
+      if ((long long)ip + ctrl > length) return BLZ_FAIL;
       warp_copy_bytes(out + op, in + ip, (int)ctrl);
       op += (int)ctrl; ip += (int)ctrl;
       if (ip >= length) break;

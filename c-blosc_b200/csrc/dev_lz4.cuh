@@ -711,13 +711,40 @@ DEV int lz4_encode_warp(const u8* __restrict__ s, const int n, u8* __restrict__ 
 }
 
 /* ---- decoder ---- */
+/* branch ids of the decoders (lz4_decode_warp and lz4_pair_parse report through the same ones); emulator builds count
+ * them so that tests can tell which tier and which match source a stream reached */
+enum {
+  LZ4D_H_DENSE_SHIFT = 0,                    /* + s: a dense step whose last segment has byte shift s (0..8) */
+  LZ4D_H_DENSE_LONGCAP = 9,                  /* the segment loop stopped at LZ4D_DENSE_LONG long matches */
+  LZ4D_H_DENSE_BAD,                          /* a sequence that reads the step's own output (or before the block) ends the run */
+  LZ4D_H_DENSE_BAD0,                         /* ... already at lane 0 (cnt == 0) */
+  LZ4D_H_DENSE_FEW,                          /* fewer than LZ4D_DENSE_MIN short and no long sequence: no dense step */
+  LZ4D_H_DENSE_RING, LZ4D_H_DENSE_GLOBAL,    /* a dense sequence's match source */
+  LZ4D_H_LONE_RING, LZ4D_H_LONE_GLOBAL, LZ4D_H_LONE_PERIOD,
+  LZ4D_H_BATCH_FAST, LZ4D_H_BATCH_WALK,      /* the 0x49249249 chain of 3-byte sequences / the shuffle walk */
+  LZ4D_H_BATCH_RING, LZ4D_H_BATCH_GLOBAL,
+  LZ4D_H_SINGLE_RING, LZ4D_H_SINGLE_GLOBAL,
+  LZ4D_H_GEN_LITBUMP,                        /* a literal run longer than the ring moves ring_lo */
+  LZ4D_H_GEN_OFF0, LZ4D_H_GEN_RING, LZ4D_H_GEN_GLOBAL, LZ4D_H_GEN_LONG, LZ4D_H_GEN_LAST,
+  LZ4D_NHIT
+};
 #ifdef SIMT_EMU
 static long long g_dbg_lz4d_batch_seqs = 0, g_dbg_lz4d_fast_seqs = 0, g_dbg_lz4d_general_seqs = 0, g_dbg_lz4d_dense_seqs = 0;
 #define LZ4D_DBG(x) do { if (lane == 0) (x)++; } while (0)
 #define LZ4D_DBGN(x, n) do { if (lane == 0) (x) += (n); } while (0)
+static int g_lz4d_fail_line = 0;             /* emulator builds remember the first check that rejected the stream */
+#define LZ4D_FAIL (g_lz4d_fail_line = g_lz4d_fail_line ? g_lz4d_fail_line : __LINE__, -1)
+#define LZ4D_FAIL_NOTE() ((void)LZ4D_FAIL)                                       /* a refusal acted on later */
+static long long g_lz4d_hit[LZ4D_NHIT];
+#define LZ4D_HIT(id) do { if (lane == 0) g_lz4d_hit[id]++; } while (0)            /* warp-uniform branch */
+#define LZ4D_HITL(id, c) do { if (c) g_lz4d_hit[id]++; } while (0)               /* per lane */
 #else
 #define LZ4D_DBG(x) do {} while (0)
 #define LZ4D_DBGN(x, n) do {} while (0)
+#define LZ4D_FAIL (-1)
+#define LZ4D_FAIL_NOTE() do {} while (0)
+#define LZ4D_HIT(id) do {} while (0)
+#define LZ4D_HITL(id, c) do {} while (0)
 #endif
 #define LZ4D_RING 16384                      /* bytes of recent output mirrored in shared memory, per warp */
 #define LZ4D_RMASK (LZ4D_RING - 1)
@@ -746,8 +773,8 @@ DEV int lz4_decode_warp(const u8* __restrict__ in, const int csize, u8* out, con
   if (lane < 10) ((u32*)(ring_ptr + LZ4D_RING))[24 + lane] = 0;
   __syncwarp();
   int ring_lo = 0;                           /* positions [max(ring_lo, op-RING), op) are valid in the ring */
-  if (cap == 0) return (csize == 1 && in[0] == 0) ? 0 : -1;   /* lz4.c:2062-2066 */
-  if (csize == 0) return -1;
+  if (cap == 0) return (csize == 1 && in[0] == 0) ? 0 : LZ4D_FAIL;   /* lz4.c:2062-2066 */
+  if (csize == 0) return LZ4D_FAIL;
   int dense_skip = 0, dense_back = 0;
   for (;;) {
     /* ---- dense path: a run of literal-free sequences, one per lane ----
@@ -794,10 +821,14 @@ DEV int lz4_decode_warp(const u8* __restrict__ in, const int csize, u8* out, con
        * 8 bytes of slack because the word-wise copy below reads up to 7 bytes past the end of its source */
       const unsigned bad = __ballot_sync(FULLMASK, lane < cnt && (off < incl + 8 || match < 0));
       if (bad) cnt = __ffs((int)bad) - 1;
+      if (bad) LZ4D_HIT(cnt == 0 ? LZ4D_H_DENSE_BAD0 : LZ4D_H_DENSE_BAD);
       const unsigned longm = __ballot_sync(FULLMASK, lane < cnt && kind == 2);
       if (cnt >= LZ4D_DENSE_MIN || longm) {
         const int total = __shfl_sync(FULLMASK, incl, cnt - 1);
         const bool from_ring = off <= LZ4D_RING - LZ4D_DENSE_OUT - 64 && match >= ring_lo;
+        LZ4D_HIT(LZ4D_H_DENSE_SHIFT + sft);
+        if (sft == LZ4D_DENSE_LONG && c < 32) LZ4D_HIT(LZ4D_H_DENSE_LONGCAP);
+        LZ4D_HITL(from_ring ? LZ4D_H_DENSE_RING : LZ4D_H_DENSE_GLOBAL, lane < cnt);
         {
           /* every lane copies its own short match, 4 source bytes per step: from the ring (two aligned
            * words + funnel shift) or, for far offsets, from the output in global memory */
@@ -844,6 +875,8 @@ DEV int lz4_decode_warp(const u8* __restrict__ in, const int csize, u8* out, con
         const int tlen = 19 + (int)(tw >> 24), toff = (int)((tw >> 8) & 0xffffu), tmatch = op - toff;
         if ((tw & 0xffu) == 0x0fu && (tw >> 24) != 255u && toff != 0 && tmatch >= 0 && op + tlen <= oend - LZ4_MFLIMIT) {
           const bool tring = toff <= LZ4D_RING - 512 && tmatch >= ring_lo;
+          LZ4D_HIT(tring ? LZ4D_H_LONE_RING : LZ4D_H_LONE_GLOBAL);
+          if (toff < tlen) LZ4D_HIT(LZ4D_H_LONE_PERIOD);
           for (int k = lane; k < tlen; k += 32) {             /* sources are all before `op`: no lane waits for another */
             const int src = tmatch + (toff >= tlen ? k : k % toff);
             const u32 v = tring ? smem_ld_u8(ring, (u32)src & LZ4D_RMASK) : (u32)out[src];
@@ -857,6 +890,7 @@ DEV int lz4_decode_warp(const u8* __restrict__ in, const int csize, u8* out, con
           continue;
         }
       }
+      if (cnt > 0) LZ4D_HIT(LZ4D_H_DENSE_FEW);
       dense_back = dense_back < 8 ? dense_back + 1 : 8;   /* not that kind of data right here: back off */
       dense_skip = dense_back;
     }
@@ -905,7 +939,9 @@ DEV int lz4_decode_warp(const u8* __restrict__ in, const int csize, u8* out, con
       }
       if (nseq > 0) {
         const int match = op + my_opre + lit - off;            /* meaningful on real lanes */
-        if (__ballot_sync(FULLMASK, my_rank >= 0 && match < 0)) return -1;   /* lz4.c:2356 */
+        if (__ballot_sync(FULLMASK, my_rank >= 0 && match < 0)) return LZ4D_FAIL;   /* lz4.c:2356 */
+        LZ4D_HIT((g3 & 0x49249249u) == 0x49249249u ? LZ4D_H_BATCH_FAST : LZ4D_H_BATCH_WALK);
+        LZ4D_HITL(off <= LZ4D_RING - LZ4D_BATCH_OUT - 64 && match >= ring_lo ? LZ4D_H_BATCH_RING : LZ4D_H_BATCH_GLOBAL, my_rank >= 0);
         u32* tbl = (u32*)(ring_ptr + LZ4D_RING);               /* 11 x {info, off} then 10 start-bit words */
         u32* smask = tbl + 24;
         if (my_rank >= 0) {
@@ -957,8 +993,9 @@ DEV int lz4_decode_warp(const u8* __restrict__ in, const int csize, u8* out, con
         const int off = (int)(ow & 0xffffu);
         const int match = op + lit - off;
         if (off >= total && op + total <= oend - LZ4_MFLIMIT) { /* no self-overlap; far from the end of the block */
-          if (match < 0) return -1;                            /* lz4.c:2356 (off == 0 cannot get here: off >= total >= 4) */
+          if (match < 0) return LZ4D_FAIL;                     /* lz4.c:2356 (off == 0 cannot get here: off >= total >= 4) */
           const bool use_ring = off <= LZ4D_RING - 64 && match >= ring_lo;
+          LZ4D_HIT(use_ring ? LZ4D_H_SINGLE_RING : LZ4D_H_SINGLE_GLOBAL);
           if (lane < total) {
             u32 v;
             if (lane < lit) v = in[ip + 1 + lane];
@@ -980,24 +1017,24 @@ DEV int lz4_decode_warp(const u8* __restrict__ in, const int csize, u8* out, con
     int len = (int)(token >> 4);
     if (len == 15) {                                          /* read_variable_length(ip, iend-15, 1) */
       u32 sb;
-      if (ip >= iend - 15) return -1;
+      if (ip >= iend - 15) return LZ4D_FAIL;
       do {
         sb = in[ip++];
         len += (int)sb;
-        if (ip > iend - 15) return -1;
-        if (len > oend) return -1;                            /* same verdict as the cpy>oend test below, no int overflow */
+        if (ip > iend - 15) return LZ4D_FAIL;
+        if (len > oend) return LZ4D_FAIL;                     /* same verdict as the cpy>oend test below, no int overflow */
       } while (sb == 255);
     }
     int cpy = op + len;
     const bool last = cpy > oend - LZ4_MFLIMIT || ip + len > iend - (2 + 1 + LZ4_LASTLITERALS);   /* lz4.c:2289-2331 */
-    if (last && (ip + len != iend || cpy > oend)) return -1;
+    if (last && (ip + len != iend || cpy > oend)) return LZ4D_FAIL;
     for (int k = lane; k < len; k += 32) {                    /* literals -> output (+ ring) */
       const u32 v = in[ip + k];
       out[op + k] = (u8)v;
       smem_st_u8(ring, (u32)(op + k) & LZ4D_RMASK, v);
     }
-    if (len > LZ4D_RING - 64) ring_lo = cpy - (LZ4D_RING - 64) > ring_lo ? cpy - (LZ4D_RING - 64) : ring_lo;
-    if (last) { op += len; break; }
+    if (len > LZ4D_RING - 64) { ring_lo = cpy - (LZ4D_RING - 64) > ring_lo ? cpy - (LZ4D_RING - 64) : ring_lo; LZ4D_HIT(LZ4D_H_GEN_LITBUMP); }
+    if (last) { LZ4D_HIT(LZ4D_H_GEN_LAST); op += len; break; }
     ip += len; op = cpy;
     const int off = (int)in[ip] | ((int)in[ip + 1] << 8);
     ip += 2;
@@ -1008,19 +1045,20 @@ DEV int lz4_decode_warp(const u8* __restrict__ in, const int csize, u8* out, con
       do {
         sb = in[ip++];
         len += (int)sb;
-        if (ip > iend - LZ4_LASTLITERALS + 1) return -1;
-        if (len > oend) return -1;                            /* keeps `len` from overflowing on hostile input */
+        if (ip > iend - LZ4_LASTLITERALS + 1) return LZ4D_FAIL;
+        if (len > oend) return LZ4D_FAIL;                     /* keeps `len` from overflowing on hostile input */
       } while (sb == 255);
     }
     len += 4;
-    if (match < 0) return -1;                                 /* lz4.c:2356 */
+    if (match < 0) return LZ4D_FAIL;                          /* lz4.c:2356 */
     cpy = op + len;
-    if (cpy > oend - LZ4_LASTLITERALS) return -1;             /* lz4.c:2423 */
+    if (cpy > oend - LZ4_LASTLITERALS) return LZ4D_FAIL;      /* lz4.c:2423 */
     __syncwarp();                                             /* earlier output must be visible to all lanes */
     if (off == 0) {
       /* not a valid stream, but LZ4_decompress_safe accepts it: every copy routine first clears the
        * destination word ("silence msan warning when offset==0", lz4.c:2386-2390; LZ4_memcpy_using_offset_base)
        * and then replicates it, so the match decodes to zeros */
+      LZ4D_HIT(LZ4D_H_GEN_OFF0);
       for (int k = lane; k < len; k += 32) out[op + k] = 0;
       ring_lo = cpy;
     } else if (len <= 2048) {
@@ -1028,6 +1066,7 @@ DEV int lz4_decode_warp(const u8* __restrict__ in, const int csize, u8* out, con
        * sources are read from global memory, but the output still goes into the ring so that it
        * stays a mirror of the last 16 KiB */
       const bool from_ring = off <= LZ4D_RING - 2048 - 64 && match >= ring_lo;
+      LZ4D_HIT(from_ring ? LZ4D_H_GEN_RING : LZ4D_H_GEN_GLOBAL);
       for (int k0 = 0; k0 < len; k0 += 32) {
         const int k = k0 + lane;
         if (k < len) {
@@ -1038,6 +1077,7 @@ DEV int lz4_decode_warp(const u8* __restrict__ in, const int csize, u8* out, con
         }
       }
     } else {
+      LZ4D_HIT(LZ4D_H_GEN_LONG);
       warp_copy_match(out, op, match, len);                   /* global sources; ring no longer mirrors this span */
       ring_lo = cpy;
     }

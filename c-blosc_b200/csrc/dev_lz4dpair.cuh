@@ -197,8 +197,8 @@ DEV int lz4_pair_parse(const u8* __restrict__ in, const int csize, u8* out, cons
   const StreamBase ib = make_stream_base(in);
   int ip = 0, op = 0, k = 0, result = 0;
   int ring_lo = 0;
-  if (cap == 0) return (csize == 1 && in[0] == 0) ? 0 : -1;   /* lz4.c:2062-2066 */
-  if (csize == 0) return -1;
+  if (cap == 0) return (csize == 1 && in[0] == 0) ? 0 : LZ4D_FAIL;   /* lz4.c:2062-2066 */
+  if (csize == 0) return LZ4D_FAIL;
   {
     Lz4pSlot* q = lz4p_acquire(slots, k);
     if (lane == 0) {
@@ -243,10 +243,14 @@ DEV int lz4_pair_parse(const u8* __restrict__ in, const int csize, u8* out, cons
       const int dst = op + incl - ml, match = dst - off;
       const unsigned bad = __ballot_sync(FULLMASK, lane < cnt && (off < incl + 8 || match < 0));
       if (bad) cnt = __ffs((int)bad) - 1;
+      if (bad) LZ4D_HIT(cnt == 0 ? LZ4D_H_DENSE_BAD0 : LZ4D_H_DENSE_BAD);
       const unsigned longm = __ballot_sync(FULLMASK, lane < cnt && kind == 2);
       if (cnt >= LZ4D_DENSE_MIN || longm) {
         const int total = __shfl_sync(FULLMASK, incl, cnt - 1);
         const bool from_ring = off <= LZ4D_RING - LZ4D_DENSE_OUT - 64 && match >= ring_lo;
+        LZ4D_HIT(LZ4D_H_DENSE_SHIFT + sft);
+        if (sft == LZ4D_DENSE_LONG && c < 32) LZ4D_HIT(LZ4D_H_DENSE_LONGCAP);
+        LZ4D_HITL(from_ring ? LZ4D_H_DENSE_RING : LZ4D_H_DENSE_GLOBAL, lane < cnt);
         Lz4pSlot* q = lz4p_acquire(slots, k);
         q->w[2 * lane] = (u32)dst;
         q->w[2 * lane + 1] = (u32)off | ((u32)ml << 16) | ((u32)kind << 28) | (from_ring ? 0x80000000u : 0u);
@@ -262,6 +266,8 @@ DEV int lz4_pair_parse(const u8* __restrict__ in, const int csize, u8* out, cons
         const int tlen = 19 + (int)(tw >> 24), toff = (int)((tw >> 8) & 0xffffu), tmatch = op - toff;
         if ((tw & 0xffu) == 0x0fu && (tw >> 24) != 255u && toff != 0 && tmatch >= 0 && op + tlen <= oend - LZ4_MFLIMIT) {
           const bool tring = toff <= LZ4D_RING - 512 && tmatch >= ring_lo;
+          LZ4D_HIT(tring ? LZ4D_H_LONE_RING : LZ4D_H_LONE_GLOBAL);
+          if (toff < tlen) LZ4D_HIT(LZ4D_H_LONE_PERIOD);
           Lz4pSlot* q = lz4p_acquire(slots, k);
           if (lane == 0) { q->type = LZ4P_LONE; q->p[0] = (u32)op; q->p[1] = (u32)tlen; q->p[2] = (u32)toff; q->p[3] = tring ? 1u : 0u; }
           lz4p_publish(k);
@@ -271,6 +277,7 @@ DEV int lz4_pair_parse(const u8* __restrict__ in, const int csize, u8* out, cons
           continue;
         }
       }
+      if (cnt > 0) LZ4D_HIT(LZ4D_H_DENSE_FEW);
       dense_back = dense_back < 8 ? dense_back + 1 : 8;
       dense_skip = dense_back;
     }
@@ -314,7 +321,9 @@ DEV int lz4_pair_parse(const u8* __restrict__ in, const int csize, u8* out, cons
       }
       if (nseq > 0) {
         const int match = op + my_opre + lit - off;
-        if (__ballot_sync(FULLMASK, my_rank >= 0 && match < 0)) { result = -1; break; }   /* lz4.c:2356 */
+        if (__ballot_sync(FULLMASK, my_rank >= 0 && match < 0)) { result = LZ4D_FAIL; break; }   /* lz4.c:2356 */
+        LZ4D_HIT((g3 & 0x49249249u) == 0x49249249u ? LZ4D_H_BATCH_FAST : LZ4D_H_BATCH_WALK);
+        LZ4D_HITL(off <= LZ4D_RING - LZ4D_BATCH_OUT - 64 && match >= ring_lo ? LZ4D_H_BATCH_RING : LZ4D_H_BATCH_GLOBAL, my_rank >= 0);
         Lz4pSlot* q = lz4p_acquire(slots, k);
         if (lane < 10) q->w[22 + lane] = 0;
         __syncwarp();
@@ -343,8 +352,9 @@ DEV int lz4_pair_parse(const u8* __restrict__ in, const int csize, u8* out, cons
         const int off = (int)(ow & 0xffffu);
         const int match = op + lit - off;
         if (off >= total && op + total <= oend - LZ4_MFLIMIT) {
-          if (match < 0) { result = -1; break; }              /* lz4.c:2356 */
+          if (match < 0) { result = LZ4D_FAIL; break; }       /* lz4.c:2356 */
           const bool use_ring = off <= LZ4D_RING - 64 && match >= ring_lo;
+          LZ4D_HIT(use_ring ? LZ4D_H_SINGLE_RING : LZ4D_H_SINGLE_GLOBAL);
           Lz4pSlot* q = lz4p_acquire(slots, k);
           if (lane == 0) {
             q->type = LZ4P_SINGLE; q->p[0] = (u32)ip; q->p[1] = (u32)op; q->p[2] = (u32)lit; q->p[3] = (u32)total; q->p[4] = (u32)off;
@@ -363,21 +373,22 @@ DEV int lz4_pair_parse(const u8* __restrict__ in, const int csize, u8* out, cons
     int len = (int)(token >> 4);
     if (len == 15) {                                          /* read_variable_length(ip, iend-15, 1) */
       u32 sb;
-      if (ip >= iend - 15) { result = -1; break; }
+      if (ip >= iend - 15) { result = LZ4D_FAIL; break; }
       do {
         sb = in[ip++];
         len += (int)sb;
-        if (ip > iend - 15) { result = -1; break; }
-        if (len > oend) { result = -1; break; }
+        if (ip > iend - 15) { result = LZ4D_FAIL; break; }
+        if (len > oend) { result = LZ4D_FAIL; break; }
       } while (sb == 255);
       if (result < 0) break;
     }
     int cpy = op + len;
     const bool last = cpy > oend - LZ4_MFLIMIT || ip + len > iend - (2 + 1 + LZ4_LASTLITERALS);   /* lz4.c:2289-2331 */
-    if (last && (ip + len != iend || cpy > oend)) { result = -1; break; }
+    if (last && (ip + len != iend || cpy > oend)) { result = LZ4D_FAIL; break; }
     const int lsrc = ip, lop = op;
-    if (len > LZ4D_RING - 64) ring_lo = cpy - (LZ4D_RING - 64) > ring_lo ? cpy - (LZ4D_RING - 64) : ring_lo;
+    if (len > LZ4D_RING - 64) { ring_lo = cpy - (LZ4D_RING - 64) > ring_lo ? cpy - (LZ4D_RING - 64) : ring_lo; LZ4D_HIT(LZ4D_H_GEN_LITBUMP); }
     if (last) {
+      LZ4D_HIT(LZ4D_H_GEN_LAST);
       Lz4pSlot* q = lz4p_acquire(slots, k);
       if (lane == 0) { q->type = LZ4P_GENERAL; q->p[0] = (u32)lsrc; q->p[1] = (u32)lop; q->p[2] = (u32)len; q->p[3] = 0u; q->p[4] = 0u; q->p[5] = 0u; }
       lz4p_publish(k);
@@ -395,8 +406,8 @@ DEV int lz4_pair_parse(const u8* __restrict__ in, const int csize, u8* out, cons
       do {
         sb = in[ip++];
         mlen += (int)sb;
-        if (ip > iend - LZ4_LASTLITERALS + 1) { result = -1; break; }
-        if (mlen > oend) { result = -1; break; }
+        if (ip > iend - LZ4_LASTLITERALS + 1) { result = LZ4D_FAIL; break; }
+        if (mlen > oend) { result = LZ4D_FAIL; break; }
       } while (sb == 255);
       if (result < 0) break;
     }
@@ -405,13 +416,14 @@ DEV int lz4_pair_parse(const u8* __restrict__ in, const int csize, u8* out, cons
      * looks at the match */
     int how = 0;
     bool ok = true;
-    if (match < 0) ok = false;                                /* lz4.c:2356 */
+    if (match < 0) { ok = false; LZ4D_FAIL_NOTE(); }          /* lz4.c:2356 */
     cpy = op + mlen;
-    if (ok && cpy > oend - LZ4_LASTLITERALS) ok = false;      /* lz4.c:2423 */
+    if (ok && cpy > oend - LZ4_LASTLITERALS) { ok = false; LZ4D_FAIL_NOTE(); }   /* lz4.c:2423 */
     if (ok) {
       if (off == 0) { how = 0; ring_lo = cpy; }
       else if (mlen <= 2048) how = (off <= LZ4D_RING - 2048 - 64 && match >= ring_lo) ? 1 : 2;
       else { how = 3; ring_lo = cpy; }
+      LZ4D_HIT(how == 0 ? LZ4D_H_GEN_OFF0 : how == 1 ? LZ4D_H_GEN_RING : how == 2 ? LZ4D_H_GEN_GLOBAL : LZ4D_H_GEN_LONG);
     }
     {
       Lz4pSlot* q = lz4p_acquire(slots, k);

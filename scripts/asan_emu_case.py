@@ -1,7 +1,8 @@
 #!/usr/bin/env python
 """Workload for the AddressSanitizer build of the emulated library (make -C tests/emu asan):
   LD_PRELOAD=$(gcc -print-file-name=libasan.so) ASAN_OPTIONS=detect_leaks=0 python scripts/asan_emu_case.py
-exact / fast / lz4hc / BloscLZ paths, exact-size buffers, damaged chunks, crafted and damaged zstd frames and zlib streams."""
+exact / fast / lz4hc / BloscLZ paths, exact-size buffers, damaged chunks, crafted and damaged zstd frames and zlib streams,
+crafted, random and damaged LZ4 and BloscLZ streams."""
 import os, sys, ctypes as C, numpy as np
 sys.path.insert(0, os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), 'tests'))
 from datagen import gen, compress, decompress
@@ -74,5 +75,38 @@ for st,cap in streams:
 for name,ch,n in iedges.chunk_corpus():
     c=np.frombuffer(ch,np.uint8).copy(); out=np.zeros(n,np.uint8)
     emu.blosc_decompress_ctx(c.ctypes.data_as(C.c_void_p),out.ctypes.data_as(C.c_void_p),C.c_size_t(n),C.c_int(1))
+    cases+=1
+# the LZ4 and BloscLZ decoders on crafted streams (tests/test_lz_decode_edges.py): accepted, rejected, random and damaged
+# streams, each in an input buffer of exactly its size (the decoders' 12-byte window loads claim to stay below ip+109,
+# ip+42 and ip+12 at their tiers' entry conditions); both LZ4 decoders; the ring-reuse lists; then the chunks
+import random
+import test_lz_decode_edges as ledges
+for f in ("emu_lz4_decode","emu_lz4_decode_pair","emu_blz_decode"):
+    getattr(emu,f).restype=C.c_int; getattr(emu,f).argtypes=[C.c_void_p,C.c_int,C.c_void_p,C.c_int]
+lz=[(b,cap) for b,c,caps,_,_ in ledges.ACCEPT.values() for cap in (caps or [len(c)])]+[(b,cap) for b,cap,_ in ledges.REJECT.values()]
+rng=random.Random(5)
+for t in range(100):
+    b,c=ledges.random_block(rng); lz+=[(b,len(c)),(ledges._damaged(b,rng,2),len(c))]
+for b,cap in lz:
+    src=np.frombuffer(b,np.uint8).copy(); out=np.zeros(max(cap,1),np.uint8)
+    for f in (emu.emu_lz4_decode,emu.emu_lz4_decode_pair):
+        f(src.ctypes.data_as(C.c_void_p),C.c_int(len(b)),out.ctypes.data_as(C.c_void_p),C.c_int(cap))
+        cases+=1
+blz=[(s,cap) for s,_,cap,_,_ in ledges.BACCEPT.values()]+[(s,cap) for s,cap,_ in ledges.BREJECT.values()]
+for t in range(100):
+    s,c=ledges.random_blz(rng); blz+=[(s,len(c)),(ledges._damaged(s,rng,2),len(c))]
+for s,cap in blz:
+    src=np.frombuffer(s,np.uint8).copy(); out=np.zeros(max(cap,1),np.uint8)
+    emu.emu_blz_decode(src.ctypes.data_as(C.c_void_p),C.c_int(len(s)),out.ctypes.data_as(C.c_void_p),C.c_int(cap))
+    cases+=1
+emu.emu_lz4_decode_list.restype=None
+for pair in (0,1):
+    for name,a,(b,want) in ledges.ring_pairs():
+        ledges.decode_list(emu,[a[0],b],[len(a[1]),len(want)],pair)
+        cases+=1
+for name,ch,n in ledges.chunk_corpus():
+    c=np.frombuffer(ch,np.uint8).copy(); out=np.zeros(n,np.uint8)
+    emu.blosc_decompress_ctx(c.ctypes.data_as(C.c_void_p),out.ctypes.data_as(C.c_void_p),C.c_size_t(n),C.c_int(1))
+    emu.blosc_getitem(c.ctypes.data_as(C.c_void_p),C.c_int(0),C.c_int(n//ch[3]),out.ctypes.data_as(C.c_void_p))
     cases+=1
 print("asan workload ok, cases", cases)

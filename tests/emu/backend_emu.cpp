@@ -202,6 +202,7 @@ int emu_lz4_encode_team(const unsigned char* src, int n, unsigned char* dst, int
 }
 int emu_lz4_decode(const unsigned char* src, int csize, unsigned char* dst, int cap) {
   int result = 0;
+  g_lz4d_fail_line = 0;
   simt::launch(simt::Dim3(1), simt::Dim3(32), LZ4D_SMEM, [&] {
     int r = lz4_decode_warp(src, csize, dst, cap, simt::g_dynsmem);
     if ((threadIdx.x & 31) == 13) result = r;
@@ -211,6 +212,7 @@ int emu_lz4_decode(const unsigned char* src, int csize, unsigned char* dst, int 
 /* the same stream through a parser / copier pair */
 int emu_lz4_decode_pair(const unsigned char* src, int csize, unsigned char* dst, int cap) {
   int result = 0;
+  g_lz4d_fail_line = 0;
   simt::launch(simt::Dim3(1), simt::Dim3(64), LZ4P_SMEM, [&] {
     unsigned char* smem = simt::g_dynsmem;
     Lz4pSlot* slots = (Lz4pSlot*)(smem + LZ4D_RING);
@@ -233,12 +235,40 @@ int emu_blz_encode(int clevel, const unsigned char* src, int n, unsigned char* d
 }
 int emu_blz_decode(const unsigned char* src, int csize, unsigned char* dst, int cap) {
   int result = 0;
+  g_blz_fail_line = 0;
   simt::launch(simt::Dim3(1), simt::Dim3(32), 0, [&] {
     int r = blz_decode_warp(src, csize, dst, cap);
     if ((threadIdx.x & 31) == 0) result = r;
   });
   return result;
 }
+
+/* several LZ4 streams one after another in one launch, through the same warp (pair = 0) or the same parser / copier
+ * pair (pair = 1), as a CTA that draws several tickets: the ring is not cleared between streams.  results[i] and
+ * lines[i] are each stream's return code and first refusing line. */
+void emu_lz4_decode_list(const unsigned char* const* srcs, const int* csizes, unsigned char* const* dsts, const int* caps,
+                         int n, int pair, int* results, int* lines) {
+  simt::launch(simt::Dim3(1), simt::Dim3(pair ? 64 : 32), pair ? LZ4P_SMEM : LZ4D_SMEM, [&] {
+    unsigned char* smem = simt::g_dynsmem;
+    Lz4pSlot* slots = (Lz4pSlot*)(smem + LZ4D_RING);
+    if (pair && (threadIdx.x >> 5) == 1) { lz4_pair_copier(smem, slots); return; }
+    for (int i = 0; i < n; i++) {
+      __syncwarp();
+      if ((threadIdx.x & 31) == 0) g_lz4d_fail_line = 0;
+      __syncwarp();
+      const int r = pair ? lz4_pair_parse(srcs[i], csizes[i], dsts[i], caps[i], slots)
+                         : lz4_decode_warp(srcs[i], csizes[i], dsts[i], caps[i], smem);
+      __syncwarp();
+      if ((threadIdx.x & 31) == 13) { results[i] = r; lines[i] = g_lz4d_fail_line; }
+    }
+    if (pair) lz4_pair_quit(slots);
+  });
+}
+int emu_lz4d_fail_line(void) { return g_lz4d_fail_line; }
+int emu_blz_fail_line(void) { return g_blz_fail_line; }
+/* branch counters of the LZ4 decoders (LZ4D_H_*) and of the BloscLZ decoder (BLZ_H_*): copied out and cleared */
+int emu_lz4d_hits(long long* h) { for (int i = 0; i < LZ4D_NHIT; i++) { h[i] = g_lz4d_hit[i]; g_lz4d_hit[i] = 0; } return LZ4D_NHIT; }
+int emu_blz_hits(long long* h) { for (int i = 0; i < BLZ_NHIT; i++) { h[i] = g_blz_hit[i]; g_blz_hit[i] = 0; } return BLZ_NHIT; }
 
 int emu_zlib_fail_line(void) { return g_inf_fail_line; }
 int emu_zlib_decode(const unsigned char* src, int csize, unsigned char* dst, int cap) {
