@@ -516,18 +516,12 @@ __global__ void __launch_bounds__(COMPACT_THREADS) compact_kernel(CompactArgs a)
  * word-pair form of ld_u32 would touch up to 3 bytes past cbytes */
 DEV int ld_i32(const u8* p) { return (int)((u32)p[0] | ((u32)p[1] << 8) | ((u32)p[2] << 16) | ((u32)p[3] << 24)); }
 
-#define DECODE_WARPS 4
-/* dynamic shared memory: DECODE_WARPS * LZ4D_SMEM bytes (per-warp ring of recent output) */
-/* One instantiation per codec: the bit-serial inflate must not cost the LZ decoders registers,
- * stack or instruction-cache footprint. */
-template <int CODEC>
-__global__ void __launch_bounds__(DECODE_WARPS * 32) decode_kernel(DecodeArgs a) {
-#ifdef SIMT_EMU
-  u8* smem = simt::g_dynsmem;
-#else
-  extern __shared__ __align__(16) u8 smem[];
-#endif
-  const int warp = (int)(threadIdx.x >> 5);
+/* The stream loop of a decode launch, for one warp: every stream it draws is located by walking the size prefixes of
+ * its block up to its split (blosc.c:760-771, :784), then copied if stored raw (:773-776) or handed to
+ * `codec(src, cs, out, len)`, which returns the decoded size (:778-782).  Failures go to a.status; the warp that
+ * completes the stream count publishes it to status_out and puts the counters back to zero. */
+template <class Codec>
+DEV void decode_streams(const DecodeArgs& a, Codec codec) {
   int mine = 0;
   for (;;) {
     const int idx = next_stream(a.queue, a.queue_base, a.map);
@@ -535,7 +529,6 @@ __global__ void __launch_bounds__(DECODE_WARPS * 32) decode_kernel(DecodeArgs a)
     int block, len, split;
     long long off;
     stream_locate(a.map, idx, &block, &off, &len, &split);
-    /* walk the size prefixes of this block up to our split (blosc.c:760-771, :784) */
     int so = ld_i32(a.chunk + 16 + 4ll * block);
     int cs = 0, err = 0;
     for (int s = 0; s <= split; s++) {
@@ -548,15 +541,8 @@ __global__ void __launch_bounds__(DECODE_WARPS * 32) decode_kernel(DecodeArgs a)
     if (!err) {
       u8* out = a.out + (off - a.out_shift);
       const u8* src = a.chunk + so;
-      if (cs == len) warp_copy_bytes(out, src, len);                    /* stored raw, blosc.c:773-776 */
-      else {
-        int n;
-        if (CODEC == B2_CODEC_LZ4) n = lz4_decode_warp(src, cs, out, len, smem + (size_t)warp * LZ4D_SMEM);
-        else if (CODEC == B2_CODEC_ZLIB) n = zlib_decode_warp(src, cs, out, len, smem + (size_t)warp * LZ4D_SMEM);
-        else if (CODEC == B2_CODEC_ZSTD) n = zstd_decode_warp(src, cs, out, len, smem + (size_t)warp * LZ4D_SMEM);
-        else n = blz_decode_warp(src, cs, out, len);
-        if (n != len) err = B2_ERR_CODEC;                               /* blosc.c:778-782 */
-      }
+      if (cs == len) warp_copy_bytes(out, src, len);                    /* stored raw */
+      else if (codec(src, cs, out, len) != len) err = B2_ERR_CODEC;
     }
     if (err && lane_id() == 0) atomicMin(a.status, err);
     mine++;
@@ -572,6 +558,26 @@ __global__ void __launch_bounds__(DECODE_WARPS * 32) decode_kernel(DecodeArgs a)
   if (lane_id() == 0) { *a.status_out = ld_cg_i32(a.status); *a.status = 0; *a.done = 0; }
 }
 
+#define DECODE_WARPS 4
+/* dynamic shared memory: DECODE_WARPS * LZ4D_SMEM bytes (per-warp ring of recent output) */
+/* One instantiation per codec: the bit-serial inflate must not cost the LZ decoders registers,
+ * stack or instruction-cache footprint. */
+template <int CODEC>
+__global__ void __launch_bounds__(DECODE_WARPS * 32) decode_kernel(DecodeArgs a) {
+#ifdef SIMT_EMU
+  u8* smem = simt::g_dynsmem;
+#else
+  extern __shared__ __align__(16) u8 smem[];
+#endif
+  u8* wsmem = smem + (size_t)(threadIdx.x >> 5) * LZ4D_SMEM;
+  decode_streams(a, [&](const u8* src, int cs, u8* out, int len) {
+    if (CODEC == B2_CODEC_LZ4) return lz4_decode_warp(src, cs, out, len, wsmem);
+    if (CODEC == B2_CODEC_ZLIB) return zlib_decode_warp(src, cs, out, len, wsmem);
+    if (CODEC == B2_CODEC_ZSTD) return zstd_decode_warp(src, cs, out, len, wsmem);
+    return blz_decode_warp(src, cs, out, len);
+  });
+}
+
 
 /* LZ4 chunks: one CTA of two warps per stream -- a parser that walks the tokens and a copier that owns the output
  * (dev_lz4dpair.cuh).  The parser warp alone draws tickets, checks the size prefixes, counts finished streams and
@@ -585,39 +591,6 @@ __global__ void __launch_bounds__(64) decode_pair_kernel(DecodeArgs a) {
 #endif
   Lz4pSlot* slots = (Lz4pSlot*)(smem + LZ4D_RING);
   if ((threadIdx.x >> 5) == 1) { lz4_pair_copier(smem, slots); return; }
-  int mine = 0;
-  for (;;) {
-    const int idx = next_stream(a.queue, a.queue_base, a.map);
-    if (idx < 0) break;
-    int block, len, split;
-    long long off;
-    stream_locate(a.map, idx, &block, &off, &len, &split);
-    int so = ld_i32(a.chunk + 16 + 4ll * block);
-    int cs = 0, err = 0;
-    for (int s = 0; s <= split; s++) {
-      if (so < 0 || so > a.cbytes - 4) { err = B2_ERR_BOUNDS; break; }
-      cs = ld_i32(a.chunk + so);
-      so += 4;
-      if (cs < 0 || cs > a.cbytes - so) { err = B2_ERR_BOUNDS; break; }
-      if (s < split) so += cs;
-    }
-    if (!err) {
-      u8* out = a.out + (off - a.out_shift);
-      const u8* src = a.chunk + so;
-      if (cs == len) warp_copy_bytes(out, src, len);                    /* stored raw, blosc.c:773-776 */
-      else if (lz4_pair_parse(src, cs, out, len, slots) != len) err = B2_ERR_CODEC;   /* blosc.c:778-782 */
-    }
-    if (err && lane_id() == 0) atomicMin(a.status, err);
-    mine++;
-    __syncwarp();
-  }
+  decode_streams(a, [&](const u8* src, int cs, u8* out, int len) { return lz4_pair_parse(src, cs, out, len, slots); });
   lz4_pair_quit(slots);
-  if (mine == 0) return;
-  __threadfence();
-  int last = 0;
-  if (lane_id() == 0) last = atomicAdd(a.done, mine) + mine == a.map.nstreams;
-  last = __shfl_sync(FULLMASK, last, 0);
-  if (!last) return;
-  __threadfence();
-  if (lane_id() == 0) { *a.status_out = ld_cg_i32(a.status); *a.status = 0; *a.done = 0; }
 }

@@ -12,15 +12,18 @@
  * lane wins, and only probes up to and including it are committed to the table, so
  * the table evolves exactly as in the serial code and the output is byte-identical.
  *
- * Decoder: LZ4_decompress_safe semantics (lz4.c:2022-2445).  Four tiers: a dense path for
+ * Decoder: LZ4_decompress_safe semantics (lz4.c:2022-2445).  Five tiers: a dense path for
  * chains of literal-free sequences (one 3-byte sequence per lane, long matches with one
  * extra length byte taken inline: up to 32 sequences per step, every lane copying its own
- * match), a batch path (every lane speculatively parses the sequence that would start at
+ * match), a lone long match that overlaps its own output, a batch path (every lane speculatively parses the sequence that would start at
  * its input byte; the chain of real starts is resolved with one ballot or a short shuffle
  * walk and up to 11 sequences are copied 32 output bytes per instruction), a
  * single-sequence fast path, and the general path with warp-wide literal and
  * period-replicating match copies.  A per-warp shared-memory ring mirrors the last 16 KiB
  * of output so match sources do not wait behind the global stores that produced them.
+ * The tier walk (lz4d_walk) is written once and hands the copies of every step to a copy
+ * routine: run by the same warp (lz4_decode_warp), or by a second warp that takes them from a
+ * queue (lz4_pair_parse, dev_lz4dpair.cuh).
  */
 #pragma once
 #include "dev_common.cuh"
@@ -711,7 +714,7 @@ DEV int lz4_encode_warp(const u8* __restrict__ s, const int n, u8* __restrict__ 
 }
 
 /* ---- decoder ---- */
-/* branch ids of the decoders (lz4_decode_warp and lz4_pair_parse report through the same ones); emulator builds count
+/* branch ids of the tier walk (lz4_decode_warp and lz4_pair_parse both run it); emulator builds count
  * them so that tests can tell which tier and which match source a stream reached */
 enum {
   LZ4D_H_DENSE_SHIFT = 0,                    /* + s: a dense step whose last segment has byte shift s (0..8) */
@@ -734,7 +737,6 @@ static long long g_dbg_lz4d_batch_seqs = 0, g_dbg_lz4d_fast_seqs = 0, g_dbg_lz4d
 #define LZ4D_DBGN(x, n) do { if (lane == 0) (x) += (n); } while (0)
 static int g_lz4d_fail_line = 0;             /* emulator builds remember the first check that rejected the stream */
 #define LZ4D_FAIL (g_lz4d_fail_line = g_lz4d_fail_line ? g_lz4d_fail_line : __LINE__, -1)
-#define LZ4D_FAIL_NOTE() ((void)LZ4D_FAIL)                                       /* a refusal acted on later */
 static long long g_lz4d_hit[LZ4D_NHIT];
 #define LZ4D_HIT(id) do { if (lane == 0) g_lz4d_hit[id]++; } while (0)            /* warp-uniform branch */
 #define LZ4D_HITL(id, c) do { if (c) g_lz4d_hit[id]++; } while (0)               /* per lane */
@@ -742,7 +744,6 @@ static long long g_lz4d_hit[LZ4D_NHIT];
 #define LZ4D_DBG(x) do {} while (0)
 #define LZ4D_DBGN(x, n) do {} while (0)
 #define LZ4D_FAIL (-1)
-#define LZ4D_FAIL_NOTE() do {} while (0)
 #define LZ4D_HIT(id) do {} while (0)
 #define LZ4D_HITL(id, c) do {} while (0)
 #endif
@@ -752,29 +753,205 @@ static long long g_lz4d_hit[LZ4D_NHIT];
 #define LZ4D_DENSE_LONG 8                    /* long matches (one extra length byte) a dense step takes inline */
 #define LZ4D_DENSE_OUT 2624                  /* a dense step writes <= 24 x 18 + 8 x 273 bytes */
 #define LZ4D_DENSE_MIN 4                     /* fewer chained 3-byte sequences than this: the 11-wide batch path is as good */
-#define LZ4D_SCRATCH 256                     /* per-warp shared scratch after the ring: sequence table + start-bit words */
+#define LZ4D_SCRATCH 256                     /* per-warp shared scratch after the ring: the batch table (lz4d_batch_table) */
 #define LZ4D_SMEM (LZ4D_RING + LZ4D_SCRATCH)
 
-/* LZ4_decompress_safe for one stream (lz4.c:2451-2456; safe-loop rules :2234-2436).
+/* ---- decoder copy routines, one per tier ----
+ * lz4_decode_warp calls them inline; the pair decoder's copier warp (dev_lz4dpair.cuh) calls them on the fields of a
+ * descriptor.  Each one writes its output both to `out` and to the ring, so that the ring keeps mirroring the most
+ * recent output; none ends with a __syncwarp (the caller makes the bytes visible). */
+enum { LZ4D_ZERO = 0, LZ4D_FROM_RING = 1, LZ4D_FROM_GLOBAL = 2, LZ4D_LONG = 3 };   /* how a general-path match is copied */
+#define LZ4D_TBL_START 22                    /* batch table: 11 x {info, offset}, then 10 start-bit words */
+
+/* dense step: lanes [0, cnt) hold one sequence each (kind 1: 4..18-byte match, kind 2: long match, lanes `longm`),
+ * its output at dst and its source off bytes back -- before the step's first output byte */
+DEV void lz4d_copy_dense(u8* out, smem_addr_t ring, int dst, int off, int ml, int kind, bool from_ring, int cnt,
+                         unsigned longm) {
+  const int lane = lane_id();
+  const int match = dst - off;
+  {
+    /* every lane copies its own short match, 4 source bytes per step: from the ring (two aligned
+     * words + funnel shift) or, for far offsets, from the output in global memory */
+    const int mls = (lane < cnt && kind == 1) ? ml : 0;
+    const int mlmax = __ballot_sync(FULLMASK, mls > 16) ? 18 : (__ballot_sync(FULLMASK, mls > 8) ? 16 : 8);
+    u8* o = out + dst;
+#pragma unroll 1
+    for (int k = 0; k < mlmax; k += 4) {
+      if (k < mls) {
+        u32 v;
+        if (from_ring) {
+          const u32 m = (u32)(match + k);
+          v = __funnelshift_r(smem_ld_u32(ring, m & (LZ4D_RMASK & ~3u)), smem_ld_u32(ring, (m + 4u) & (LZ4D_RMASK & ~3u)), (m & 3u) * 8u);
+        } else v = ld_u32(out + match + k);       /* may read a few bytes past the source: they are not used */
+        const int nb = mls - k;
+        const u32 r = (u32)(dst + k);
+        o[k] = (u8)v; smem_st_u8(ring, r & LZ4D_RMASK, v);
+        if (nb > 1) { o[k + 1] = (u8)(v >> 8); smem_st_u8(ring, (r + 1u) & LZ4D_RMASK, v >> 8); }
+        if (nb > 2) { o[k + 2] = (u8)(v >> 16); smem_st_u8(ring, (r + 2u) & LZ4D_RMASK, v >> 16); }
+        if (nb > 3) { o[k + 3] = (u8)(v >> 24); smem_st_u8(ring, (r + 3u) & LZ4D_RMASK, v >> 24); }
+      }
+    }
+  }
+  /* the long ones, by the whole warp (their sources also lie before this step's output) */
+  for (unsigned tm = longm; tm; tm &= tm - 1u) {
+    const int t = __ffs((int)tm) - 1;
+    const int td = __shfl_sync(FULLMASK, dst, t), tmt = __shfl_sync(FULLMASK, match, t), tl = __shfl_sync(FULLMASK, ml, t);
+    const bool tring = __shfl_sync(FULLMASK, (int)from_ring, t) != 0;
+    for (int k = lane; k < tl; k += 32) {
+      const u32 v = tring ? smem_ld_u8(ring, (u32)(tmt + k) & LZ4D_RMASK) : (u32)out[tmt + k];
+      out[td + k] = (u8)v;
+      smem_st_u8(ring, (u32)(td + k) & LZ4D_RMASK, v);
+    }
+  }
+}
+
+/* one long match whose source overlaps its own output (small offsets): period copy by the warp */
+DEV void lz4d_copy_lone(u8* out, smem_addr_t ring, int op, int len, int off, bool from_ring) {
+  const int match = op - off;
+  for (int k = lane_id(); k < len; k += 32) {             /* sources are all before `op`: no lane waits for another */
+    const int src = match + (off >= len ? k : k % off);
+    const u32 v = from_ring ? smem_ld_u8(ring, (u32)src & LZ4D_RMASK) : (u32)out[src];
+    out[op + k] = (u8)v;
+    smem_st_u8(ring, (u32)(op + k) & LZ4D_RMASK, v);
+  }
+}
+
+/* the batch's sequence table (tbl[0..21]: {output offset | literals << 9 | input lane << 13, offset} by rank) and its
+ * start bits (tbl[22..31]: bit y = a sequence starts at output byte y of the batch), written by the real lanes */
+DEV void lz4d_batch_table(u32* tbl, int my_rank, int my_opre, int lit, int off) {
+  const int lane = lane_id();
+  if (lane < 10) tbl[LZ4D_TBL_START + lane] = 0;
+  __syncwarp();
+  if (my_rank >= 0) {
+    tbl[2 * my_rank] = (u32)my_opre | ((u32)lit << 9) | ((u32)lane << 13);
+    tbl[2 * my_rank + 1] = (u32)off;
+    atomicOr(&tbl[LZ4D_TBL_START + (my_opre >> 5)], 1u << (my_opre & 31));
+  }
+}
+
+/* the batch's `total` output bytes, 32 per instruction: lane y finds its sequence by counting start bits */
+DEV void lz4d_copy_batch(const u8* in, u8* out, smem_addr_t ring, int ip, int op, int total, int ring_lo, const u32* tbl) {
+  const int lane = lane_id();
+  int kbase = 0;
+  for (int r = 0; r * 32 < total; r++) {
+    const u32 w = tbl[LZ4D_TBL_START + r];
+    const int y = r * 32 + lane;
+    if (y < total) {
+      const int k = kbase + __popc(w & ((2u << lane) - 1u)) - 1;
+      const u32 e0 = tbl[2 * k], offk = tbl[2 * k + 1];
+      const int opre = (int)(e0 & 511u), litk = (int)((e0 >> 9) & 15u), lanek = (int)(e0 >> 13);
+      const int j = y - opre;
+      u32 v;
+      if (j < litk) v = in[ip + lanek + 1 + j];
+      else {
+        const int src = op + opre + litk - (int)offk + (j - litk);
+        const int m0 = op + opre + litk - (int)offk;
+        if ((int)offk <= LZ4D_RING - LZ4D_BATCH_OUT - 64 && m0 >= ring_lo) v = smem_ld_u8(ring, (u32)src & LZ4D_RMASK);
+        else v = out[src];
+      }
+      out[op + y] = (u8)v;
+      smem_st_u8(ring, (u32)(op + y) & LZ4D_RMASK, v);
+    }
+    kbase += __popc(w);
+  }
+}
+
+/* one short sequence (lit literals at in[ip+1..], then a match off bytes back), one lane per output byte */
+DEV void lz4d_copy_single(const u8* in, u8* out, smem_addr_t ring, int ip, int op, int lit, int total, int off,
+                          bool use_ring) {
+  const int lane = lane_id();
+  const int match = op + lit - off;
+  if (lane < total) {
+    u32 v;
+    if (lane < lit) v = in[ip + 1 + lane];
+    else if (use_ring) v = smem_ld_u8(ring, (u32)(match + lane - lit) & LZ4D_RMASK);
+    else v = out[match + lane - lit];
+    out[op + lane] = (u8)v;
+    smem_st_u8(ring, (u32)(op + lane) & LZ4D_RMASK, v);
+  }
+}
+
+/* len literals from in[lsrc..] to out[op..], then (mlen > 0) a match of mlen bytes off bytes back, copied as `how` says */
+DEV void lz4d_copy_general(const u8* in, u8* out, smem_addr_t ring, int lsrc, int op, int len, int mlen, int off, int how) {
+  const int lane = lane_id();
+  for (int k = lane; k < len; k += 32) {
+    const u32 v = in[lsrc + k];
+    out[op + k] = (u8)v;
+    smem_st_u8(ring, (u32)(op + k) & LZ4D_RMASK, v);
+  }
+  if (mlen == 0) return;
+  op += len;
+  const int match = op - off;
+  __syncwarp();                                             /* earlier output must be visible to all lanes */
+  if (how == LZ4D_ZERO) {
+    for (int k = lane; k < mlen; k += 32) out[op + k] = 0;
+  } else if (how != LZ4D_LONG) {
+    /* sources lie before `op`; inside the ring they are not overwritten by this copy.  Far
+     * sources are read from global memory, but the output still goes into the ring so that it
+     * stays a mirror of the last 16 KiB */
+    const bool from_ring = how == LZ4D_FROM_RING;
+    for (int k0 = 0; k0 < mlen; k0 += 32) {
+      const int k = k0 + lane;
+      if (k < mlen) {
+        const int src = match + (off >= mlen ? k : k % off);
+        const u32 v = from_ring ? smem_ld_u8(ring, (u32)src & LZ4D_RMASK) : (u32)out[src];
+        out[op + k] = (u8)v;
+        smem_st_u8(ring, (u32)(op + k) & LZ4D_RMASK, v);
+      }
+    }
+  } else warp_copy_match(out, op, match, mlen);             /* global sources; ring no longer mirrors this span */
+}
+
+/* The copies of the single-warp decoder: made on the spot, by the parsing warp.  `ring_ptr` is LZ4D_SMEM bytes of
+ * warp-private shared memory: the ring, then the batch table. */
+struct Lz4dWarpCopies {
+  const u8* in;
+  u8* out;
+  u8* ring_ptr;
+  smem_addr_t ring;
+  DEV Lz4dWarpCopies(u8* out_, u8* ring_ptr_) : in(nullptr), out(out_), ring_ptr(ring_ptr_), ring(smem_addr(ring_ptr_)) {}
+  DEV void start(const u8* in_) { in = in_; }
+  DEV void dense(int dst, int off, int ml, int kind, bool from_ring, int cnt, unsigned longm) {
+    lz4d_copy_dense(out, ring, dst, off, ml, kind, from_ring, cnt, longm);
+    __syncwarp();
+  }
+  DEV void lone(int op, int len, int off, bool from_ring) { lz4d_copy_lone(out, ring, op, len, off, from_ring); __syncwarp(); }
+  DEV u32* batch_table() { return (u32*)(ring_ptr + LZ4D_RING); }
+  DEV void batch(int ip, int op, int total, int ring_lo) {
+    __syncwarp();
+    lz4d_copy_batch(in, out, ring, ip, op, total, ring_lo, batch_table());
+    __syncwarp();
+  }
+  DEV void single(int ip, int op, int lit, int total, int off, bool use_ring) {
+    lz4d_copy_single(in, out, ring, ip, op, lit, total, off, use_ring);
+    __syncwarp();
+  }
+  DEV void literals(int lsrc, int op, int len) { lz4d_copy_general(in, out, ring, lsrc, op, len, 0, 0, LZ4D_ZERO); }
+  DEV void match(int op, int mlen, int off, int how) {
+    lz4d_copy_general(in, out, ring, 0, op, 0, mlen, off, how);
+    __syncwarp();
+  }
+  DEV void finish() {}
+};
+
+/* LZ4_decompress_safe for one stream (lz4.c:2451-2456; safe-loop rules :2234-2436): the tier walk.
  * Returns the number of bytes written or -1.  offset==0 decodes to zeros, as in the reference.
  *
- * `ring` (LZ4D_RING bytes of warp-private shared memory) mirrors the most recent output so
- * that match sources -- a few KiB back in >99% of the sequences of shuffled data -- come
- * from shared memory instead of a global load behind the stores that produced them.
- * Fast path: token, literals (<= 8) and offset are parsed from one 12-byte register window,
- * and the whole sequence (literals + match, <= 26 bytes) is produced by one predicated
- * load/store step, one lane per output byte. */
-DEV int lz4_decode_warp(const u8* __restrict__ in, const int csize, u8* out, const int cap, u8* ring_ptr) {
+ * The walk keeps ip / op / ring_lo and decides, for every step, what is copied where; `cp` performs the copies
+ * (Lz4dWarpCopies: the same warp, now; Lz4dPairCopies in dev_lz4dpair.cuh: a second warp, from a queue).  The ring
+ * mirrors the most recent output so that match sources -- a few KiB back in >99% of the sequences of shuffled data --
+ * come from shared memory instead of a global load behind the stores that produced them; `ring_lo` is where that
+ * mirror begins to be valid: positions [max(ring_lo, op-RING), op) are in the ring. */
+template <class Copies>
+DEV int lz4d_walk(const u8* __restrict__ in, const int csize, const int cap, Copies& cp) {
   const int iend = csize, oend = cap;
   const int lane = lane_id();
   const StreamBase ib = make_stream_base(in);
-  const smem_addr_t ring = smem_addr(ring_ptr);
-  int ip = 0, op = 0;
-  if (lane < 10) ((u32*)(ring_ptr + LZ4D_RING))[24 + lane] = 0;
-  __syncwarp();
-  int ring_lo = 0;                           /* positions [max(ring_lo, op-RING), op) are valid in the ring */
+  int ip = 0, op = 0, result = 0;
+  int ring_lo = 0;
   if (cap == 0) return (csize == 1 && in[0] == 0) ? 0 : LZ4D_FAIL;   /* lz4.c:2062-2066 */
   if (csize == 0) return LZ4D_FAIL;
+  cp.start(in);
   int dense_skip = 0, dense_back = 0;
   for (;;) {
     /* ---- dense path: a run of literal-free sequences, one per lane ----
@@ -818,7 +995,7 @@ DEV int lz4_decode_warp(const u8* __restrict__ in, const int csize, u8* out, con
       }
       const int dst = op + incl - ml, match = dst - off;
       /* first sequence that reads its own batch's output (or is invalid: off == 0, match < 0) ends the run;
-       * 8 bytes of slack because the word-wise copy below reads up to 7 bytes past the end of its source */
+       * 8 bytes of slack because the word-wise copy reads up to 7 bytes past the end of its source */
       const unsigned bad = __ballot_sync(FULLMASK, lane < cnt && (off < incl + 8 || match < 0));
       if (bad) cnt = __ffs((int)bad) - 1;
       if (bad) LZ4D_HIT(cnt == 0 ? LZ4D_H_DENSE_BAD0 : LZ4D_H_DENSE_BAD);
@@ -829,47 +1006,13 @@ DEV int lz4_decode_warp(const u8* __restrict__ in, const int csize, u8* out, con
         LZ4D_HIT(LZ4D_H_DENSE_SHIFT + sft);
         if (sft == LZ4D_DENSE_LONG && c < 32) LZ4D_HIT(LZ4D_H_DENSE_LONGCAP);
         LZ4D_HITL(from_ring ? LZ4D_H_DENSE_RING : LZ4D_H_DENSE_GLOBAL, lane < cnt);
-        {
-          /* every lane copies its own short match, 4 source bytes per step: from the ring (two aligned
-           * words + funnel shift) or, for far offsets, from the output in global memory */
-          const int mls = (lane < cnt && kind == 1) ? ml : 0;
-          const int mlmax = __ballot_sync(FULLMASK, mls > 16) ? 18 : (__ballot_sync(FULLMASK, mls > 8) ? 16 : 8);
-          u8* o = out + dst;
-#pragma unroll 1
-          for (int k = 0; k < mlmax; k += 4) {
-            if (k < mls) {
-              u32 v;
-              if (from_ring) {
-                const u32 m = (u32)(match + k);
-                v = __funnelshift_r(smem_ld_u32(ring, m & (LZ4D_RMASK & ~3u)), smem_ld_u32(ring, (m + 4u) & (LZ4D_RMASK & ~3u)), (m & 3u) * 8u);
-              } else v = ld_u32(out + match + k);       /* may read a few bytes past the source: they are not used */
-              const int nb = mls - k;
-              const u32 r = (u32)(dst + k);
-              o[k] = (u8)v; smem_st_u8(ring, r & LZ4D_RMASK, v);
-              if (nb > 1) { o[k + 1] = (u8)(v >> 8); smem_st_u8(ring, (r + 1u) & LZ4D_RMASK, v >> 8); }
-              if (nb > 2) { o[k + 2] = (u8)(v >> 16); smem_st_u8(ring, (r + 2u) & LZ4D_RMASK, v >> 16); }
-              if (nb > 3) { o[k + 3] = (u8)(v >> 24); smem_st_u8(ring, (r + 3u) & LZ4D_RMASK, v >> 24); }
-            }
-          }
-        }
-        /* the long ones, by the whole warp (their sources also lie before this step's output) */
-        for (unsigned tm = longm; tm; tm &= tm - 1u) {
-          const int t = __ffs((int)tm) - 1;
-          const int td = __shfl_sync(FULLMASK, dst, t), tmt = __shfl_sync(FULLMASK, match, t), tl = __shfl_sync(FULLMASK, ml, t);
-          const bool tring = __shfl_sync(FULLMASK, (int)from_ring, t) != 0;
-          for (int k = lane; k < tl; k += 32) {
-            const u32 v = tring ? smem_ld_u8(ring, (u32)(tmt + k) & LZ4D_RMASK) : (u32)out[tmt + k];
-            out[td + k] = (u8)v;
-            smem_st_u8(ring, (u32)(td + k) & LZ4D_RMASK, v);
-          }
-        }
-        __syncwarp();
+        cp.dense(dst, off, ml, kind, from_ring, cnt, longm);
         ip += 3 * cnt + __popc(longm); op += total;
         LZ4D_DBGN(g_dbg_lz4d_dense_seqs, cnt);
         dense_back = 0;
         continue;
       }
-      /* a lone long match whose source overlaps its own output (small offsets): period copy by the warp */
+      /* a lone long match whose source overlaps its own output (small offsets) */
       {
         const u32 tw = __shfl_sync(FULLMASK, b0, 0);
         const int tlen = 19 + (int)(tw >> 24), toff = (int)((tw >> 8) & 0xffffu), tmatch = op - toff;
@@ -877,13 +1020,7 @@ DEV int lz4_decode_warp(const u8* __restrict__ in, const int csize, u8* out, con
           const bool tring = toff <= LZ4D_RING - 512 && tmatch >= ring_lo;
           LZ4D_HIT(tring ? LZ4D_H_LONE_RING : LZ4D_H_LONE_GLOBAL);
           if (toff < tlen) LZ4D_HIT(LZ4D_H_LONE_PERIOD);
-          for (int k = lane; k < tlen; k += 32) {             /* sources are all before `op`: no lane waits for another */
-            const int src = tmatch + (toff >= tlen ? k : k % toff);
-            const u32 v = tring ? smem_ld_u8(ring, (u32)src & LZ4D_RMASK) : (u32)out[src];
-            out[op + k] = (u8)v;
-            smem_st_u8(ring, (u32)(op + k) & LZ4D_RMASK, v);
-          }
-          __syncwarp();
+          cp.lone(op, tlen, toff, tring);
           ip += 4; op += tlen;
           LZ4D_DBG(g_dbg_lz4d_dense_seqs);
           dense_back = 0;
@@ -939,48 +1076,19 @@ DEV int lz4_decode_warp(const u8* __restrict__ in, const int csize, u8* out, con
       }
       if (nseq > 0) {
         const int match = op + my_opre + lit - off;            /* meaningful on real lanes */
-        if (__ballot_sync(FULLMASK, my_rank >= 0 && match < 0)) return LZ4D_FAIL;   /* lz4.c:2356 */
+        if (__ballot_sync(FULLMASK, my_rank >= 0 && match < 0)) { result = LZ4D_FAIL; break; }   /* lz4.c:2356 */
         LZ4D_HIT((g3 & 0x49249249u) == 0x49249249u ? LZ4D_H_BATCH_FAST : LZ4D_H_BATCH_WALK);
         LZ4D_HITL(off <= LZ4D_RING - LZ4D_BATCH_OUT - 64 && match >= ring_lo ? LZ4D_H_BATCH_RING : LZ4D_H_BATCH_GLOBAL, my_rank >= 0);
-        u32* tbl = (u32*)(ring_ptr + LZ4D_RING);               /* 11 x {info, off} then 10 start-bit words */
-        u32* smask = tbl + 24;
-        if (my_rank >= 0) {
-          tbl[2 * my_rank] = (u32)my_opre | ((u32)lit << 9) | ((u32)lane << 13);
-          tbl[2 * my_rank + 1] = (u32)off;
-          atomicOr(&smask[my_opre >> 5], 1u << (my_opre & 31));
-        }
-        __syncwarp();
-        int kbase = 0;
-        for (int r = 0; r * 32 < total; r++) {
-          const u32 w = smask[r];
-          const int y = r * 32 + lane;
-          if (y < total) {
-            const int k = kbase + __popc(w & ((2u << lane) - 1u)) - 1;
-            const u32 e0 = tbl[2 * k], offk = tbl[2 * k + 1];
-            const int opre = (int)(e0 & 511u), litk = (int)((e0 >> 9) & 15u), lanek = (int)(e0 >> 13);
-            const int j = y - opre;
-            u32 v;
-            if (j < litk) v = in[ip + lanek + 1 + j];
-            else {
-              const int src = op + opre + litk - (int)offk + (j - litk);
-              const int m0 = op + opre + litk - (int)offk;
-              if ((int)offk <= LZ4D_RING - LZ4D_BATCH_OUT - 64 && m0 >= ring_lo) v = smem_ld_u8(ring, (u32)src & LZ4D_RMASK);
-              else v = out[src];
-            }
-            out[op + y] = (u8)v;
-            smem_st_u8(ring, (u32)(op + y) & LZ4D_RMASK, v);
-          }
-          kbase += __popc(w);
-        }
-        __syncwarp();
-        if (lane < 10) smask[lane] = 0;
-        __syncwarp();
+        lz4d_batch_table(cp.batch_table(), my_rank, my_opre, lit, off);
+        cp.batch(ip, op, total, ring_lo);
         ip += consumed; op += total;
         LZ4D_DBGN(g_dbg_lz4d_batch_seqs, nseq);
         continue;
       }
     }
-    /* ---- single-sequence fast path: short sequence, source strictly before its own output ---- */
+    /* ---- single-sequence fast path: short sequence, source strictly before its own output ----
+     * Token, literals (<= 9) and offset are parsed from one 12-byte register window, and the whole
+     * sequence (<= 27 bytes) is produced by one predicated load/store step, one lane per output byte. */
     if (ip + 20 <= iend) {
       u32 b0, b1, b2;
       ldp_win12(ib, ip, b0, b1, b2);
@@ -993,18 +1101,10 @@ DEV int lz4_decode_warp(const u8* __restrict__ in, const int csize, u8* out, con
         const int off = (int)(ow & 0xffffu);
         const int match = op + lit - off;
         if (off >= total && op + total <= oend - LZ4_MFLIMIT) { /* no self-overlap; far from the end of the block */
-          if (match < 0) return LZ4D_FAIL;                     /* lz4.c:2356 (off == 0 cannot get here: off >= total >= 4) */
+          if (match < 0) { result = LZ4D_FAIL; break; }        /* lz4.c:2356 (off == 0 cannot get here: off >= total >= 4) */
           const bool use_ring = off <= LZ4D_RING - 64 && match >= ring_lo;
           LZ4D_HIT(use_ring ? LZ4D_H_SINGLE_RING : LZ4D_H_SINGLE_GLOBAL);
-          if (lane < total) {
-            u32 v;
-            if (lane < lit) v = in[ip + 1 + lane];
-            else if (use_ring) v = smem_ld_u8(ring, (u32)(match + lane - lit) & LZ4D_RMASK);
-            else v = out[match + lane - lit];
-            out[op + lane] = (u8)v;
-            smem_st_u8(ring, (u32)(op + lane) & LZ4D_RMASK, v);
-          }
-          __syncwarp();
+          cp.single(ip, op, lit, total, off, use_ring);
           ip += 3 + lit; op += total;
           LZ4D_DBG(g_dbg_lz4d_fast_seqs);
           continue;
@@ -1017,73 +1117,65 @@ DEV int lz4_decode_warp(const u8* __restrict__ in, const int csize, u8* out, con
     int len = (int)(token >> 4);
     if (len == 15) {                                          /* read_variable_length(ip, iend-15, 1) */
       u32 sb;
-      if (ip >= iend - 15) return LZ4D_FAIL;
+      if (ip >= iend - 15) { result = LZ4D_FAIL; break; }
       do {
         sb = in[ip++];
         len += (int)sb;
-        if (ip > iend - 15) return LZ4D_FAIL;
-        if (len > oend) return LZ4D_FAIL;                     /* same verdict as the cpy>oend test below, no int overflow */
+        if (ip > iend - 15) { result = LZ4D_FAIL; break; }
+        if (len > oend) { result = LZ4D_FAIL; break; }        /* same verdict as the cpy>oend test below, no int overflow */
       } while (sb == 255);
+      if (result < 0) break;
     }
     int cpy = op + len;
     const bool last = cpy > oend - LZ4_MFLIMIT || ip + len > iend - (2 + 1 + LZ4_LASTLITERALS);   /* lz4.c:2289-2331 */
-    if (last && (ip + len != iend || cpy > oend)) return LZ4D_FAIL;
-    for (int k = lane; k < len; k += 32) {                    /* literals -> output (+ ring) */
-      const u32 v = in[ip + k];
-      out[op + k] = (u8)v;
-      smem_st_u8(ring, (u32)(op + k) & LZ4D_RMASK, v);
-    }
+    if (last && (ip + len != iend || cpy > oend)) { result = LZ4D_FAIL; break; }
+    cp.literals(ip, op, len);                                 /* written even if the match turns out to be refused */
     if (len > LZ4D_RING - 64) { ring_lo = cpy - (LZ4D_RING - 64) > ring_lo ? cpy - (LZ4D_RING - 64) : ring_lo; LZ4D_HIT(LZ4D_H_GEN_LITBUMP); }
-    if (last) { LZ4D_HIT(LZ4D_H_GEN_LAST); op += len; break; }
+    if (last) { LZ4D_HIT(LZ4D_H_GEN_LAST); result = cpy; break; }
     ip += len; op = cpy;
     const int off = (int)in[ip] | ((int)in[ip + 1] << 8);
     ip += 2;
     const int match = op - off;
-    len = (int)(token & 15u);
-    if (len == 15) {                                          /* read_variable_length(ip, iend-4, 0) */
+    int mlen = (int)(token & 15u);
+    if (mlen == 15) {                                         /* read_variable_length(ip, iend-4, 0) */
       u32 sb;
       do {
         sb = in[ip++];
-        len += (int)sb;
-        if (ip > iend - LZ4_LASTLITERALS + 1) return LZ4D_FAIL;
-        if (len > oend) return LZ4D_FAIL;                     /* keeps `len` from overflowing on hostile input */
+        mlen += (int)sb;
+        if (ip > iend - LZ4_LASTLITERALS + 1) { result = LZ4D_FAIL; break; }
+        if (mlen > oend) { result = LZ4D_FAIL; break; }       /* keeps `mlen` from overflowing on hostile input */
       } while (sb == 255);
+      if (result < 0) break;
     }
-    len += 4;
-    if (match < 0) return LZ4D_FAIL;                          /* lz4.c:2356 */
-    cpy = op + len;
-    if (cpy > oend - LZ4_LASTLITERALS) return LZ4D_FAIL;      /* lz4.c:2423 */
-    __syncwarp();                                             /* earlier output must be visible to all lanes */
+    mlen += 4;
+    if (match < 0) { result = LZ4D_FAIL; break; }             /* lz4.c:2356 */
+    cpy = op + mlen;
+    if (cpy > oend - LZ4_LASTLITERALS) { result = LZ4D_FAIL; break; }   /* lz4.c:2423 */
+    int how = LZ4D_ZERO;
     if (off == 0) {
       /* not a valid stream, but LZ4_decompress_safe accepts it: every copy routine first clears the
        * destination word ("silence msan warning when offset==0", lz4.c:2386-2390; LZ4_memcpy_using_offset_base)
        * and then replicates it, so the match decodes to zeros */
+      ring_lo = cpy;
       LZ4D_HIT(LZ4D_H_GEN_OFF0);
-      for (int k = lane; k < len; k += 32) out[op + k] = 0;
-      ring_lo = cpy;
-    } else if (len <= 2048) {
-      /* sources lie before `op`; inside the ring they are not overwritten by this copy.  Far
-       * sources are read from global memory, but the output still goes into the ring so that it
-       * stays a mirror of the last 16 KiB */
-      const bool from_ring = off <= LZ4D_RING - 2048 - 64 && match >= ring_lo;
-      LZ4D_HIT(from_ring ? LZ4D_H_GEN_RING : LZ4D_H_GEN_GLOBAL);
-      for (int k0 = 0; k0 < len; k0 += 32) {
-        const int k = k0 + lane;
-        if (k < len) {
-          const int src = match + (off >= len ? k : k % off);
-          const u32 v = from_ring ? smem_ld_u8(ring, (u32)src & LZ4D_RMASK) : (u32)out[src];
-          out[op + k] = (u8)v;
-          smem_st_u8(ring, (u32)(op + k) & LZ4D_RMASK, v);
-        }
-      }
+    } else if (mlen <= 2048) {
+      how = off <= LZ4D_RING - 2048 - 64 && match >= ring_lo ? LZ4D_FROM_RING : LZ4D_FROM_GLOBAL;
+      LZ4D_HIT(how == LZ4D_FROM_RING ? LZ4D_H_GEN_RING : LZ4D_H_GEN_GLOBAL);
     } else {
-      LZ4D_HIT(LZ4D_H_GEN_LONG);
-      warp_copy_match(out, op, match, len);                   /* global sources; ring no longer mirrors this span */
+      how = LZ4D_LONG;
       ring_lo = cpy;
+      LZ4D_HIT(LZ4D_H_GEN_LONG);
     }
-    __syncwarp();
+    cp.match(op, mlen, off, how);
     op = cpy;
   }
+  cp.finish();
   __syncwarp();
-  return op;
+  return result;
+}
+
+/* one warp per stream; `ring_ptr`: LZ4D_SMEM bytes of warp-private shared memory */
+DEV int lz4_decode_warp(const u8* __restrict__ in, const int csize, u8* out, const int cap, u8* ring_ptr) {
+  Lz4dWarpCopies cp(out, ring_ptr);
+  return lz4d_walk(in, csize, cap, cp);
 }

@@ -1,17 +1,19 @@
 """The LZ4 and BloscLZ decoders (csrc/dev_lz4.cuh, dev_lz4dpair.cuh, dev_blosclz.cuh) tier by tier, on streams
 written to order.
 
-lz4_decode_warp has five tiers -- dense, lone long match, batch, single sequence, general -- each with its own entry
+The LZ4 tier walk (lz4d_walk) has five tiers -- dense, lone long match, batch, single sequence, general -- each with its own entry
 condition and its own rule for reading a match from the 16 KiB shared-memory ring that mirrors recent output or from
 global memory (offset thresholds 13696 / 15872 / 16000 / 16320 / 14272, and `ring_lo`, which moves after a literal run
-longer than 16320 bytes, after a match longer than 2048 bytes and after an offset-0 fill).  lz4_pair_parse /
-lz4_pair_copier restate all of it across two warps.  Real encoder output almost never reaches these boundaries, and a
+longer than 16320 bytes, after a match longer than 2048 bytes and after an offset-0 fill).  lz4_decode_warp runs it
+with the copies made by the same warp, lz4_pair_parse / lz4_pair_copier with the copies handed to a second warp; both
+are tested on every stream.  Real encoder output almost never reaches these boundaries, and a
 wrong threshold or a missing `ring_lo` update gives plausible wrong bytes rather than a crash.
 
 tests/lz_write.py writes blocks from explicit sequences.  Accept corpus: one scenario per tier x source x boundary,
 each decoded by emu_lz4_decode, emu_lz4_decode_pair, the oracle and (when oracle/_ref is built) LZ4_decompress_safe,
 at cap = n and n + 9 with a canary after cap; each asserts the branch ids (LZ4D_H_*) it was written to reach, in both
-decoders.  Reject corpus: one defect each, naming the LZ4D_FAIL / BLZ_FAIL line that must refuse it.  Ledgers fail if a
+decoders.  Reject corpus: one defect each, naming the LZ4D_FAIL / BLZ_FAIL line that must refuse it (in both LZ4
+decoders).  Ledgers fail if a
 fail line or a branch id goes unreached.  The reference's verdicts for the crafted corpus are pinned in
 tests/golden/reference_results.json."""
 import ctypes as C
@@ -28,8 +30,7 @@ from datagen import assert_pinned, ptr, sz
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 CSRC = os.path.join(ROOT, "c-blosc_b200", "csrc")
-SRC_WARP = os.path.join(CSRC, "dev_lz4.cuh")
-SRC_PAIR = os.path.join(CSRC, "dev_lz4dpair.cuh")
+SRC_LZ4 = os.path.join(CSRC, "dev_lz4.cuh")
 SRC_BLZ = os.path.join(CSRC, "dev_blosclz.cuh")
 CANARY = 0x77
 
@@ -50,7 +51,7 @@ def _enum_names(path, first, last):
 
 def test_branch_id_tables_match_source():
     names = []
-    text = open(SRC_WARP).read()
+    text = open(SRC_LZ4).read()
     body = text[text.index("LZ4D_H_DENSE_SHIFT = 0"):text.index("LZ4D_NHIT")]
     for line in body.split("\n"):
         line = line.split("/*")[0]
@@ -390,7 +391,7 @@ def test_lz4_accept_corpus_emu(lemu, lorc, lref, name):
 
 
 # ------------------------------------------------------------------------------------------------
-# reject corpus: one defect each, and the LZ4D_FAIL line that must catch it (in each decoder)
+# reject corpus: one defect each, and the LZ4D_FAIL line that must catch it (in both decoders)
 # ------------------------------------------------------------------------------------------------
 def fail_lines(path, macro):
     """{line number: text} of every line of `path` that uses `macro` (not its definition)"""
@@ -403,24 +404,20 @@ def line_of(path, macro, fragment):
     return hits_[0]
 
 
-# site -> (fragment in dev_lz4.cuh, fragment in dev_lz4dpair.cuh)
+# site -> fragment of its LZ4D_FAIL line in the tier walk (dev_lz4.cuh)
 SITES = {
-    "cap0": ("(csize == 1 && in[0] == 0) ? 0 : LZ4D_FAIL", "(csize == 1 && in[0] == 0) ? 0 : LZ4D_FAIL"),
-    "csize0": ("if (csize == 0) return LZ4D_FAIL", "if (csize == 0) return LZ4D_FAIL"),
-    "batch_match": ("my_rank >= 0 && match < 0)) return LZ4D_FAIL", "my_rank >= 0 && match < 0)) { result = LZ4D_FAIL"),
-    "single_match": ("if (match < 0) return LZ4D_FAIL;                     /* lz4.c:2356 (off",
-                     "if (match < 0) { result = LZ4D_FAIL; break; }       /* lz4.c:2356 */"),
-    "litlen_start": ("if (ip >= iend - 15) return LZ4D_FAIL", "if (ip >= iend - 15) { result = LZ4D_FAIL"),
-    "litlen_bytes": ("if (ip > iend - 15) return LZ4D_FAIL", "if (ip > iend - 15) { result = LZ4D_FAIL"),
-    "litlen_oend": ("if (len > oend) return LZ4D_FAIL;                     /* same", "if (len > oend) { result = LZ4D_FAIL"),
-    "last": ("if (last && (ip + len != iend || cpy > oend)) return LZ4D_FAIL",
-             "if (last && (ip + len != iend || cpy > oend)) { result = LZ4D_FAIL"),
-    "mlen_bytes": ("if (ip > iend - LZ4_LASTLITERALS + 1) return LZ4D_FAIL",
-                   "if (ip > iend - LZ4_LASTLITERALS + 1) { result = LZ4D_FAIL"),
-    "mlen_oend": ("if (len > oend) return LZ4D_FAIL;                     /* keeps", "if (mlen > oend) { result = LZ4D_FAIL"),
-    "general_match": ("if (match < 0) return LZ4D_FAIL;                          /* lz4.c:2356 */",
-                      "if (match < 0) { ok = false; LZ4D_FAIL_NOTE(); }"),
-    "match_oend": ("if (cpy > oend - LZ4_LASTLITERALS) return LZ4D_FAIL", "cpy > oend - LZ4_LASTLITERALS) { ok = false"),
+    "cap0": "(csize == 1 && in[0] == 0) ? 0 : LZ4D_FAIL",
+    "csize0": "if (csize == 0) return LZ4D_FAIL",
+    "batch_match": "my_rank >= 0 && match < 0)) { result = LZ4D_FAIL",
+    "single_match": "if (match < 0) { result = LZ4D_FAIL; break; }        /* lz4.c:2356 (off",
+    "litlen_start": "if (ip >= iend - 15) { result = LZ4D_FAIL",
+    "litlen_bytes": "if (ip > iend - 15) { result = LZ4D_FAIL",
+    "litlen_oend": "if (len > oend) { result = LZ4D_FAIL",
+    "last": "if (last && (ip + len != iend || cpy > oend)) { result = LZ4D_FAIL",
+    "mlen_bytes": "if (ip > iend - LZ4_LASTLITERALS + 1) { result = LZ4D_FAIL",
+    "mlen_oend": "if (mlen > oend) { result = LZ4D_FAIL",
+    "general_match": "if (match < 0) { result = LZ4D_FAIL; break; }             /* lz4.c:2356 */",
+    "match_oend": "if (cpy > oend - LZ4_LASTLITERALS) { result = LZ4D_FAIL; break; }",
 }
 REJECT = {}           # name -> (block, cap, site)
 
@@ -472,12 +469,13 @@ _build_reject()
 
 
 @pytest.mark.parametrize("name", sorted(REJECT))
-def test_lz4_reject_corpus_emu(lemu, lorc, lref, name):
+def test_lz4_reject_corpus_one_fail_line_emu(lemu, lorc, lref, name):
+    """each defect is refused at its named line of the tier walk, by the single warp and by the pair alike"""
     blk, cap, site = REJECT[name]
     got, l1, l2, _, _ = lz4_all(lemu, lorc, lref, blk, cap)
     assert got is None
-    assert l1 == line_of(SRC_WARP, "LZ4D_FAIL", SITES[site][0]), (l1, fail_lines(SRC_WARP, "LZ4D_FAIL").get(l1))
-    assert l2 == line_of(SRC_PAIR, "LZ4D_FAIL", SITES[site][1]), (l2, fail_lines(SRC_PAIR, "LZ4D_FAIL").get(l2))
+    assert l1 == l2, ("warp and pair refuse at different lines", l1, l2)
+    assert l1 == line_of(SRC_LZ4, "LZ4D_FAIL", SITES[site]), (l1, fail_lines(SRC_LZ4, "LZ4D_FAIL").get(l1))
 
 
 # ------------------------------------------------------------------------------------------------
@@ -617,17 +615,16 @@ def _damaged(blk, rng, k):
     return bytes(b)
 
 
-def test_lz4_ledger(lemu, lorc, lref):
-    reached_w = {line_of(SRC_WARP, "LZ4D_FAIL", SITES[s][0]) for _, _, s in REJECT.values()}
-    reached_p = {line_of(SRC_PAIR, "LZ4D_FAIL", SITES[s][1]) for _, _, s in REJECT.values()}
+def test_lz4_ledger_one_walk(lemu, lorc, lref):
+    """every LZ4D_FAIL line of the tier walk is named by a reject scenario, and every branch id is reached"""
+    reached = {line_of(SRC_LZ4, "LZ4D_FAIL", SITES[s]) for _, _, s in REJECT.values()}
     seen = set()
     for blk, content, caps, _, _ in ACCEPT.values():
         for cap in caps or (len(content),):
             _, _, _, h1, h2 = lz4_all(lemu, lorc, lref, blk, cap)
             seen |= h1 | h2
-    missing_w = {k: t.strip() for k, t in fail_lines(SRC_WARP, "LZ4D_FAIL").items() if k not in reached_w}
-    missing_p = {k: t.strip() for k, t in fail_lines(SRC_PAIR, "LZ4D_FAIL").items() if k not in reached_p}
-    assert not missing_w and not missing_p, (missing_w, missing_p)
+    missing = {k: t.strip() for k, t in fail_lines(SRC_LZ4, "LZ4D_FAIL").items() if k not in reached}
+    assert not missing, missing
     assert set(H) - seen == set(LZ4_UNREACHED_HITS), sorted(set(H) - seen)
 
 
