@@ -11,7 +11,7 @@ extern "C" {
 #endif
 
 enum { FILT_SHUFFLE = 0, FILT_UNSHUFFLE = 1, FILT_BITSHUFFLE = 2, FILT_BITUNSHUFFLE = 3 };
-enum { B2_CODEC_BLOSCLZ = 0, B2_CODEC_LZ4 = 1, B2_CODEC_ZLIB = 2 /* decode only */, B2_CODEC_ZSTD = 3 };
+enum { B2_CODEC_BLOSCLZ = 0, B2_CODEC_LZ4 = 1, B2_CODEC_ZLIB = 2, B2_CODEC_ZSTD = 3 };
 
 typedef struct FilterArgs {
   const uint8_t* src;
@@ -114,6 +114,10 @@ typedef struct FastArgs {
   int zstd;
   uint32_t* recs;                  /* 64 records per segment, segment-major as segs */
   uint32_t* nrec;                  /* records per segment */
+  /* DEFLATE encoder (dev_deflate.cuh): the zstd encoder's records, offsets <= 32768, then one warp per stream writes
+   * its zlib stream (zstd is 0) */
+  int deflate;
+  int flevel;                      /* zlib's FLEVEL for the clevel (deflate.c), in the stream header */
 } FastArgs;
 
 typedef struct CompactArgs {

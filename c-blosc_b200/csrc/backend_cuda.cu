@@ -62,6 +62,8 @@ extern "C" int b2_device_prepare(void) {
   CK(cudaFuncSetAttribute(parse_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, B2_FAST_WIN_MAX + 64));
   CK(cudaFuncSetAttribute(zparse_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, B2_FAST_WIN_MAX + 64));
   CK(cudaFuncSetAttribute(zenc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, ZE_WARPS * ZE_SMEM_BYTES));
+  CK(cudaFuncSetAttribute(dparse_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, B2_FAST_WIN_MAX + 64));
+  CK(cudaFuncSetAttribute(denc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, DZ_WARPS * DZ_SMEM_BYTES));
   CK(cudaFuncSetAttribute(filter_kernel<0>, cudaFuncAttributeMaxDynamicSharedMemorySize, FILT_WARPS * 16 * FILT_TILE));
   CK(cudaFuncSetAttribute(filter_kernel<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, FILT_WARPS * 16 * FILT_TILE));
   CK(cudaFuncSetAttribute(filter_kernel<4>, cudaFuncAttributeMaxDynamicSharedMemorySize, FILT_WARPS * 16 * FILT_TILE));
@@ -236,7 +238,8 @@ extern "C" int b2_launch_encode(const EncodeArgs* a, b2_stream_t s) {
 }
 
 /* segment-parallel LZ4: the hash-chain index of every stream, then one lane per segment; a->zstd: the same index and
- * parse into zstd sequence records, then one warp per zstd frame (dev_zstdenc.cuh) */
+ * parse into zstd sequence records, then one warp per zstd frame (dev_zstdenc.cuh); a->deflate: the same records with
+ * offsets <= 32768, then one warp per zlib stream (dev_deflate.cuh) */
 extern "C" int b2_launch_fast(const FastArgs* a, b2_stream_t s) {
   if (a->map.nstreams <= 0) return 0;
   {
@@ -259,7 +262,8 @@ extern "C" int b2_launch_fast(const FastArgs* a, b2_stream_t s) {
     FastArgs args = *a;
     args.queue_base = *a->queue_base_host;
     *a->queue_base_host += (unsigned)njobs + (unsigned)ctas;      /* one ticket-drawing thread per CTA */
-    if (a->zstd) zparse_kernel<<<(unsigned)ctas, threads, smem, s->s>>>(args);
+    if (a->deflate) dparse_kernel<<<(unsigned)ctas, threads, smem, s->s>>>(args);
+    else if (a->zstd) zparse_kernel<<<(unsigned)ctas, threads, smem, s->s>>>(args);
     else parse_kernel<<<(unsigned)ctas, threads, smem, s->s>>>(args);
     CK(cudaGetLastError());
   }
@@ -267,6 +271,13 @@ extern "C" int b2_launch_fast(const FastArgs* a, b2_stream_t s) {
     const int ctas = (a->map.nstreams + ZE_WARPS - 1) / ZE_WARPS;
     ProfScope ps(B2_K_ZENC, s->s);
     zenc_kernel<<<ctas, ZE_WARPS * 32, ZE_WARPS * ZE_SMEM_BYTES, s->s>>>(*a);
+    CK(cudaGetLastError());
+    return 0;
+  }
+  if (a->deflate) {                                               /* one warp per zlib stream */
+    const int ctas = (a->map.nstreams + DZ_WARPS - 1) / DZ_WARPS;
+    ProfScope ps(B2_K_DENC, s->s);
+    denc_kernel<<<ctas, DZ_WARPS * 32, DZ_WARPS * DZ_SMEM_BYTES, s->s>>>(*a);
     CK(cudaGetLastError());
     return 0;
   }

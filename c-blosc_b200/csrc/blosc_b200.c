@@ -287,12 +287,20 @@ static int zstd_enabled(void) {
   return e && *e && atoi(e) != 0;
 }
 
+/* BLOSC_B200_ZLIB=1 (read on every call, independent of the zstd switch) does the same for zlib: "zlib" chunks are
+ * then written (dev_deflate.cuh).  Unset, it is a reference built with -DDEACTIVATE_ZLIB, which still reads them. */
+static int zlib_enabled(void) {
+  const char* e = getenv("BLOSC_B200_ZLIB");
+  return e && *e && atoi(e) != 0;
+}
+
 int blosc_compcode_to_compname(int compcode, const char** compname) {    /* blosc.c:329-374 */
   static const char* names[6] = {BLOSC_BLOSCLZ_COMPNAME, BLOSC_LZ4_COMPNAME, BLOSC_LZ4HC_COMPNAME,
                                  BLOSC_SNAPPY_COMPNAME, BLOSC_ZLIB_COMPNAME, BLOSC_ZSTD_COMPNAME};
   *compname = (compcode >= 0 && compcode < 6) ? names[compcode] : NULL;
   /* codecs this build can ENCODE; like a reference built without the others */
   if (compcode == BLOSC_BLOSCLZ || compcode == BLOSC_LZ4 || compcode == BLOSC_LZ4HC) return compcode;
+  if (compcode == BLOSC_ZLIB && zlib_enabled()) return compcode;
   if (compcode == BLOSC_ZSTD && zstd_enabled()) return compcode;
   return -1;
 }
@@ -301,12 +309,16 @@ int blosc_compname_to_compcode(const char* compname) {                    /* blo
   if (strcmp(compname, BLOSC_BLOSCLZ_COMPNAME) == 0) return BLOSC_BLOSCLZ;
   if (strcmp(compname, BLOSC_LZ4_COMPNAME) == 0) return BLOSC_LZ4;
   if (strcmp(compname, BLOSC_LZ4HC_COMPNAME) == 0) return BLOSC_LZ4HC;
+  if (strcmp(compname, BLOSC_ZLIB_COMPNAME) == 0 && zlib_enabled()) return BLOSC_ZLIB;
   if (strcmp(compname, BLOSC_ZSTD_COMPNAME) == 0 && zstd_enabled()) return BLOSC_ZSTD;
   return -1;
 }
 
-const char* blosc_list_compressors(void) {                                  /* blosc.c:2033-2056 */
-  if (zstd_enabled()) return BLOSC_BLOSCLZ_COMPNAME "," BLOSC_LZ4_COMPNAME "," BLOSC_LZ4HC_COMPNAME "," BLOSC_ZSTD_COMPNAME;
+const char* blosc_list_compressors(void) {                                  /* blosc.c:2029-2042 */
+  const int zl = zlib_enabled(), zs = zstd_enabled();
+  if (zl && zs) return BLOSC_BLOSCLZ_COMPNAME "," BLOSC_LZ4_COMPNAME "," BLOSC_LZ4HC_COMPNAME "," BLOSC_ZLIB_COMPNAME "," BLOSC_ZSTD_COMPNAME;
+  if (zl) return BLOSC_BLOSCLZ_COMPNAME "," BLOSC_LZ4_COMPNAME "," BLOSC_LZ4HC_COMPNAME "," BLOSC_ZLIB_COMPNAME;
+  if (zs) return BLOSC_BLOSCLZ_COMPNAME "," BLOSC_LZ4_COMPNAME "," BLOSC_LZ4HC_COMPNAME "," BLOSC_ZSTD_COMPNAME;
   return BLOSC_BLOSCLZ_COMPNAME "," BLOSC_LZ4_COMPNAME "," BLOSC_LZ4HC_COMPNAME;
 }
 const char* blosc_get_version_string(void) { return BLOSC_VERSION_STRING; }
@@ -317,6 +329,8 @@ int blosc_get_complib_info(const char* compname, char** complib, char** version)
   if (strcmp(compname, BLOSC_BLOSCLZ_COMPNAME) == 0) { code = BLOSC_BLOSCLZ_LIB; lib = "BloscLZ"; ver = "2.5.1"; }
   else if (strcmp(compname, BLOSC_LZ4_COMPNAME) == 0 || strcmp(compname, BLOSC_LZ4HC_COMPNAME) == 0) {
     code = BLOSC_LZ4_LIB; lib = "LZ4"; ver = "1.10.0";
+  } else if (strcmp(compname, BLOSC_ZLIB_COMPNAME) == 0 && zlib_enabled()) {
+    code = BLOSC_ZLIB_LIB; lib = "Zlib"; ver = "1.3.1";          /* the zlib release the streams are checked against */
   } else if (strcmp(compname, BLOSC_ZSTD_COMPNAME) == 0 && zstd_enabled()) {
     code = BLOSC_ZSTD_LIB; lib = "Zstd"; ver = "1.5.6";         /* the zstd release the frames are checked against */
   }
@@ -589,6 +603,7 @@ static int compress_impl(int clevel, int doshuffle, size_t typesize, size_t nbyt
   if (compcode == BLOSC_BLOSCLZ) compformat = BLOSC_BLOSCLZ_FORMAT;
   else if (compcode == BLOSC_LZ4) compformat = BLOSC_LZ4_FORMAT;
   else if (compcode == BLOSC_LZ4HC) compformat = BLOSC_LZ4HC_FORMAT;     /* blosc.c:1170-1172: the LZ4 format */
+  else if (compcode == BLOSC_ZLIB) compformat = BLOSC_ZLIB_FORMAT;       /* blosc.c:1183-1188 */
   else if (compcode == BLOSC_ZSTD) compformat = BLOSC_ZSTD_FORMAT;       /* blosc.c:1190-1196 */
   else {
     fprintf(stderr, "Blosc has not been compiled with '%s' ", compressor ? compressor : "(null)");
@@ -672,9 +687,10 @@ static int compress_impl(int clevel, int doshuffle, size_t typesize, size_t nbyt
     ea.scan = sa;
     launched = 1;
     memset(&ca, 0, sizeof ca);
-    if (compcode == BLOSC_ZSTD) {
+    if (compcode == BLOSC_ZSTD || compcode == BLOSC_ZLIB) {
       /* the zstd encoder (dev_zstdenc.cuh): the index and windows of the segment-parallel parse, sequence records
-       * instead of LZ4 bytes, then one warp per zstd frame */
+       * instead of LZ4 bytes, then one warp per zstd frame.  The DEFLATE encoder (dev_deflate.cuh) shares the parse,
+       * with offsets <= 32768, then one warp writes each zlib stream. */
       FastArgs fx;
       const int neblock = bs / nsplits;
       const int longest = neblock > leftover ? neblock : leftover;
@@ -697,7 +713,10 @@ static int compress_impl(int clevel, int doshuffle, size_t typesize, size_t nbyt
       if (buf_ensure(&w->prev, 2 * (size_t)nb + 64)) break;
       if (buf_ensure(recs, (size_t)nsegs * B2_FAST_SEG + 64)) break;
       if (buf_ensure(&w->segs, (size_t)nsegs * 4 + 64)) break;
-      fx.prev = (uint16_t*)w->prev.p; fx.zstd = 1; fx.recs = (uint32_t*)recs->p; fx.nrec = (uint32_t*)w->segs.p;
+      fx.zstd = compcode == BLOSC_ZSTD; fx.deflate = compcode == BLOSC_ZLIB;
+      /* zlib's FLEVEL for compress2(.., clevel) (blosc.c:472-483, deflate.c) */
+      fx.flevel = clevel < 2 ? 0 : (clevel < 6 ? 1 : (clevel == 6 ? 2 : 3));
+      fx.prev = (uint16_t*)w->prev.p; fx.recs = (uint32_t*)recs->p; fx.nrec = (uint32_t*)w->segs.p;
       fx.queue = ea.queue; fx.queue_base_host = ea.queue_base_host; fx.done = ea.done;
       fx.fold_scan = ea.fold_scan; fx.scan = sa;
       if (b2_launch_fast(&fx, w->stream)) break;

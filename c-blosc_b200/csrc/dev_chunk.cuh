@@ -22,6 +22,7 @@
 #include "dev_lz4dpair.cuh"
 #include "dev_zstd.cuh"
 #include "dev_zstdenc.cuh"
+#include "dev_deflate.cuh"
 
 
 
@@ -244,8 +245,9 @@ __global__ void __launch_bounds__(INDEX_WARPS * 32) index_kernel(FastArgs a) {
 /* One CTA per window of a stream (at most B2_FAST_WIN_MAX bytes): the window's bytes are staged in shared memory, then every THREAD parses one segment of FAST_SEG bytes.
  * Candidate compares -- the random accesses of LZ matching -- hit shared memory; only the chain links (prev[]) and
  * candidates in front of the window come from L2. */
-/* ZSTD: the same windows and segments, parsed into zstd sequence records (dev_zstdenc.cuh) instead of LZ4 bytes */
-template <bool ZSTD>
+/* ZSTD: the same windows and segments, parsed into zstd sequence records (dev_zstdenc.cuh) instead of LZ4 bytes, with
+ * offsets <= MAXD (DZ_MAXD: the DEFLATE encoder, dev_deflate.cuh) */
+template <bool ZSTD, int MAXD = 65535>
 DEV void fast_parse_body(const FastArgs& a, u8* smem) {
   u32* sdata = (u32*)smem;
   int* sjob = (int*)(smem + a.win_bytes + 48);
@@ -303,7 +305,7 @@ DEV void fast_parse_body(const FastArgs& a, u8* smem) {
       const int sa = k * FAST_SEG, sb = sa + FAST_SEG < len ? sa + FAST_SEG : len;
       if (ZSTD) {
         const long long gk = (long long)idx * a.segs_full + k;
-        a.nrec[gk] = (u32)zse_parse_lane(v, len, a.prev + off, sa, sb, a.recs + gk * ZE_SEG_RECS, a.depth, a.lazy);
+        a.nrec[gk] = (u32)zse_parse_lane<MAXD>(v, len, a.prev + off, sa, sb, a.recs + gk * ZE_SEG_RECS, a.depth, a.lazy);
       } else {
         lz4f_parse_lane(v, len, a.prev + off, sa, sb, a.slots + off + sa, &segs[k], a.depth, a.accel, a.lazy);
       }
@@ -316,6 +318,7 @@ __global__ void __launch_bounds__(B2_FAST_WIN_MAX / FAST_SEG, 3) parse_kernel(Fa
 #ifdef SIMT_EMU
   u8* smem = simt::g_dynsmem;
   if (a.zstd) { fast_parse_body<true>(a, smem); return; }     /* the emulator launches the zstd parse under this name */
+  if (a.deflate) { fast_parse_body<true, DZ_MAXD>(a, smem); return; }   /* and the DEFLATE parse */
 #else
   extern __shared__ __align__(16) u8 smem[];
 #endif
@@ -332,15 +335,31 @@ __global__ void __launch_bounds__(B2_FAST_WIN_MAX / FAST_SEG, 3) zparse_kernel(F
   fast_parse_body<true>(a, smem);
 }
 
+/* FastArgs.deflate: the DEFLATE encoder's parse, offsets <= 32768 (the backend launches it instead of parse_kernel) */
+__global__ void __launch_bounds__(B2_FAST_WIN_MAX / FAST_SEG, 3) dparse_kernel(FastArgs a) {
+#ifdef SIMT_EMU
+  u8* smem = simt::g_dynsmem;
+#else
+  extern __shared__ __align__(16) u8 smem[];
+#endif
+  fast_parse_body<true, DZ_MAXD>(a, smem);
+}
+
 /* One warp per stream: scan of its segment records (pending literals, continued matches, output offsets, compressed
  * size); the warp that finishes the last stream runs the block scan, exactly as in encode_kernel. */
 #define FSCAN_WARPS 4
 DEV void zenc_body(const FastArgs& a, ZeSm* S);
+DEV void denc_body(const FastArgs& a, DzSm* S);
 __global__ void __launch_bounds__(FSCAN_WARPS * 32) fscan_kernel(FastArgs a) {
 #ifdef SIMT_EMU
   if (a.zstd) {                                    /* the emulator launches the zstd entropy stage under this name */
     __shared__ ZeSm ztab[FSCAN_WARPS];
     zenc_body(a, &ztab[threadIdx.x >> 5]);
+    return;
+  }
+  if (a.deflate) {                                 /* and the DEFLATE one */
+    __shared__ DzSm dtab[FSCAN_WARPS];
+    denc_body(a, &dtab[threadIdx.x >> 5]);
     return;
   }
 #endif
@@ -372,6 +391,7 @@ __global__ void __launch_bounds__(FSCAN_WARPS * 32) fscan_kernel(FastArgs a) {
 
 
 /* ---- segment-parallel zstd (dev_zstdenc.cuh): index_kernel, zparse_kernel, then one warp per frame ---- */
+DEV void fast_streams_done(const FastArgs& a, const int mine);
 DEV void zenc_body(const FastArgs& a, ZeSm* S) {
   const int lane = lane_id(), warp = (int)(threadIdx.x >> 5), nwarps = (int)(blockDim.x >> 5);
   int mine = 0;
@@ -389,7 +409,12 @@ DEV void zenc_body(const FastArgs& a, ZeSm* S) {
     mine++;
     __syncwarp();
   }
-  /* whoever completes the stream count does the block scan, exactly as in encode_kernel */
+  fast_streams_done(a, mine);
+}
+
+/* whoever completes the stream count does the block scan, exactly as in encode_kernel */
+DEV void fast_streams_done(const FastArgs& a, const int mine) {
+  const int lane = lane_id();
   if (mine == 0) return;
   __threadfence();
   int last = 0;
@@ -410,6 +435,34 @@ __global__ void __launch_bounds__(ZE_WARPS * 32) zenc_kernel(FastArgs a) {
   extern __shared__ __align__(16) u8 smem[];
 #endif
   zenc_body(a, (ZeSm*)(smem + (size_t)(threadIdx.x >> 5) * ZE_SMEM_BYTES));
+}
+
+/* ---- segment-parallel DEFLATE (dev_deflate.cuh): index_kernel, dparse_kernel, then one warp per zlib stream ---- */
+DEV void denc_body(const FastArgs& a, DzSm* S) {
+  const int lane = lane_id(), warp = (int)(threadIdx.x >> 5), nwarps = (int)(blockDim.x >> 5);
+  int mine = 0;
+  for (int idx = (int)blockIdx.x * nwarps + warp; idx < a.map.nstreams; idx += (int)gridDim.x * nwarps) {
+    int block, len, split;
+    long long off;
+    stream_locate(a.map, idx, &block, &off, &len, &split);
+    const long long gseg = (long long)idx * a.segs_full;
+    int c = dz_stream(*S, a.in + off, len, a.recs + gseg * ZE_SEG_RECS, a.nrec + gseg, (u8*)(a.prev + off), a.slots + off, a.flevel);
+    if (c >= len) c = len;                         /* blosc.c:705-714: incompressible split is stored raw */
+    if (lane == 0) { a.csizes[idx] = c; a.needs[idx] = c; }
+    mine++;
+    __syncwarp();
+  }
+  fast_streams_done(a, mine);
+}
+
+/* One warp per stream: its zlib stream; the tables and the bit window live in the warp's DZ_SMEM_BYTES */
+__global__ void __launch_bounds__(DZ_WARPS * 32) denc_kernel(FastArgs a) {
+#ifdef SIMT_EMU
+  u8* smem = simt::g_dynsmem;
+#else
+  extern __shared__ __align__(16) u8 smem[];
+#endif
+  denc_body(a, (DzSm*)(smem + (size_t)(threadIdx.x >> 5) * DZ_SMEM_BYTES));
 }
 
 

@@ -231,7 +231,8 @@ DEV int fast_count(const FastView& v, int p, int q, int lim) {
 DEV int fast_lit_ext(int lit) { return lit >= 15 ? 1 + (lit - 15) / 255 : 0; }
 
 /* Longest match for position ip among: the offset `rep`, the offsets 1..4, and up to `de` candidates of the hash
- * chain.  Returns its length (0: none) and *off. */
+ * chain no farther than MAXD (DEFLATE's window is 32768).  Returns its length (0: none) and *off. */
+template <int MAXD = 65535>
 DEV int lz4f_search(const FastView& v, const u16* __restrict__ prev, const int ip, const int mlim, const int rep, const int rep_len,
                     const int de, int* off) {
   const u32 wip = fast_ld32(v, ip);
@@ -247,7 +248,7 @@ DEV int lz4f_search(const FastView& v, const u16* __restrict__ prev, const int i
       const int dl = (int)prev[q];
       if (dl == 0) break;
       q -= dl;
-      if (ip - q > 65535) break;
+      if (ip - q > MAXD) break;
       /* a candidate can only win if it also matches where the best match so far ends (the LZ4HC test,
        * lz4hc.c LZ4HC_InsertAndGetWiderMatch): most candidates are turned down by this one compare */
       if (best >= 4 && fast_ld32(v, q + best - 3) != wend) continue;

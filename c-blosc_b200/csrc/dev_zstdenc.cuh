@@ -33,7 +33,9 @@
 
 /* ---- zparse: one lane, one segment [a, b) of the stream ----
  * record = literal length (8 bits, from the end of the previous match or the segment start) | (match length - 4) << 8
- * | offset << 16.  Returns the number of records. */
+ * | offset << 16, offsets <= MAXD (the DEFLATE encoder, dev_deflate.cuh, parses with 32768).  Returns the number of
+ * records. */
+template <int MAXD = 65535>
 DEV int zse_parse_lane(const FastView& v, const int n, const u16* __restrict__ prev, const int a, const int b,
                        u32* __restrict__ rec, const int depth, const int lazy) {
   const int mlim = b < n ? b : n, mfl = mlim - 4;    /* a match lies inside the segment and has >= 4 bytes */
@@ -48,7 +50,7 @@ DEV int zse_parse_lane(const FastView& v, const int n, const u16* __restrict__ p
       if (dl == 0) break;
       q -= dl;
       const int o = a - 1 - q;
-      if (o > 65535) break;
+      if (o > MAXD) break;
       if (fast_ld32(v, a - o) == wa) {
         const int len = 4 + fast_count(v, a + 4, a - o + 4, mlim - (a + 4));
         if (len > bl) { bl = len; rep = o; }
@@ -64,10 +66,10 @@ DEV int zse_parse_lane(const FastView& v, const int n, const u16* __restrict__ p
     nsearch++;
     if (de < 2) de = 2;
     int boff = 0;
-    int best = lz4f_search(v, prev, ip, mlim, rep, ip == a ? pre : 0, de, &boff);
+    int best = lz4f_search<MAXD>(v, prev, ip, mlim, rep, ip == a ? pre : 0, de, &boff);
     if (best >= 4 && best < lazy && ip + 1 <= mfl) {
       int boff2 = 0;
-      const int best2 = lz4f_search(v, prev, ip + 1, mlim, rep, 0, de, &boff2);
+      const int best2 = lz4f_search<MAXD>(v, prev, ip + 1, mlim, rep, 0, de, &boff2);
       if (best2 > best + 1) { ip++; best = best2; boff = boff2; }
     }
     if (best >= 4 && ip + best <= mlim) {
@@ -285,54 +287,64 @@ DEV long long ze_cost(const u32* cnt, int nsym, const short* norm, int nnorm, in
   return c;
 }
 
-/* ---- Huffman code lengths <= 11 for the present literals; returns the longest code (0: fewer than two symbols) ---- */
-DEV int ze_huf_lengths(ZeSm& S) {
+/* ---- length-limited Huffman code lengths, shared with the DEFLATE encoder (dev_deflate.cuh) ----
+ * hist[0, nsym) -> len[0, nsym), every length <= maxlen and the code complete (Kraft sum exactly 1).  Scratch: leaf[nsym]
+ * (the present symbols by ascending count, then symbol), nc / par[2 nsym].  Returns the number of present symbols; when
+ * that is below 2 nothing is written to len. */
+DEV int huf_limited_lengths(const u32* hist, const int nsym, const int maxlen, u16* leaf, u32* nc, u16* par, u8* len) {
   int n = 0;
-  for (int s = 0; s < 256; s++) if (S.hist[s]) S.leaf[n++] = (u16)s;
-  if (n < 2) return 0;
+  for (int s = 0; s < nsym; s++) if (hist[s]) leaf[n++] = (u16)s;
+  if (n < 2) return n;
   for (int i = 1; i < n; i++) {                     /* by count, then symbol: ascending */
-    const u16 x = S.leaf[i];
+    const u16 x = leaf[i];
     int j = i - 1;
-    while (j >= 0 && S.hist[S.leaf[j]] > S.hist[x]) { S.leaf[j + 1] = S.leaf[j]; j--; }
-    S.leaf[j + 1] = x;
+    while (j >= 0 && hist[leaf[j]] > hist[x]) { leaf[j + 1] = leaf[j]; j--; }
+    leaf[j + 1] = x;
   }
   /* two-queue Huffman: leaves 0..n-1, internal nodes n..2n-2 (created in non-decreasing weight order) */
-  for (int i = 0; i < n; i++) S.nc[i] = S.hist[S.leaf[i]];
+  for (int i = 0; i < n; i++) nc[i] = hist[leaf[i]];
   int li = 0, ni = n, nn = n;
   for (int k = 0; k < n - 1; k++) {
     int pick[2];
     for (int t = 0; t < 2; t++) {
-      if (li < n && (ni >= nn || S.nc[li] <= S.nc[ni])) pick[t] = li++;
+      if (li < n && (ni >= nn || nc[li] <= nc[ni])) pick[t] = li++;
       else pick[t] = ni++;
     }
-    S.nc[nn] = S.nc[pick[0]] + S.nc[pick[1]];
-    S.par[pick[0]] = (u16)nn; S.par[pick[1]] = (u16)nn;
+    nc[nn] = nc[pick[0]] + nc[pick[1]];
+    par[pick[0]] = (u16)nn; par[pick[1]] = (u16)nn;
     nn++;
   }
   /* depths, root (nn-1) first: reuse nc[] for them */
-  S.nc[nn - 1] = 0;
-  for (int k = nn - 2; k >= 0; k--) S.nc[k] = S.nc[S.par[k]] + 1;
-  for (int s = 0; s < 256; s++) S.hlen[s] = 0;
-  int kraft = 0;                                     /* sum of 2^(11 - len) */
+  nc[nn - 1] = 0;
+  for (int k = nn - 2; k >= 0; k--) nc[k] = nc[par[k]] + 1;
+  for (int s = 0; s < nsym; s++) len[s] = 0;
+  int kraft = 0;                                     /* sum of 2^(maxlen - len) */
   for (int i = 0; i < n; i++) {
-    int l = (int)S.nc[i];
-    if (l > ZS_HUFLOG) l = ZS_HUFLOG;
-    S.hlen[S.leaf[i]] = (u8)l;
-    kraft += 1 << (ZS_HUFLOG - l);
+    int l = (int)nc[i];
+    if (l > maxlen) l = maxlen;
+    len[leaf[i]] = (u8)l;
+    kraft += 1 << (maxlen - l);
   }
-  while (kraft > (1 << ZS_HUFLOG)) {                 /* too many codes after the clamp: lengthen the rarest */
-    for (int i = 0; i < n && kraft > (1 << ZS_HUFLOG); i++) {
-      const int s = S.leaf[i];
-      if (S.hlen[s] < ZS_HUFLOG) { kraft -= 1 << (ZS_HUFLOG - 1 - S.hlen[s]); S.hlen[s]++; }
+  while (kraft > (1 << maxlen)) {                    /* too many codes after the clamp: lengthen the rarest */
+    for (int i = 0; i < n && kraft > (1 << maxlen); i++) {
+      const int s = leaf[i];
+      if (len[s] < maxlen) { kraft -= 1 << (maxlen - 1 - len[s]); len[s]++; }
     }
   }
-  while (kraft < (1 << ZS_HUFLOG)) {                 /* room left: shorten the most frequent that fit */
-    for (int i = n - 1; i >= 0 && kraft < (1 << ZS_HUFLOG); i--) {
-      const int s = S.leaf[i];
-      const int add = 1 << (ZS_HUFLOG - S.hlen[s]);
-      if (S.hlen[s] > 1 && add <= (1 << ZS_HUFLOG) - kraft) { kraft += add; S.hlen[s]--; }
+  while (kraft < (1 << maxlen)) {                    /* room left: shorten the most frequent that fit */
+    for (int i = n - 1; i >= 0 && kraft < (1 << maxlen); i--) {
+      const int s = leaf[i];
+      const int add = 1 << (maxlen - len[s]);
+      if (len[s] > 1 && add <= (1 << maxlen) - kraft) { kraft += add; len[s]--; }
     }
   }
+  return n;
+}
+
+/* ---- Huffman code lengths <= 11 for the present literals; returns the longest code (0: fewer than two symbols) ---- */
+DEV int ze_huf_lengths(ZeSm& S) {
+  const int n = huf_limited_lengths(S.hist, 256, ZS_HUFLOG, S.leaf, S.nc, S.par, S.hlen);
+  if (n < 2) return 0;
   int maxb = 0;
   for (int i = 0; i < n; i++) if (S.hlen[S.leaf[i]] > maxb) maxb = S.hlen[S.leaf[i]];
   /* canonical codes in the decoder's order (zs_huf_table): longer codes first, within a length by symbol */

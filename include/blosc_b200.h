@@ -22,6 +22,10 @@
  *     like a reference built with zstd: "zstd" is listed, named and encoded (segment-parallel GPU
  *     encoder, one zstd frame per block).  The header is the reference's and every reference build
  *     with zstd decodes the chunks, but the frames are not ZSTD_compress's bytes;
+ *   - with BLOSC_B200_ZLIB=1 (read on every call, independent of BLOSC_B200_ZSTD) it behaves like a
+ *     reference built with zlib: "zlib" is listed, named and encoded (segment-parallel GPU encoder,
+ *     one zlib stream per split).  Every zlib reads the streams, but they are not compress2's bytes
+ *     and their sizes differ;
  *   - there is no CPU codec: without a CUDA device every compress/decompress call
  *     prints a message on stderr and returns -1.
  */
