@@ -196,9 +196,9 @@ extern "C" int b2_launch_filter(const FilterArgs* a, b2_stream_t s) {
 
 /* LZ4 with the plain 16 KiB table can run in team mode (one CTA of four warps per stream).  It shortens the
  * critical path of a hard stream but keeps fewer streams in flight, so it pays when most streams of a block are
- * cheap and one is hard -- measured on an H100 on the bench.c planes: encode 4.53 -> 4.17 ms at typesize 4 (one
- * hard byte-plane of four), but 5.24 -> 9.83 ms at typesize 2 (both planes hard), 1.42 -> 2.03 ms at typesize 8 and
- * 1.26 -> 2.62 ms at typesize 16.  Default: blocks of four splits when the
+ * cheap and one is hard -- measured on an H100 (700 W power limit) on the bench.c planes: encode 4.53 -> 3.96 ms at
+ * typesize 4 (one hard byte-plane of four), but 5.24 -> 9.37 ms at typesize 2 (both planes hard), 1.42 -> 1.96 ms at typesize 8 and
+ * 1.26 -> 2.54 ms at typesize 16.  Default: blocks of four splits when the
  * chunk has the device to itself (a frame keeps several chunks in flight: streams per SM win there);
  * BLOSC_B200_LZ4_TEAM=0 / 1 forces it off / on. */
 static int team_wanted(const EncodeArgs* a) {
@@ -207,6 +207,16 @@ static int team_wanted(const EncodeArgs* a) {
   if (a->codec != B2_CODEC_LZ4 || a->table_bytes != LZ4_TABLE_BYTES) return 0;
   return env >= 0 ? env : (a->map.nsplits == 4 && !a->many);
 }
+
+#ifdef B2_LZ4_CYCLES
+/* the team encoder's per-stream cycle counters (dev_lz4.cuh, LZ4C_*): LZ4C_MAXSTREAMS x LZ4C_N u64 */
+extern "C" int b2_lz4_cycles_read(unsigned long long* dst, int nstreams) {
+  if (nstreams > LZ4C_MAXSTREAMS) nstreams = LZ4C_MAXSTREAMS;
+  CK(cudaDeviceSynchronize());
+  CK(cudaMemcpyFromSymbol(dst, g_lz4_cycles, (size_t)nstreams * LZ4C_N * sizeof(unsigned long long)));
+  return nstreams;
+}
+#endif
 
 extern "C" int b2_launch_encode(const EncodeArgs* a, b2_stream_t s) {
   if (team_wanted(a)) {

@@ -173,6 +173,10 @@ __global__ void encode_kernel(EncodeArgs a) {
 #define TEAM_WARPS 4
 #define TEAM_CTAS_PER_SM 8
 #define TEAM_SMEM_BYTES (LZ4_TABLE_BYTES + ((LZ4T_SMEM_BYTES + 15) & ~15))
+#define TEAM_SM_SLOTS 1024
+#ifndef SIMT_EMU
+__device__ unsigned g_team_sm_seq[TEAM_SM_SLOTS];    /* team CTAs started on each SM so far (wraps; only mod 4 is used) */
+#endif
 __global__ void __launch_bounds__(TEAM_WARPS * 32, TEAM_CTAS_PER_SM) encode_team_kernel(EncodeArgs a) {
 #ifdef SIMT_EMU
   u8* smem = simt::g_dynsmem;
@@ -182,11 +186,25 @@ __global__ void __launch_bounds__(TEAM_WARPS * 32, TEAM_CTAS_PER_SM) encode_team
   void* tab = smem;
   Lz4Team* tm = (Lz4Team*)(smem + LZ4_TABLE_BYTES);
   const int warp = (int)(threadIdx.x >> 5);
-  /* CTAs land on the SMs round-robin, so the CTAs of one SM differ in blockIdx / num_sms: rotating the
-   * walker role with it puts the (busy) walkers of co-resident teams on different sub-partitions */
-  const int walker = (int)((blockIdx.x / (unsigned)(a.num_sms > 0 ? a.num_sms : 1)) & 3u);
+  /* The walker is the busy warp of a team, so the walkers of co-resident teams should run on different SM
+   * sub-partitions.  CTAs do not land on the SMs in blockIdx order, so each CTA takes the next slot of its SM from a
+   * per-SM counter and makes the warp that runs on that sub-partition (%warpid mod 4) the walker. */
+  int walker = (int)((blockIdx.x / (unsigned)(a.num_sms > 0 ? a.num_sms : 1)) & 3u);
+#ifndef SIMT_EMU
+  if (lane_id() == 0) { unsigned w; asm volatile("mov.u32 %0, %%warpid;" : "=r"(w)); tm->sub[warp] = (int)(w & 3u); }
+  if (threadIdx.x == 0) {
+    unsigned sm; asm volatile("mov.u32 %0, %%smid;" : "=r"(sm));
+    tm->slot = (int)(atomicAdd(&g_team_sm_seq[sm % TEAM_SM_SLOTS], 1u) & 3u);
+  }
+#endif
   if (threadIdx.x == 0) { tm->cmd = 0; tm->gen = 0; }
+#ifdef B2_LZ4_CYCLES
+  if (threadIdx.x < LZ4C_N) tm->cyc[threadIdx.x] = 0;
+#endif
   __syncthreads();
+#ifndef SIMT_EMU
+  for (int k = 3; k >= 0; k--) if (tm->sub[k] == tm->slot) walker = k;
+#endif
   if (warp != walker) { lz4_team_preparer(tm, tab, (warp - walker - 1) & 3); return; }
   int mine = 0;
   for (;;) {
@@ -198,8 +216,23 @@ __global__ void __launch_bounds__(TEAM_WARPS * 32, TEAM_CTAS_PER_SM) encode_team
     const u8* in = a.in + off;
     u8* out = a.slots + off;
     int c, need = 0;
+    LZ4C_T(c_total);
     if (len < 65536 + LZ4_MFLIMIT - 1) c = lz4_encode_warp<true, false, true>(in, len, out, len, a.accel, tab, &need, tm);   /* lz4.c:710,1389 */
     else c = lz4_encode_warp<false, false, true>(in, len, out, len, a.accel, tab, &need, tm);
+#ifdef B2_LZ4_CYCLES
+    {
+      const unsigned long long total = (unsigned long long)(clock64() - c_total);
+      unsigned smid, wid;
+      asm volatile("mov.u32 %0, %%smid;" : "=r"(smid));
+      asm volatile("mov.u32 %0, %%warpid;" : "=r"(wid));
+      __syncwarp();
+      const int k = lane_id();
+      if (idx < LZ4C_MAXSTREAMS && k < LZ4C_N)
+        g_lz4_cycles[idx][k] = k == LZ4C_TOTAL ? total : k == LZ4C_SMID ? smid : k == LZ4C_SUBP ? (wid & 3u) : tm->cyc[k];
+      __syncwarp();
+      if (k < LZ4C_N) tm->cyc[k] = 0;
+    }
+#endif
     if (c <= 0 || c >= len) c = len;           /* blosc.c:705-714: incompressible split is stored raw */
     if (lane_id() == 0) { a.csizes[idx] = c; a.needs[idx] = need; }
     mine++;

@@ -233,6 +233,42 @@ static long long g_dbg_lz4t_sessions = 0, g_dbg_lz4t_seqs = 0, g_dbg_lz4t_stale 
 #define LZ4T_QUIT 1
 #define LZ4T_END 0xffffffffu               /* verdict of a tile too close to the end of the stream to be prepared */
 #define LZ4T_LONG 13                       /* match-length field: 13 = "13 or more bytes after the first four" */
+/* a preparer pulls the bytes this far past its tile into L1 (measured on an H100, power limit 400 and 700 W, on the bench.c planes, typesize 4:
+ * encode 4.17 -> 4.08 ms; 4 and 16 KiB ahead into L2 instead: 4.10 and 4.15 ms) */
+#define LZ4T_PREFETCH 512
+
+/* Cycle accounting (builds with -DB2_LZ4_CYCLES only, scripts/lz4_cycles.py): the walker and the preparers
+ * add the clock64() time of each phase into counters in Lz4Team, and the kernel copies them per stream into
+ * g_lz4_cycles.  Without the flag the macros are empty and the kernels compile to the same SASS. */
+enum {
+  LZ4C_TOTAL,        /* the whole lz4_encode_warp call */
+  LZ4C_START,        /* session start-up: GO to all preparers until the first tile is in the ring */
+  LZ4C_SESSION,      /* rest of a session, waits included */
+  LZ4C_FULLWAIT,     /* of that: walker waiting at bar_sync(FULL) */
+  LZ4C_REPROBE,      /* stale verdict / post-match probe done by the scalar code */
+  LZ4C_SEARCH,       /* search after a chain break (scalar probes, 32-wide rounds, catch-up) */
+  LZ4C_SESSIONS, LZ4C_SEQS, LZ4C_CHAIN_SEQS,
+  LZ4C_PREP_BUSY,    /* preparers, summed over the three: GO returned .. FULL arrived */
+  LZ4C_PREP_OWN,     /* of that: load of the tile's own bytes, hash, table read */
+  LZ4C_PREP_GATHER,  /* of that: candidate gather and compare */
+  LZ4C_PREP_TILES,
+  LZ4C_SMID, LZ4C_SUBP,
+  LZ4C_N = 16
+};
+#ifdef B2_LZ4_CYCLES
+#define LZ4C_MAXSTREAMS 16384
+__device__ unsigned long long g_lz4_cycles[LZ4C_MAXSTREAMS][LZ4C_N];
+#define LZ4C_T(t) const long long t = clock64()
+#define LZ4C_TW(t) const long long t = TEAM ? clock64() : 0ll     /* in code that encode_kernel shares */
+#define LZ4C_ADD(k, v) do { if (lane_id() == 0) atomicAdd(&tm->cyc[k], (unsigned long long)(v)); } while (0)
+#define LZ4C_SPAN(k, t) LZ4C_ADD(k, clock64() - (t))
+#else
+#define LZ4C_T(t) do {} while (0)
+#define LZ4C_TW(t) do {} while (0)
+#define LZ4C_ADD(k, v) do {} while (0)
+#define LZ4C_SPAN(k, t) do {} while (0)
+#endif
+
 struct Lz4Team {
   uint2 vd[LZ4T_RING];                     /* .x verdict: bit 0 hit, bits 2..5 length field, bits 8..23 offset; .y hash */
   const u8* s;                             /* current stream */
@@ -241,6 +277,11 @@ struct Lz4Team {
   int gen;                                 /* session number: a preparer restarts at its first tile when it changes */
   int cmd;                                 /* LZ4T_QUIT ends the preparers */
   int u16;                                 /* table flavour of the current stream */
+  int sub[4];                              /* SM sub-partition of each warp of the CTA */
+  int slot;                                /* sub-partition this CTA's walker should run on */
+#ifdef B2_LZ4_CYCLES
+  unsigned long long cyc[LZ4C_N];
+#endif
 };
 #define LZ4T_SMEM_BYTES ((int)sizeof(Lz4Team))
 
@@ -254,6 +295,7 @@ DEV void lz4_team_prepare_tile(Lz4Team* tm, const void* tabmem, const u8* s, int
   if (w0 + 31 + 24 > n) { tm->vd[e] = make_uint2(LZ4T_END, 0u); return; }     /* loads below reach byte p+19 (+3) */
   const StreamBase sb = make_stream_base(s);
   u32 r[5], a0, a1, a2, a3, a4, c0, c1, c2, c3, c4;
+  LZ4C_T(c_t0);
   ldp_raw20(sb, p, r);
   ldp_take17(sb, p, r, a0, a1, a2, a3, a4);
   const u32 h = lz4_hash_seq<U16>(a0, a1);
@@ -261,6 +303,8 @@ DEV void lz4_team_prepare_tile(Lz4Team* tm, const void* tabmem, const u8* s, int
   const int snap = U16 ? (int)((const volatile u16*)tabmem)[h] : (int)((const volatile u32*)tabmem)[h];
   u32 vx = 0;
   if (snap < p) {                                      /* always true for entries the serial code could see here */
+    LZ4C_T(c_t1);
+    LZ4C_ADD(LZ4C_PREP_OWN, c_t1 - c_t0);
     ldp_gather17(sb, snap, c0, c1, c2, c3, c4);
     const u32 x1 = a1 ^ c1, x2 = a2 ^ c2, x3 = a3 ^ c3;
     u32 m;
@@ -270,6 +314,7 @@ DEV void lz4_team_prepare_tile(Lz4Team* tm, const void* tabmem, const u8* s, int
     else m = a4 != c4 ? 12u : (u32)LZ4T_LONG;
     const bool hit = (U16 || snap + 65535 >= p) && c0 == a0;
     vx = (hit ? 1u : 0u) | (m << 2) | ((u32)((p - snap) & 0xffff) << 8);
+    LZ4C_SPAN(LZ4C_PREP_GATHER, c_t1);
   }
   tm->vd[e] = make_uint2(vx, h);
 }
@@ -280,13 +325,17 @@ DEV void lz4_team_preparer(Lz4Team* tm, const void* tabmem, int i) {
   for (;;) {
     bar_sync(LZ4T_BAR_GO(i), 64);
     if (lz4t_ld_i32(&tm->cmd) == LZ4T_QUIT) return;
+    LZ4C_T(c_go);
     const int gen = lz4t_ld_i32(&tm->gen);
     if (gen != gen_seen) { gen_seen = gen; tile = i; }
     const u8* s = *(const u8* const volatile*)&tm->s;
     const int n = lz4t_ld_i32(&tm->n), w0 = lz4t_ld_i32(&tm->base) + 32 * tile;
+    lz4d_prefetch(s, w0 + LZ4T_PREFETCH + lane_id(), n);
     if (lz4t_ld_i32(&tm->u16)) lz4_team_prepare_tile<true>(tm, tabmem, s, n, w0);
     else lz4_team_prepare_tile<false>(tm, tabmem, s, n, w0);
     tile += 3;
+    LZ4C_SPAN(LZ4C_PREP_BUSY, c_go);
+    LZ4C_ADD(LZ4C_PREP_TILES, 1);
     __threadfence_block();
     bar_arrive(LZ4T_BAR_FULL(i), 64);
   }
@@ -364,6 +413,8 @@ DEV int lz4_encode_warp(const u8* __restrict__ s, const int n, u8* __restrict__ 
         bool finished = false, reanchor = false;
         if (nrec >= 24) LZ4_FLUSH_CHECKED();
         LZ4T_DBG(g_dbg_lz4t_sessions);
+        LZ4C_T(c_s0);
+        LZ4C_ADD(LZ4C_SESSIONS, 1);
         const int base = ip - 2;
         if (lane == 0) {
           tm->s = s; tm->n = n; tm->u16 = U16 ? 1 : 0; tm->base = base;
@@ -378,6 +429,8 @@ DEV int lz4_encode_warp(const u8* __restrict__ s, const int n, u8* __restrict__ 
         int ring_n = 0, rs_lo = 0, rs_1 = 0, rs_2 = 0;   /* stores so far; ring_n when tile t-2 / t-1 / t began */
         bool ovf = false;                     /* more than 32 stores inside the window: every verdict counts as stale */
         bar_sync(LZ4T_BAR_FULL(0), 64); out &= ~1u;
+        LZ4C_SPAN(LZ4C_START, c_s0);
+        LZ4C_T(c_s1);
         const smem_addr_t vda = smem_addr(tm->vd);
         for (;;) {
           const u32 e = (u32)(32 * t + li);
@@ -413,6 +466,7 @@ DEV int lz4_encode_warp(const u8* __restrict__ s, const int n, u8* __restrict__ 
            * written (LZ4_FLUSH_CHECKED) */
           const bool ext = mc >= 15;
           LZ4T_DBG(g_dbg_lz4t_seqs);
+          LZ4C_ADD(LZ4C_CHAIN_SEQS, 1);
           if (lane == nrec) { rec = (ext ? 15u | ((u32)(mc - 15) << 24) : (u32)mc) | ((u32)off << 8); recop = op; }
           nrec++;
           op += ext ? 4 : 3;
@@ -435,14 +489,23 @@ DEV int lz4_encode_warp(const u8* __restrict__ s, const int n, u8* __restrict__ 
               if (ring_n == 0 || k < rs_lo) ring_h = 0xffffffffu;
               ovf = ring_n - rs_lo > 32;
             }
-            bar_sync(LZ4T_BAR_FULL(t % 3), 64); out &= ~(1u << (t % 3));
+            {
+              LZ4C_T(c_w);
+              bar_sync(LZ4T_BAR_FULL(t % 3), 64); out &= ~(1u << (t % 3));
+              LZ4C_SPAN(LZ4C_FULLWAIT, c_w);
+            }
             if (nrec >= 24) LZ4_FLUSH_CHECKED();
           }
         }
         /* leave the session: take the tiles that are still being prepared, so that every preparer is
          * parked at its GO barrier again */
-        for (int i = 0; i < 3; i++)
-          if (out & (1u << i)) bar_sync(LZ4T_BAR_FULL(i), 64);
+        {
+          LZ4C_T(c_w);
+          for (int i = 0; i < 3; i++)
+            if (out & (1u << i)) bar_sync(LZ4T_BAR_FULL(i), 64);
+          LZ4C_SPAN(LZ4C_FULLWAIT, c_w);
+        }
+        LZ4C_SPAN(LZ4C_SESSION, c_s1);
         if (finished) break;
         if (reanchor) continue;
       }
@@ -518,6 +581,7 @@ DEV int lz4_encode_warp(const u8* __restrict__ s, const int n, u8* __restrict__ 
       }
       if (scalar_post) {
         /* ---- fill table at ip-2, test position ip (lz4.c:1236-1294); no literals on a hit ---- */
+        LZ4C_TW(c_r);
         u32 b0, b1, b2 = 0;
         const bool wide = ip + 14 <= n;
         if (wide) ldp_win12(sb, ip - 2, b0, b1, b2);
@@ -539,10 +603,12 @@ DEV int lz4_encode_warp(const u8* __restrict__ s, const int n, u8* __restrict__ 
           }
         }
         if (!hit) ip++;                                                    /* lz4.c:1298 */
+        if (TEAM) LZ4C_SPAN(LZ4C_REPROBE, c_r);
       }
 
       if (!hit) {
         /* ---- find a match (lz4.c:1043-1101): two scalar probes, then 32-wide rounds ---- */
+        LZ4C_TW(c_f);
         bool ended = false;
         for (int it = 0; it < LZ4_SCALAR_PROBES; it++) {
           const int pos = ip + (it ? 1 + (it - 1) * accel : 0);            /* probe offsets 0, 1, 1+accel, 1+2*accel (lz4.c:1043-1053) */
@@ -602,7 +668,7 @@ DEV int lz4_encode_warp(const u8* __restrict__ s, const int n, u8* __restrict__ 
             if (nvalid < 32) break;                                  /* ran into the end: last literals */
           }
         }
-        if (!hit) break;                                             /* -> last literals */
+        if (!hit) { if (TEAM) LZ4C_SPAN(LZ4C_SEARCH, c_f); break; }  /* -> last literals */
 
         /* ---- catch up (lz4.c:1107-1109) ---- */
         if (ip > anchor && match > 0 && s[ip - 1] == s[match - 1]) {
@@ -616,6 +682,7 @@ DEV int lz4_encode_warp(const u8* __restrict__ s, const int n, u8* __restrict__ 
           }
         }
         lit = ip - back - anchor;
+        if (TEAM) LZ4C_SPAN(LZ4C_SEARCH, c_f);
       }
 
       /* ---- match length (lz4.c:1182-1184): LZ4_count(start+4, ...) = catch-up bytes + forward bytes.
@@ -646,6 +713,7 @@ DEV int lz4_encode_warp(const u8* __restrict__ s, const int n, u8* __restrict__ 
       mc += back;
 
       /* ---- emit (lz4.c:1112-1226) ---- */
+      if (TEAM) LZ4C_ADD(LZ4C_SEQS, 1);
       LZ4_FLUSH_CHECKED();
       const int token = op++;
       if (!imm) LZ4_LIMIT(op + lit + (2 + 1 + LZ4_LASTLITERALS) + lit / 255);

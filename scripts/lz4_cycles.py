@@ -1,0 +1,118 @@
+#!/usr/bin/env python
+"""lz4_cycles.py -- where the LZ4 team encoder's cycles go, per phase, on the headline workload
+(bench.py: LZ4, shuffle, typesize 4, clevel 5, 256 MiB of bench.c data).
+
+    python scripts/lz4_cycles.py [--lib variant.so] [-D FLAG ...]
+
+Builds the library with -DB2_LZ4_CYCLES into a temporary directory (or takes an instrumented build
+given with --lib), compresses the buffer in team mode (one warm-up call, then the measured one) and
+prints, per split of a block, the streams' sequence counts and clock64() cycles, then the phase
+breakdown of the hard streams (more than 1000 sequences) per sequence.  Phases (dev_lz4.cuh, LZ4C_*):
+  start    GO to the preparers until the session's first tile is ready
+  chain    the walker's own work in a session (session time minus its FULL waits)
+  fullwait the walker waiting at bar_sync(FULL) for a tile
+  reprobe  stale verdicts and post-match probes done by the scalar code
+  search   the search after a chain break (scalar probes, 32-wide rounds, catch-up)
+  other    the rest of the call (emission of searched sequences, table init, last literals)
+and, for the preparers, the cycles from GO to FULL per tile, split into the load of the tile's own
+bytes (with hash and table read) and the candidate gather (with compare)."""
+import argparse
+import ctypes as C
+import os
+import subprocess
+import sys
+import tempfile
+
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+sys.path.insert(0, ROOT)
+
+# dev_lz4.cuh, enum LZ4C_*
+TOTAL, START, SESSION, FULLWAIT, REPROBE, SEARCH, SESSIONS, SEQS, CHAIN_SEQS, PREP_BUSY, PREP_OWN, PREP_GATHER, \
+    PREP_TILES, SMID, SUBP = range(15)
+NCOL = 16
+MAXSTREAMS = 16384
+
+
+def build(tmp, flags):
+    import __graft_entry__ as g
+    lib = os.path.join(tmp, "libblosc_b200_cycles.so")
+    nvcc = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
+    subprocess.run([nvcc, *g.NVCC_FLAGS, "-DB2_LZ4_CYCLES", *flags, os.path.join(g.CSRC, "backend_cuda.cu"),
+                    os.path.join(g.CSRC, "blosc_b200.c"), "-o", lib], check=True)
+    return lib
+
+
+def main():
+    ap = argparse.ArgumentParser()
+    ap.add_argument("--lib", help="an instrumented build (-DB2_LZ4_CYCLES) to use instead of building one")
+    ap.add_argument("-D", dest="defs", action="append", default=[], help="extra preprocessor definition for the build")
+    args = ap.parse_args()
+    tmp = tempfile.mkdtemp(prefix="lz4_cycles_")
+    os.environ["BLOSC_B200_LIB"] = args.lib or build(tmp, ["-D" + d for d in args.defs])
+    os.environ["BLOSC_B200_LZ4_TEAM"] = "1"
+
+    import numpy as np
+    import torch
+
+    import __graft_entry__ as g
+    from bench import WORKLOADS, CFG2, bench_words
+    pkg = g.load_package()
+    pkg.lib.b2_lz4_cycles_read.restype = C.c_int
+    pkg.lib.b2_lz4_cycles_read.argtypes = [C.c_void_p, C.c_int]
+
+    comp, shuf, ts, clevel, nbytes = WORKLOADS[CFG2]
+    d_src = torch.from_numpy(bench_words(nbytes, np).copy()).cuda()
+    d_chunk = torch.zeros(nbytes + 16, dtype=torch.uint8, device="cuda")
+    cb = pkg.compress_ctx(clevel, shuf, ts, nbytes, d_src, d_chunk, nbytes + 16, comp)
+    pkg.set_profiling(True); pkg.prof_reset()
+    cb = pkg.compress_ctx(clevel, shuf, ts, nbytes, d_src, d_chunk, nbytes + 16, comp)
+    prof = pkg.prof_get(); pkg.set_profiling(False)
+    rec = np.zeros((MAXSTREAMS, NCOL), np.uint64)
+    ns = pkg.lib.b2_lz4_cycles_read(rec.ctypes.data_as(C.c_void_p), MAXSTREAMS)
+    props = torch.cuda.get_device_properties(0)
+    print(f"{props.name}, {props.multi_processor_count} SMs; {CFG2}: cbytes {cb}; kernels (ms) "
+          f"{ {k: round(v[0] / max(v[1], 1), 3) for k, v in prof.items() if v[1]} }")
+    try:
+        q = subprocess.run(["nvidia-smi", "--query-gpu=power.limit,clocks.max.sm,clocks.sm", "--format=csv,noheader"],
+                           capture_output=True, text=True, timeout=30).stdout.strip()
+        print(f"power limit, max SM clock, SM clock: {q}")
+    except (OSError, subprocess.SubprocessError):
+        pass
+
+    # a full block of a typesize-4 shuffle is 4 streams, one per byte-plane
+    r = rec[:ns].astype(np.float64)
+    used = r[:, TOTAL] > 0
+    nsplits = 4
+    print("split streams  seqs/stream  cycles/stream  cycles/seq")
+    for sp in range(nsplits):
+        m = used & (np.arange(ns) % nsplits == sp)
+        if not m.any():
+            continue
+        seqs, tot = r[m, SEQS] + r[m, CHAIN_SEQS], r[m, TOTAL]
+        print(f"{sp:5d} {m.sum():7d} {seqs.mean():12.0f} {tot.mean():14.0f} {tot.sum() / max(seqs.sum(), 1):11.1f}")
+
+    hard = used & (r[:, SEQS] + r[:, CHAIN_SEQS] > 1000)
+    if not hard.any():
+        print("no hard streams")
+        return
+    h = r[hard]
+    seqs = (h[:, SEQS] + h[:, CHAIN_SEQS]).sum()
+    chain = h[:, SESSION] - h[:, FULLWAIT]
+    other = h[:, TOTAL] - h[:, START] - h[:, SESSION] - h[:, REPROBE] - h[:, SEARCH]
+    print(f"hard streams: {hard.sum()}, {seqs / hard.sum():.0f} sequences each ({h[:, CHAIN_SEQS].sum() / seqs:.1%} in a chain), "
+          f"{h[:, SESSIONS].sum() / hard.sum():.0f} sessions each; "
+          f"{len(set(zip(h[:, SMID].astype(int), h[:, SUBP].astype(int))))} distinct (SM, sub-partition) walker slots, "
+          f"{len(set(h[:, SMID].astype(int)))} SMs")
+    print("walker phase   cycles/seq   share")
+    tot = h[:, TOTAL].sum()
+    for name, v in (("start", h[:, START].sum()), ("chain", chain.sum()), ("fullwait", h[:, FULLWAIT].sum()),
+                    ("reprobe", h[:, REPROBE].sum()), ("search", h[:, SEARCH].sum()), ("other", other.sum()),
+                    ("total", tot)):
+        print(f"  {name:10s} {v / seqs:10.1f} {v / tot:7.1%}")
+    tiles = h[:, PREP_TILES].sum()
+    print(f"preparers: {tiles / hard.sum():.0f} tiles per stream; cycles per tile: GO..FULL {h[:, PREP_BUSY].sum() / tiles:.0f}, "
+          f"own bytes {h[:, PREP_OWN].sum() / tiles:.0f}, gather {h[:, PREP_GATHER].sum() / tiles:.0f}")
+
+
+if __name__ == "__main__":
+    main()
