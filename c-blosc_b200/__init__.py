@@ -23,7 +23,7 @@ LIB_PATH = os.path.join(_HERE, "lib", "libblosc_b200.so")
 BLOSC_NOSHUFFLE, BLOSC_SHUFFLE, BLOSC_BITSHUFFLE = 0, 1, 2
 BLOSC_MAX_OVERHEAD = 16
 FILT_SHUFFLE, FILT_UNSHUFFLE, FILT_BITSHUFFLE, FILT_BITUNSHUFFLE = 0, 1, 2, 3
-KERNEL_KINDS = ("filter", "encode", "scan", "compact", "decode", "unfilter", "index", "parse", "zenc", "denc")
+KERNEL_KINDS = ("filter", "encode", "scan", "compact", "decode", "unfilter", "index", "parse", "zenc", "denc", "senc")
 HAS_FAST_PARSE = True      # BLOSC_B200_PARSE=fast: segment-parallel LZ4 parse (csrc/dev_lz4fast.cuh)
 
 

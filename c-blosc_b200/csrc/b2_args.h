@@ -11,7 +11,7 @@ extern "C" {
 #endif
 
 enum { FILT_SHUFFLE = 0, FILT_UNSHUFFLE = 1, FILT_BITSHUFFLE = 2, FILT_BITUNSHUFFLE = 3 };
-enum { B2_CODEC_BLOSCLZ = 0, B2_CODEC_LZ4 = 1, B2_CODEC_ZLIB = 2, B2_CODEC_ZSTD = 3 };
+enum { B2_CODEC_BLOSCLZ = 0, B2_CODEC_LZ4 = 1, B2_CODEC_ZLIB = 2, B2_CODEC_ZSTD = 3, B2_CODEC_SNAPPY = 4 };
 
 typedef struct FilterArgs {
   const uint8_t* src;
@@ -118,6 +118,10 @@ typedef struct FastArgs {
    * its zlib stream (zstd is 0) */
   int deflate;
   int flevel;                      /* zlib's FLEVEL for the clevel (deflate.c), in the stream header */
+  /* snappy encoder (dev_snappy.cuh): the zstd encoder's records, then one warp per stream writes its snappy stream
+   * (zstd and deflate are 0); the last warp's block scan applies blosc_c's snappy maxout rule */
+  int snappy;
+  int ebsize;                      /* blocksize + 4 typesize: the per-block maxbytes of t_blosc's pool (blosc.c:1745) */
 } FastArgs;
 
 typedef struct CompactArgs {

@@ -49,10 +49,11 @@ int  b2_launch_compact(const CompactArgs* a, b2_stream_t s);
 int  b2_launch_decode(const DecodeArgs* a, b2_stream_t s);
 int  b2_launch_fast(const FastArgs* a, b2_stream_t s);      /* index_kernel + parse_kernel (segment-parallel LZ4); with
                                                              * a->zstd: index_kernel + zparse_kernel + zenc_kernel (zstd);
-                                                             * a->deflate: index_kernel + dparse_kernel + denc_kernel (zlib) */
+                                                             * a->deflate: index_kernel + dparse_kernel + denc_kernel (zlib);
+                                                             * a->snappy: index_kernel + zparse_kernel + senc_kernel */
 
 /* profiling: per-kernel-kind CUDA-event timing (off by default) */
-enum { B2_K_FILTER = 0, B2_K_ENCODE, B2_K_SCAN, B2_K_COMPACT, B2_K_DECODE, B2_K_UNFILTER, B2_K_INDEX, B2_K_PARSE, B2_K_ZENC, B2_K_DENC, B2_K_COUNT };
+enum { B2_K_FILTER = 0, B2_K_ENCODE, B2_K_SCAN, B2_K_COMPACT, B2_K_DECODE, B2_K_UNFILTER, B2_K_INDEX, B2_K_PARSE, B2_K_ZENC, B2_K_DENC, B2_K_SENC, B2_K_COUNT };
 void b2_prof_enable(int on);
 void b2_prof_reset(void);
 int  b2_prof_get(int kind, double* ms_total, long long* launches);

@@ -58,6 +58,7 @@ extern "C" int b2_device_prepare(void) {
   CK(cudaFuncSetAttribute(decode_kernel<B2_CODEC_BLOSCLZ>, cudaFuncAttributeMaxDynamicSharedMemorySize, DECODE_WARPS * LZ4D_SMEM));
   CK(cudaFuncSetAttribute(decode_kernel<B2_CODEC_ZLIB>, cudaFuncAttributeMaxDynamicSharedMemorySize, DECODE_WARPS * LZ4D_SMEM));
   CK(cudaFuncSetAttribute(decode_kernel<B2_CODEC_ZSTD>, cudaFuncAttributeMaxDynamicSharedMemorySize, DECODE_WARPS * LZ4D_SMEM));
+  CK(cudaFuncSetAttribute(decode_kernel<B2_CODEC_SNAPPY>, cudaFuncAttributeMaxDynamicSharedMemorySize, DECODE_WARPS * LZ4D_SMEM));
   CK(cudaFuncSetAttribute(index_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, INDEX_WARPS * FAST_TAB_BYTES));
   CK(cudaFuncSetAttribute(parse_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, B2_FAST_WIN_MAX + 64));
   CK(cudaFuncSetAttribute(zparse_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, B2_FAST_WIN_MAX + 64));
@@ -247,35 +248,49 @@ extern "C" int b2_launch_encode(const EncodeArgs* a, b2_stream_t s) {
   return 0;
 }
 
-/* segment-parallel LZ4: the hash-chain index of every stream, then one lane per segment; a->zstd: the same index and
- * parse into zstd sequence records, then one warp per zstd frame (dev_zstdenc.cuh); a->deflate: the same records with
- * offsets <= 32768, then one warp per zlib stream (dev_deflate.cuh) */
-extern "C" int b2_launch_fast(const FastArgs* a, b2_stream_t s) {
-  if (a->map.nstreams <= 0) return 0;
+/* the front half of every segment-parallel encoder: the hash-chain index of every stream, then one lane per segment --
+ * LZ4 bytes (parse_kernel), or zstd sequence records (`records`: zparse_kernel; a->deflate: dparse_kernel, offsets
+ * <= 32768) */
+static int launch_fast_front(const FastArgs* a, bool records, b2_stream_t s) {
   {
     int ctas = (a->map.nstreams + INDEX_WARPS - 1) / INDEX_WARPS;
     ProfScope ps(B2_K_INDEX, s->s);
     index_kernel<<<ctas, INDEX_WARPS * 32, INDEX_WARPS * FAST_TAB_BYTES, s->s>>>(*a);
     CK(cudaGetLastError());
   }
-  {
-    const long long njobs = (long long)a->map.nfull * a->map.nsplits * a->groups_full + a->groups_left;
-    const int threads = a->threads;
-    const size_t smem = (size_t)a->win_bytes + 64;
-    int per_sm = (int)((size_t)220 * 1024 / (smem + 1024));
-    if (per_sm * threads > 2048) per_sm = 2048 / threads;
-    if (per_sm < 1) per_sm = 1;
-    long long ctas = njobs;
-    const long long cap = (long long)num_sms() * per_sm;
-    if (ctas > cap) ctas = cap;
-    ProfScope ps(B2_K_PARSE, s->s);
-    FastArgs args = *a;
-    args.queue_base = *a->queue_base_host;
-    *a->queue_base_host += (unsigned)njobs + (unsigned)ctas;      /* one ticket-drawing thread per CTA */
-    if (a->deflate) dparse_kernel<<<(unsigned)ctas, threads, smem, s->s>>>(args);
-    else if (a->zstd) zparse_kernel<<<(unsigned)ctas, threads, smem, s->s>>>(args);
-    else parse_kernel<<<(unsigned)ctas, threads, smem, s->s>>>(args);
+  const long long njobs = (long long)a->map.nfull * a->map.nsplits * a->groups_full + a->groups_left;
+  const int threads = a->threads;
+  const size_t smem = (size_t)a->win_bytes + 64;
+  int per_sm = (int)((size_t)220 * 1024 / (smem + 1024));
+  if (per_sm * threads > 2048) per_sm = 2048 / threads;
+  if (per_sm < 1) per_sm = 1;
+  long long ctas = njobs;
+  const long long cap = (long long)num_sms() * per_sm;
+  if (ctas > cap) ctas = cap;
+  ProfScope ps(B2_K_PARSE, s->s);
+  FastArgs args = *a;
+  args.queue_base = *a->queue_base_host;
+  *a->queue_base_host += (unsigned)njobs + (unsigned)ctas;      /* one ticket-drawing thread per CTA */
+  if (a->deflate) dparse_kernel<<<(unsigned)ctas, threads, smem, s->s>>>(args);
+  else if (records) zparse_kernel<<<(unsigned)ctas, threads, smem, s->s>>>(args);
+  else parse_kernel<<<(unsigned)ctas, threads, smem, s->s>>>(args);
+  CK(cudaGetLastError());
+  return 0;
+}
+
+/* segment-parallel LZ4: the front half, then the stream scan; a->zstd: the front half with records, then one warp per
+ * zstd frame (dev_zstdenc.cuh); a->deflate: the same records with offsets <= 32768, then one warp per zlib stream
+ * (dev_deflate.cuh); a->snappy: the zstd records, then one warp per snappy stream (dev_snappy.cuh), whose last warp
+ * runs the block scan with blosc_c's snappy maxout rule */
+extern "C" int b2_launch_fast(const FastArgs* a, b2_stream_t s) {
+  if (a->map.nstreams <= 0) return 0;
+  if (launch_fast_front(a, a->zstd || a->snappy, s)) return -1;
+  if (a->snappy) {                                                /* one warp per snappy stream */
+    const int ctas = (a->map.nstreams + SN_WARPS - 1) / SN_WARPS;
+    ProfScope ps(B2_K_SENC, s->s);
+    senc_kernel<<<ctas, SN_WARPS * 32, 0, s->s>>>(*a);
     CK(cudaGetLastError());
+    return 0;
   }
   if (a->zstd) {                                                  /* one warp per zstd frame */
     const int ctas = (a->map.nstreams + ZE_WARPS - 1) / ZE_WARPS;
@@ -354,6 +369,7 @@ extern "C" int b2_launch_decode(const DecodeArgs* a, b2_stream_t s) {
   if (a->codec == B2_CODEC_LZ4) decode_kernel<B2_CODEC_LZ4><<<ctas, wpc * 32, sm, s->s>>>(args);
   else if (a->codec == B2_CODEC_ZLIB) decode_kernel<B2_CODEC_ZLIB><<<ctas, wpc * 32, sm, s->s>>>(args);
   else if (a->codec == B2_CODEC_ZSTD) decode_kernel<B2_CODEC_ZSTD><<<ctas, wpc * 32, sm, s->s>>>(args);
+  else if (a->codec == B2_CODEC_SNAPPY) decode_kernel<B2_CODEC_SNAPPY><<<ctas, wpc * 32, sm, s->s>>>(args);
   else decode_kernel<B2_CODEC_BLOSCLZ><<<ctas, wpc * 32, sm, s->s>>>(args);
   CK(cudaGetLastError());
   return 0;

@@ -294,12 +294,21 @@ static int zlib_enabled(void) {
   return e && *e && atoi(e) != 0;
 }
 
+/* BLOSC_B200_SNAPPY=1 (read on every call, independent of the other two) does the same for snappy: "snappy" chunks are
+ * written (dev_snappy.cuh) and read.  Unset, it is a reference built without snappy, which neither writes nor reads
+ * them (blosc.c:547-553). */
+static int snappy_enabled(void) {
+  const char* e = getenv("BLOSC_B200_SNAPPY");
+  return e && *e && atoi(e) != 0;
+}
+
 int blosc_compcode_to_compname(int compcode, const char** compname) {    /* blosc.c:329-374 */
   static const char* names[6] = {BLOSC_BLOSCLZ_COMPNAME, BLOSC_LZ4_COMPNAME, BLOSC_LZ4HC_COMPNAME,
                                  BLOSC_SNAPPY_COMPNAME, BLOSC_ZLIB_COMPNAME, BLOSC_ZSTD_COMPNAME};
   *compname = (compcode >= 0 && compcode < 6) ? names[compcode] : NULL;
   /* codecs this build can ENCODE; like a reference built without the others */
   if (compcode == BLOSC_BLOSCLZ || compcode == BLOSC_LZ4 || compcode == BLOSC_LZ4HC) return compcode;
+  if (compcode == BLOSC_SNAPPY && snappy_enabled()) return compcode;
   if (compcode == BLOSC_ZLIB && zlib_enabled()) return compcode;
   if (compcode == BLOSC_ZSTD && zstd_enabled()) return compcode;
   return -1;
@@ -309,17 +318,25 @@ int blosc_compname_to_compcode(const char* compname) {                    /* blo
   if (strcmp(compname, BLOSC_BLOSCLZ_COMPNAME) == 0) return BLOSC_BLOSCLZ;
   if (strcmp(compname, BLOSC_LZ4_COMPNAME) == 0) return BLOSC_LZ4;
   if (strcmp(compname, BLOSC_LZ4HC_COMPNAME) == 0) return BLOSC_LZ4HC;
+  if (strcmp(compname, BLOSC_SNAPPY_COMPNAME) == 0 && snappy_enabled()) return BLOSC_SNAPPY;
   if (strcmp(compname, BLOSC_ZLIB_COMPNAME) == 0 && zlib_enabled()) return BLOSC_ZLIB;
   if (strcmp(compname, BLOSC_ZSTD_COMPNAME) == 0 && zstd_enabled()) return BLOSC_ZSTD;
   return -1;
 }
 
+/* the reference's order, minus the codecs that are switched off: one string per combination of the three switches
+ * (snappy | zlib << 1 | zstd << 2), built once, so that a returned pointer stays valid whatever the switches do later */
+static char g_complists[8][64];
+static pthread_once_t g_complists_once = PTHREAD_ONCE_INIT;
+static void build_complists(void) {
+  for (int m = 0; m < 8; m++)
+    snprintf(g_complists[m], sizeof g_complists[m], "%s,%s,%s%s%s%s", BLOSC_BLOSCLZ_COMPNAME, BLOSC_LZ4_COMPNAME,
+             BLOSC_LZ4HC_COMPNAME, (m & 1) ? "," BLOSC_SNAPPY_COMPNAME : "", (m & 2) ? "," BLOSC_ZLIB_COMPNAME : "",
+             (m & 4) ? "," BLOSC_ZSTD_COMPNAME : "");
+}
 const char* blosc_list_compressors(void) {                                  /* blosc.c:2029-2042 */
-  const int zl = zlib_enabled(), zs = zstd_enabled();
-  if (zl && zs) return BLOSC_BLOSCLZ_COMPNAME "," BLOSC_LZ4_COMPNAME "," BLOSC_LZ4HC_COMPNAME "," BLOSC_ZLIB_COMPNAME "," BLOSC_ZSTD_COMPNAME;
-  if (zl) return BLOSC_BLOSCLZ_COMPNAME "," BLOSC_LZ4_COMPNAME "," BLOSC_LZ4HC_COMPNAME "," BLOSC_ZLIB_COMPNAME;
-  if (zs) return BLOSC_BLOSCLZ_COMPNAME "," BLOSC_LZ4_COMPNAME "," BLOSC_LZ4HC_COMPNAME "," BLOSC_ZSTD_COMPNAME;
-  return BLOSC_BLOSCLZ_COMPNAME "," BLOSC_LZ4_COMPNAME "," BLOSC_LZ4HC_COMPNAME;
+  pthread_once(&g_complists_once, build_complists);
+  return g_complists[snappy_enabled() | zlib_enabled() << 1 | zstd_enabled() << 2];
 }
 const char* blosc_get_version_string(void) { return BLOSC_VERSION_STRING; }
 
@@ -329,6 +346,10 @@ int blosc_get_complib_info(const char* compname, char** complib, char** version)
   if (strcmp(compname, BLOSC_BLOSCLZ_COMPNAME) == 0) { code = BLOSC_BLOSCLZ_LIB; lib = "BloscLZ"; ver = "2.5.1"; }
   else if (strcmp(compname, BLOSC_LZ4_COMPNAME) == 0 || strcmp(compname, BLOSC_LZ4HC_COMPNAME) == 0) {
     code = BLOSC_LZ4_LIB; lib = "LZ4"; ver = "1.10.0";
+  } else if (strcmp(compname, BLOSC_SNAPPY_COMPNAME) == 0 && snappy_enabled()) {
+    /* what the reference reports when its snappy does not define SNAPPY_VERSION (blosc.c:2056,2078-2084): these
+     * streams are no snappy release's */
+    code = BLOSC_SNAPPY_LIB; lib = "Snappy"; ver = "unknown";
   } else if (strcmp(compname, BLOSC_ZLIB_COMPNAME) == 0 && zlib_enabled()) {
     code = BLOSC_ZLIB_LIB; lib = "Zlib"; ver = "1.3.1";          /* the zlib release the streams are checked against */
   } else if (strcmp(compname, BLOSC_ZSTD_COMPNAME) == 0 && zstd_enabled()) {
@@ -603,6 +624,7 @@ static int compress_impl(int clevel, int doshuffle, size_t typesize, size_t nbyt
   if (compcode == BLOSC_BLOSCLZ) compformat = BLOSC_BLOSCLZ_FORMAT;
   else if (compcode == BLOSC_LZ4) compformat = BLOSC_LZ4_FORMAT;
   else if (compcode == BLOSC_LZ4HC) compformat = BLOSC_LZ4HC_FORMAT;     /* blosc.c:1170-1172: the LZ4 format */
+  else if (compcode == BLOSC_SNAPPY) compformat = BLOSC_SNAPPY_FORMAT;   /* blosc.c:1176-1181 */
   else if (compcode == BLOSC_ZLIB) compformat = BLOSC_ZLIB_FORMAT;       /* blosc.c:1183-1188 */
   else if (compcode == BLOSC_ZSTD) compformat = BLOSC_ZSTD_FORMAT;       /* blosc.c:1190-1196 */
   else {
@@ -683,14 +705,15 @@ static int compress_impl(int clevel, int doshuffle, size_t typesize, size_t nbyt
     sa.bstarts = (int*)w->bstarts.p; sa.result = w->d_result;
     sa.nsplits = nsplits; sa.nfull = nfull; sa.has_leftover = leftover > 0; sa.destsize = dsz;
     /* the warp that finishes the last stream also does the block scan (no separate 1-CTA launch) */
-    ea.fold_scan = nblocks <= B2_FOLD_SCAN_MAX_BLOCKS;
+    ea.fold_scan = nblocks <= B2_FOLD_SCAN_MAX_BLOCKS || compcode == BLOSC_SNAPPY;   /* snappy's scan is always folded */
     ea.scan = sa;
     launched = 1;
     memset(&ca, 0, sizeof ca);
-    if (compcode == BLOSC_ZSTD || compcode == BLOSC_ZLIB) {
+    if (compcode == BLOSC_ZSTD || compcode == BLOSC_ZLIB || compcode == BLOSC_SNAPPY) {
       /* the zstd encoder (dev_zstdenc.cuh): the index and windows of the segment-parallel parse, sequence records
        * instead of LZ4 bytes, then one warp per zstd frame.  The DEFLATE encoder (dev_deflate.cuh) shares the parse,
-       * with offsets <= 32768, then one warp writes each zlib stream. */
+       * with offsets <= 32768, then one warp writes each zlib stream.  The snappy encoder (dev_snappy.cuh) takes the
+       * zstd records as they are, then one warp writes each snappy stream. */
       FastArgs fx;
       const int neblock = bs / nsplits;
       const int longest = neblock > leftover ? neblock : leftover;
@@ -714,11 +737,15 @@ static int compress_impl(int clevel, int doshuffle, size_t typesize, size_t nbyt
       if (buf_ensure(recs, (size_t)nsegs * B2_FAST_SEG + 64)) break;
       if (buf_ensure(&w->segs, (size_t)nsegs * 4 + 64)) break;
       fx.zstd = compcode == BLOSC_ZSTD; fx.deflate = compcode == BLOSC_ZLIB;
+      /* snappy is a speed codec: the effort of the segment-parallel LZ4 parse (chain depth 3 clevel + 1, no lazy
+       * matching) */
+      if (compcode == BLOSC_SNAPPY) { fx.depth = 3 * clevel + 1; fx.lazy = 0; }
       /* zlib's FLEVEL for compress2(.., clevel) (blosc.c:472-483, deflate.c) */
       fx.flevel = clevel < 2 ? 0 : (clevel < 6 ? 1 : (clevel == 6 ? 2 : 3));
       fx.prev = (uint16_t*)w->prev.p; fx.recs = (uint32_t*)recs->p; fx.nrec = (uint32_t*)w->segs.p;
       fx.queue = ea.queue; fx.queue_base_host = ea.queue_base_host; fx.done = ea.done;
       fx.fold_scan = ea.fold_scan; fx.scan = sa;
+      fx.snappy = compcode == BLOSC_SNAPPY; fx.ebsize = bs + 4 * ts;
       if (b2_launch_fast(&fx, w->stream)) break;
     } else if (ea.codec == B2_CODEC_LZ4 && (compcode == BLOSC_LZ4HC || lz4_fast_wanted())) {
       FastArgs fx;
@@ -815,6 +842,11 @@ static int codec_from_header(const b2_hdr* h, int* codec) {                /* bl
   const int fmt = (h->flags & 0xe0) >> 5;
   if (fmt == BLOSC_BLOSCLZ_FORMAT) { if (h->versionlz != BLOSC_BLOSCLZ_VERSION_FORMAT) return -9; *codec = B2_CODEC_BLOSCLZ; return 0; }
   if (fmt == BLOSC_LZ4_FORMAT) { if (h->versionlz != BLOSC_LZ4_VERSION_FORMAT) return -9; *codec = B2_CODEC_LZ4; return 0; }
+  if (fmt == BLOSC_SNAPPY_FORMAT && snappy_enabled()) {               /* blosc.c:545-553 */
+    if (h->versionlz != BLOSC_SNAPPY_VERSION_FORMAT) return -9;
+    *codec = B2_CODEC_SNAPPY;
+    return 0;
+  }
   if (fmt == BLOSC_ZLIB_FORMAT) { if (h->versionlz != BLOSC_ZLIB_VERSION_FORMAT) return -9; *codec = B2_CODEC_ZLIB; return 0; }   /* blosc.c:556-561 */
   if (fmt == BLOSC_ZSTD_FORMAT) { if (h->versionlz != BLOSC_ZSTD_VERSION_FORMAT) return -9; *codec = B2_CODEC_ZSTD; return 0; }   /* blosc.c:565-571 */
   return -5;

@@ -23,6 +23,7 @@
 #include "dev_zstd.cuh"
 #include "dev_zstdenc.cuh"
 #include "dev_deflate.cuh"
+#include "dev_snappy.cuh"
 
 
 
@@ -352,6 +353,7 @@ __global__ void __launch_bounds__(B2_FAST_WIN_MAX / FAST_SEG, 3) parse_kernel(Fa
   u8* smem = simt::g_dynsmem;
   if (a.zstd) { fast_parse_body<true>(a, smem); return; }     /* the emulator launches the zstd parse under this name */
   if (a.deflate) { fast_parse_body<true, DZ_MAXD>(a, smem); return; }   /* and the DEFLATE parse */
+  if (a.snappy) { fast_parse_body<true>(a, smem); return; }          /* and the snappy encoder's (zparse) */
 #else
   extern __shared__ __align__(16) u8 smem[];
 #endif
@@ -383,6 +385,7 @@ __global__ void __launch_bounds__(B2_FAST_WIN_MAX / FAST_SEG, 3) dparse_kernel(F
 #define FSCAN_WARPS 4
 DEV void zenc_body(const FastArgs& a, ZeSm* S);
 DEV void denc_body(const FastArgs& a, DzSm* S);
+DEV void senc_body(const FastArgs& a);
 __global__ void __launch_bounds__(FSCAN_WARPS * 32) fscan_kernel(FastArgs a) {
 #ifdef SIMT_EMU
   if (a.zstd) {                                    /* the emulator launches the zstd entropy stage under this name */
@@ -395,6 +398,7 @@ __global__ void __launch_bounds__(FSCAN_WARPS * 32) fscan_kernel(FastArgs a) {
     denc_body(a, &dtab[threadIdx.x >> 5]);
     return;
   }
+  if (a.snappy) { senc_body(a); return; }          /* and the snappy stream writer */
 #endif
   const int lane = lane_id();
   const int nfs = a.map.nfull * a.map.nsplits;
@@ -498,6 +502,152 @@ __global__ void __launch_bounds__(DZ_WARPS * 32) denc_kernel(FastArgs a) {
   denc_body(a, (DzSm*)(smem + (size_t)(threadIdx.x >> 5) * DZ_SMEM_BYTES));
 }
 
+
+/* ---- snappy (dev_snappy.cuh): index_kernel, zparse_kernel, then one warp per snappy stream ---- */
+/* snappy_max_compressed_length (snappy.cc MaxCompressedLength): the output room blosc_c asks for (blosc.c:640-645) */
+DEV long long sn_bound(int n) { return 32 + (long long)n + n / 6; }
+
+/* The block scan of warp_scan_blocks with blosc_c's snappy maxout rule in front, by ONE warp.  blosc_c hands snappy
+ * maxout = snappy_max_compressed_length(neblock), clamped to the room left (blosc.c:640-651), and snappy_compress
+ * refuses any smaller buffer: a split whose room is below that bound is stored raw if neblock still fits (:705-714),
+ * and otherwise the call gives up.  The room is measured from the stream's own sizes:
+ *   - pool (t_blosc, !serial): per block, from 0 with maxbytes = ebsize (blosc.c:1745,1810);
+ *   - serial: from the chunk's start with maxbytes = destsize.  The first split short of its bound is found on the
+ *     compressed sizes; from there on every full split is short of it too (the room only shrinks), so they become
+ *     raw, and the leftover split is judged at its new position.
+ * Raw splits get csizes = their length, so compaction copies them from the input (`csizes` is a.csizes, writable). */
+#ifdef SIMT_EMU
+static int* g_sn_presizes = nullptr;          /* emulator builds: where to copy the stream sizes the rule starts from */
+static int g_sn_presizes_cap = 0;
+#endif
+DEV void warp_scan_blocks_snappy(const ScanArgs& a, int* csizes, const int ebsize) {
+  const int lane = lane_id();
+  const int nblocks = a.nfull + (a.has_leftover ? 1 : 0);
+#ifdef SIMT_EMU
+  {
+    const int ns = a.nfull * a.nsplits + (a.has_leftover ? 1 : 0);
+    if (lane == 0 && g_sn_presizes) for (int i = 0; i < ns && i < g_sn_presizes_cap; i++) g_sn_presizes[i] = csizes[i];
+    __syncwarp();
+  }
+#endif
+  const int per = (nblocks + 31) / 32;
+  const int b0 = lane * per < nblocks ? lane * per : nblocks, b1 = b0 + per < nblocks ? b0 + per : nblocks;
+  int bad = 0;
+  if (!a.serial) {
+    for (int b = b0; b < b1; b++) {
+      const int ns = b < a.nfull ? a.nsplits : 1;
+      const int neblock = b < a.nfull ? a.blocksize / a.nsplits : a.leftover;
+      long long nt = 0;
+      for (int s = 0; s < ns; s++) {
+        const long long idx = b < a.nfull ? (long long)b * a.nsplits + s : (long long)a.nfull * a.nsplits;
+        int c = ld_cg_i32(&csizes[idx]);
+        nt += 4;
+        const long long room = ebsize - nt;
+        if (room < sn_bound(neblock)) {
+          if (room >= neblock) { if (c != neblock) { c = neblock; csizes[idx] = c; } }
+          else bad = 1;
+        }
+        nt += c;
+      }
+    }
+  }
+  long long first = 0x7fffffffffffffffll;     /* serial: the first split short of its bound */
+  long long pos0 = 0, total = 0;
+  for (int pass = 0; pass < 2; pass++) {
+    long long sum = 0;
+    for (int b = b0; b < b1; b++) {
+      if (b < a.nfull) for (int s = 0; s < a.nsplits; s++) sum += 4 + (long long)ld_cg_i32(&csizes[(long long)b * a.nsplits + s]);
+      else sum += 4 + (long long)ld_cg_i32(&csizes[(long long)a.nfull * a.nsplits]);
+    }
+    long long incl = sum;
+#pragma unroll
+    for (int d = 1; d < 32; d <<= 1) {
+      const long long t = __shfl_up_sync(FULLMASK, incl, d);
+      if (lane >= d) incl += t;
+    }
+    pos0 = 16 + 4ll * nblocks + (incl - sum);
+    total = 16 + 4ll * nblocks + __shfl_sync(FULLMASK, incl, 31);
+    if (!a.serial || pass == 1) break;
+    long long pos = pos0, mine = first;
+    for (int b = b0; b < b1 && mine == first; b++) {
+      const int ns = b < a.nfull ? a.nsplits : 1;
+      const int neblock = b < a.nfull ? a.blocksize / a.nsplits : a.leftover;
+      for (int s = 0; s < ns; s++) {
+        const long long idx = b < a.nfull ? (long long)b * a.nsplits + s : (long long)a.nfull * a.nsplits;
+        if (a.destsize - (pos + 4) < sn_bound(neblock)) { mine = idx; break; }
+        pos += 4 + (long long)ld_cg_i32(&csizes[idx]);
+      }
+    }
+#pragma unroll
+    for (int d = 16; d >= 1; d >>= 1) {
+      const long long t = __shfl_xor_sync(FULLMASK, mine, d);
+      mine = t < mine ? t : mine;
+    }
+    first = mine;
+    if (first == 0x7fffffffffffffffll) break;
+    for (int b = b0 < a.nfull ? b0 : a.nfull; b < b1 && b < a.nfull; b++)
+      for (int s = 0; s < a.nsplits; s++) {
+        const long long idx = (long long)b * a.nsplits + s;
+        if (idx >= first) csizes[idx] = a.blocksize / a.nsplits;
+      }
+  }
+  long long pos = pos0, grow = 0;
+  for (int b = b0; b < b1; b++) {
+    a.bstarts[b] = (int)(pos > 0x7fffffffll ? 0x7fffffffll : pos);
+    const int ns = b < a.nfull ? a.nsplits : 1;
+    const int neblock = b < a.nfull ? a.blocksize / a.nsplits : a.leftover;
+    for (int s = 0; s < ns; s++) {
+      const long long idx = b < a.nfull ? (long long)b * a.nsplits + s : (long long)a.nfull * a.nsplits;
+      int c = ld_cg_i32(&csizes[idx]);
+      if (a.serial && idx >= first) {
+        const long long room = a.destsize - (pos + 4);
+        if (room < sn_bound(neblock)) {
+          if (room >= neblock) { if (c != neblock) { grow += neblock - c; c = neblock; csizes[idx] = c; } }   /* only the leftover split can still change */
+          else bad = 1;
+        }
+      }
+      pos += 4 + (long long)c;
+    }
+  }
+#pragma unroll
+  for (int d = 16; d >= 1; d >>= 1) grow += __shfl_xor_sync(FULLMASK, grow, d);
+  total += grow;
+  const unsigned anybad = __ballot_sync(FULLMASK, bad);
+  if (lane == 0) {
+    a.result[B2_R_CBYTES] = (int)(total > 0x7fffffffll ? 0x7fffffffll : total);
+    a.result[B2_R_FITS] = (total <= a.destsize && anybad == 0u) ? 1 : 0;       /* blosc.c:1848 / :836-839 give up */
+  }
+}
+
+/* One warp per stream: its snappy stream; whoever completes the stream count runs the snappy block scan */
+#define SN_WARPS 4
+DEV void senc_body(const FastArgs& a) {
+  const int lane = lane_id(), warp = (int)(threadIdx.x >> 5), nwarps = (int)(blockDim.x >> 5);
+  int mine = 0;
+  for (int idx = (int)blockIdx.x * nwarps + warp; idx < a.map.nstreams; idx += (int)gridDim.x * nwarps) {
+    int block, len, split;
+    long long off;
+    stream_locate(a.map, idx, &block, &off, &len, &split);
+    const long long gseg = (long long)idx * a.segs_full;
+    int c = sn_stream(a.in + off, len, a.recs + gseg * ZE_SEG_RECS, a.nrec + gseg, (u8*)(a.prev + off), a.slots + off);
+    if (c >= len) c = len;                         /* blosc.c:705-714: incompressible split is stored raw */
+    if (lane == 0) { a.csizes[idx] = c; a.needs[idx] = c; }
+    mine++;
+    __syncwarp();
+  }
+  if (mine == 0) return;
+  __threadfence();
+  int last = 0;
+  if (lane == 0) last = atomicAdd(a.done, mine) + mine == a.map.nstreams;
+  last = __shfl_sync(FULLMASK, last, 0);
+  if (!last) return;
+  __threadfence();
+  warp_scan_blocks_snappy(a.scan, a.csizes, a.ebsize);      /* (always folded: the host never launches scan_kernel for snappy) */
+  __syncwarp();
+  if (lane == 0) *a.done = 0;
+}
+
+__global__ void __launch_bounds__(SN_WARPS * 32) senc_kernel(FastArgs a) { senc_body(a); }
 
 #define SCAN_THREADS 1024
 __global__ void __launch_bounds__(SCAN_THREADS) scan_kernel(ScanArgs a) {
@@ -660,6 +810,10 @@ __global__ void __launch_bounds__(DECODE_WARPS * 32) decode_kernel(DecodeArgs a)
     if (CODEC == B2_CODEC_LZ4) return lz4_decode_warp(src, cs, out, len, wsmem);
     if (CODEC == B2_CODEC_ZLIB) return zlib_decode_warp(src, cs, out, len, wsmem);
     if (CODEC == B2_CODEC_ZSTD) return zstd_decode_warp(src, cs, out, len, wsmem);
+    if (CODEC == B2_CODEC_SNAPPY) return snappy_decode_warp(src, cs, out, len, wsmem);
+#ifdef SIMT_EMU
+    if (a.codec == B2_CODEC_SNAPPY) return snappy_decode_warp(src, cs, out, len, wsmem);   /* the emulator launches it as decode_kernel<0> */
+#endif
     return blz_decode_warp(src, cs, out, len);
   });
 }

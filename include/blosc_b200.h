@@ -17,7 +17,8 @@
  *     effort -- every reference build decodes the chunks, the header is the reference's, the
  *     bytes are not LZ4_compress_HC's; other compressors report -5 exactly like a reference built
  *     with -DDEACTIVATE_ZLIB/ZSTD/SNAPPY (blosc.c:573,1197-1208).  Decoding is wider: zlib and
- *     zstd chunks decode too (serial GPU decoders, one lane per stream); snappy chunks report -5;
+ *     zstd chunks decode too (serial GPU decoders, one lane per stream); snappy chunks report -5 unless
+ *     BLOSC_B200_SNAPPY=1;
  *   - with the environment variable BLOSC_B200_ZSTD=1 (read on every call) the library behaves
  *     like a reference built with zstd: "zstd" is listed, named and encoded (segment-parallel GPU
  *     encoder, one zstd frame per block).  The header is the reference's and every reference build
@@ -26,6 +27,9 @@
  *     reference built with zlib: "zlib" is listed, named and encoded (segment-parallel GPU encoder,
  *     one zlib stream per split).  Every zlib reads the streams, but they are not compress2's bytes
  *     and their sizes differ;
+ *   - with BLOSC_B200_SNAPPY=1 (read on every call, independent of the other two) it behaves like a reference built
+ *     with snappy: "snappy" is listed, named, encoded and decoded on the GPU (one snappy stream per split, valid snappy
+ *     but no snappy release's bytes; blosc_get_complib_info reports version "unknown");
  *   - there is no CPU codec: without a CUDA device every compress/decompress call
  *     prints a message on stderr and returns -1.
  */
@@ -79,10 +83,12 @@ extern "C" {
 #define BLOSC_BLOSCLZ_FORMAT BLOSC_BLOSCLZ_LIB
 #define BLOSC_LZ4_FORMAT BLOSC_LZ4_LIB
 #define BLOSC_LZ4HC_FORMAT BLOSC_LZ4_LIB
+#define BLOSC_SNAPPY_FORMAT BLOSC_SNAPPY_LIB
 #define BLOSC_ZLIB_FORMAT BLOSC_ZLIB_LIB
 #define BLOSC_ZSTD_FORMAT BLOSC_ZSTD_LIB
 #define BLOSC_BLOSCLZ_VERSION_FORMAT 1
 #define BLOSC_LZ4_VERSION_FORMAT 1
+#define BLOSC_SNAPPY_VERSION_FORMAT 1
 #define BLOSC_ZLIB_VERSION_FORMAT 1
 #define BLOSC_ZSTD_VERSION_FORMAT 1
 #define BLOSC_ALWAYS_SPLIT 1

@@ -2,7 +2,8 @@
 """Workload for the AddressSanitizer build of the emulated library (make -C tests/emu asan):
   LD_PRELOAD=$(gcc -print-file-name=libasan.so) ASAN_OPTIONS=detect_leaks=0 python scripts/asan_emu_case.py
 exact / fast / lz4hc / BloscLZ paths, exact-size buffers, damaged chunks, crafted and damaged zstd frames and zlib streams,
-crafted, random and damaged LZ4 and BloscLZ streams."""
+crafted, random and damaged LZ4 and BloscLZ streams, the snappy encoder (serial and pool maxout rules) and crafted,
+random and damaged snappy streams."""
 import os, sys, ctypes as C, numpy as np
 sys.path.insert(0, os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), 'tests'))
 from datagen import gen, compress, decompress
@@ -109,4 +110,35 @@ for name,ch,n in ledges.chunk_corpus():
     emu.blosc_decompress_ctx(c.ctypes.data_as(C.c_void_p),out.ctypes.data_as(C.c_void_p),C.c_size_t(n),C.c_int(1))
     emu.blosc_getitem(c.ctypes.data_as(C.c_void_p),C.c_int(0),C.c_int(n//ch[3]),out.ctypes.data_as(C.c_void_p))
     cases+=1
+os.environ['BLOSC_B200_SNAPPY']='1'        # the snappy encoder and decoder: both maxout rules, raw and compressed splits
+import snappy_read, snappy_write
+srng=np.random.default_rng(7)
+for kind in ("bench","text","lowent","mixed","zeros","rand"):
+    for n in (13, 1000, 70001, 300001):
+        src=gen(kind,n)
+        for ts,shuf,cl,bs,nt in ((4,1,5,0,1),(1,0,9,0,4),(8,2,1,0,1),(3,1,5,200000,4)):
+            dest=np.full(n+16,0xAA,np.uint8)
+            r=emu.blosc_compress_ctx(C.c_int(cl),C.c_int(shuf),C.c_size_t(ts),C.c_size_t(n),src.ctypes.data_as(C.c_void_p),dest.ctypes.data_as(C.c_void_p),C.c_size_t(n+16),b"snappy",C.c_size_t(bs),C.c_int(nt))
+            assert r>0
+            chunk=dest[:r].copy(); out=np.zeros(n,np.uint8)
+            assert emu.blosc_decompress_ctx(chunk.ctypes.data_as(C.c_void_p),out.ctypes.data_as(C.c_void_p),C.c_size_t(n),C.c_int(1))==n and (out==src).all()
+            for t in range(3):
+                c=chunk.copy(); pos=srng.integers(16,r,3); c[pos]=srng.integers(0,256,3,dtype=np.uint8)
+                emu.blosc_decompress_ctx(c.ctypes.data_as(C.c_void_p),out.ctypes.data_as(C.c_void_p),C.c_size_t(n),C.c_int(1))
+            cases+=1
+for t in range(300):                        # crafted streams, then random damage and truncation, exact-size buffers
+    lit=srng.integers(0,256,int(srng.integers(1,3000)),dtype=np.uint8).tobytes()
+    els=[("lit",lit)]+[("c2",int(srng.integers(1,65)),int(srng.integers(1,len(lit)+1))) for _ in range(int(srng.integers(0,60)))]
+    n=len(snappy_write.expand(els)); st=bytearray(snappy_write.stream(n,els))
+    if t%3==1: st[int(srng.integers(0,len(st)))]=int(srng.integers(0,256))
+    if t%3==2: st=st[:int(srng.integers(0,len(st)+1))]
+    # one unsplit block holding the stream (a stream of n bytes would be taken for a raw split)
+    if len(st)==n: st=st+b"\0"
+    hdr=bytes([2,1,0x10|(2<<5),1])+n.to_bytes(4,"little")+n.to_bytes(4,"little")+(24+len(st)).to_bytes(4,"little")+(20).to_bytes(4,"little")+len(st).to_bytes(4,"little")
+    c=np.frombuffer(hdr+bytes(st),np.uint8).copy(); out=np.zeros(n,np.uint8)
+    r=emu.blosc_decompress_ctx(c.ctypes.data_as(C.c_void_p),out.ctypes.data_as(C.c_void_p),C.c_size_t(n),C.c_int(1))
+    got,why=snappy_read.read(bytes(st),n)
+    assert (r==n)==(why is None) and (why is not None or out.tobytes()==got)
+    cases+=1
+os.environ.pop('BLOSC_B200_SNAPPY', None)
 print("asan workload ok, cases", cases)
