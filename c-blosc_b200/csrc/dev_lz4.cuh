@@ -213,26 +213,47 @@ DEV int lz4_count_tail(const StreamBase& sb, const u8* __restrict__ s, int p, in
  * for every position of a 32-position tile a preparer computes hash, table lookup, candidate
  * gather, 17-byte compare and packs the verdict {hit, match length, offset} into a shared-memory
  * ring; the walker reads the verdict of the position it lands on with one 8-byte shared load.
- * A verdict can be stale: the preparer of tile t starts when the walker has finished tile t-3, so
- * it cannot have seen the table stores of tiles t-2 .. t.  The walker keeps the hashes of exactly
- * those stores in a 32-entry register ring (one per lane) and tests "is the hash of this position
- * among them" with one compare + ballot; such a position (rare) is resolved by the scalar code.
+ * A verdict carries the candidate it was computed from (`snap`, the table entry the preparer read).
+ * It is a pure function of (position, snap): the 4-byte equality, the 65535-distance rule and the
+ * 17-byte length depend on nothing else.  The walker makes every table store in serial order, so
+ * after its store at ip-2 the live table[h(ip)] is what LZ4_compress_fast would read; when it equals
+ * snap the verdict is exact, however old it is, and otherwise (rare) the scalar code probes itself.
  * The parse, the table and the output stay byte-identical to LZ4_compress_fast.
- * Hand-offs use named barriers (bar.sync / bar.arrive, 64 threads each): GO(i) walker -> preparer i
- * "tile may be prepared", FULL(i) preparer i -> walker "tile is in the ring"; preparer i owns the
- * tiles i, i+3, i+6, ... of a session.  Waiting warps are descheduled by the barrier hardware. */
+ * Preparation follows stream positions, not chains: tile T (positions 32T .. 32T+31) lives in ring
+ * slot T mod LZ4T_TILES and is prepared by preparer T mod 3, which owns the slot (LZ4T_TILES is a
+ * multiple of 3), so a slot's entries and ready word are written by one warp in order.  The walker
+ * publishes the lowest tile it still reads (`wt`, the tile of ip-2); a preparer skips tiles below it
+ * and prepares up to LZ4T_AHEAD tiles past it, then naps.  After each tile it posts the tile number
+ * in the slot's ready word.  A chain that starts again after a search or a long match reads tiles
+ * that are prepared or in flight, or moves `wt` past them, which re-bases the preparers: nothing is
+ * restarted or drained.  Per stream, the walker starts preparer i through barrier GO(i) and, at the end,
+ * waits at barrier IDLE(i) until it has stopped (bar.sync / bar.arrive, 64 threads: the walker and
+ * preparer i); after the last stream, LZ4T_QUIT and GO(i) end it. */
 #ifdef SIMT_EMU
+/* x[]: 0 LZ4T_LONG, 1 match of 270+ bytes, 2 re-base, 3 chain start on prepared tiles, 4 chained miss, 5 walker waited for a tile */
 static long long g_dbg_lz4t_sessions = 0, g_dbg_lz4t_seqs = 0, g_dbg_lz4t_stale = 0, g_dbg_lz4t_x[6];
 #define LZ4T_DBG(x) do { if (lane_id() == 0) (x)++; } while (0)
 #else
 #define LZ4T_DBG(x) do {} while (0)
 #endif
-#define LZ4T_RING 256                      /* positions in the verdict ring = 8 tiles */
-#define LZ4T_BAR_FULL(i) (1 + (i))
+#ifndef LZ4T_TILES
+#define LZ4T_TILES 12                      /* ring slots of 32 positions; a multiple of 3 (one owner per slot) */
+#endif
+#ifndef LZ4T_AHEAD
+#define LZ4T_AHEAD 8                       /* tiles a preparer may work past `wt`; at most LZ4T_TILES - 1 */
+#endif
+#ifndef LZ4T_NAP
+#define LZ4T_NAP 128                       /* ns a preparer naps when it is LZ4T_AHEAD tiles ahead */
+#endif
+#define LZ4T_RING (32 * LZ4T_TILES)
+#define LZ4T_BAR_IDLE(i) (1 + (i))
 #define LZ4T_BAR_GO(i) (4 + (i))
 #define LZ4T_QUIT 1
-#define LZ4T_END 0xffffffffu               /* verdict of a tile too close to the end of the stream to be prepared */
+#define LZ4T_STOP 0x7fffffff               /* `wt` at the end of a stream: preparers go to IDLE(i) */
+#define LZ4T_END 0xffffffffu               /* snap of a position that was not compared (too close to the end of the
+                                            * stream, or the table held no earlier position): no table entry equals it */
 #define LZ4T_LONG 13                       /* match-length field: 13 = "13 or more bytes after the first four" */
+static_assert(LZ4T_TILES % 3 == 0 && LZ4T_AHEAD >= 1 && LZ4T_AHEAD < LZ4T_TILES && LZ4T_RING > 15 + 255 + 4, "team ring layout");
 /* a preparer pulls the bytes this far past its tile into L1 (measured on an H100, power limit 400 and 700 W, on the bench.c planes, typesize 4:
  * encode 4.17 -> 4.08 ms; 4 and 16 KiB ahead into L2 instead: 4.10 and 4.15 ms) */
 #define LZ4T_PREFETCH 512
@@ -242,17 +263,18 @@ static long long g_dbg_lz4t_sessions = 0, g_dbg_lz4t_seqs = 0, g_dbg_lz4t_stale 
  * g_lz4_cycles.  Without the flag the macros are empty and the kernels compile to the same SASS. */
 enum {
   LZ4C_TOTAL,        /* the whole lz4_encode_warp call */
-  LZ4C_START,        /* session start-up: GO to all preparers until the first tile is in the ring */
-  LZ4C_SESSION,      /* rest of a session, waits included */
-  LZ4C_FULLWAIT,     /* of that: walker waiting at bar_sync(FULL) */
+  LZ4C_START,        /* chain start: publishing `wt` until the first tiles of the chain are ready */
+  LZ4C_SESSION,      /* rest of a chain, waits included */
+  LZ4C_FULLWAIT,     /* of that: walker waiting for the ready word of a tile */
   LZ4C_REPROBE,      /* stale verdict / post-match probe done by the scalar code */
   LZ4C_SEARCH,       /* search after a chain break (scalar probes, 32-wide rounds, catch-up) */
   LZ4C_SESSIONS, LZ4C_SEQS, LZ4C_CHAIN_SEQS,
-  LZ4C_PREP_BUSY,    /* preparers, summed over the three: GO returned .. FULL arrived */
+  LZ4C_PREP_BUSY,    /* preparers, summed over the three: tile allowed .. ready word posted */
   LZ4C_PREP_OWN,     /* of that: load of the tile's own bytes, hash, table read */
   LZ4C_PREP_GATHER,  /* of that: candidate gather and compare */
   LZ4C_PREP_TILES,
   LZ4C_SMID, LZ4C_SUBP,
+  LZ4C_STALE,        /* chained positions whose verdict's snap differed from the live table */
   LZ4C_N = 16
 };
 #ifdef B2_LZ4_CYCLES
@@ -270,13 +292,14 @@ __device__ unsigned long long g_lz4_cycles[LZ4C_MAXSTREAMS][LZ4C_N];
 #endif
 
 struct Lz4Team {
-  uint2 vd[LZ4T_RING];                     /* .x verdict: bit 0 hit, bits 2..5 length field, bits 8..23 offset; .y hash */
+  uint2 vd[LZ4T_RING];                     /* .x: bit 0 hit, bits 2..5 length field, bits 8..20 hash; .y snap */
+  int rdy[LZ4T_TILES];                     /* ready word of each slot: number + 1 of the tile whose verdicts it holds */
   const u8* s;                             /* current stream */
   int n;
-  int base;                                /* position of ring entry 0 in this session */
-  int gen;                                 /* session number: a preparer restarts at its first tile when it changes */
-  int cmd;                                 /* LZ4T_QUIT ends the preparers */
   int u16;                                 /* table flavour of the current stream */
+  int wt;                                  /* lowest tile the walker still reads, or LZ4T_STOP */
+  int gen;                                 /* streams started by this team (zeroed at launch, with cmd) */
+  int cmd;                                 /* LZ4T_QUIT ends the preparers */
   int sub[4];                              /* SM sub-partition of each warp of the CTA */
   int slot;                                /* sub-partition this CTA's walker should run on */
 #ifdef B2_LZ4_CYCLES
@@ -286,23 +309,25 @@ struct Lz4Team {
 #define LZ4T_SMEM_BYTES ((int)sizeof(Lz4Team))
 
 DEV int lz4t_ld_i32(const int* p) { return *(const volatile int*)p; }
+DEV void lz4t_st_i32(int* p, int v) { *(volatile int*)p = v; }
 
 template <bool U16>
-DEV void lz4_team_prepare_tile(Lz4Team* tm, const void* tabmem, const u8* s, int n, int w0) {
+DEV void lz4_team_prepare_tile(Lz4Team* tm, const void* tabmem, const u8* s, int n, int tile) {
   const int lane = lane_id();
-  const int p = w0 + lane;
-  const int e = (w0 - lz4t_ld_i32(&tm->base) + lane) & (LZ4T_RING - 1);
-  if (w0 + 31 + 24 > n) { tm->vd[e] = make_uint2(LZ4T_END, 0u); return; }     /* loads below reach byte p+19 (+3) */
+  const int w0 = 32 * tile, p = w0 + lane;
+  const int e = (tile % LZ4T_TILES) * 32 + lane;
+  if (w0 + 31 + 24 > n) { tm->vd[e] = make_uint2(0u, LZ4T_END); return; }     /* loads below reach byte p+19 (+3) */
   const StreamBase sb = make_stream_base(s);
   u32 r[5], a0, a1, a2, a3, a4, c0, c1, c2, c3, c4;
   LZ4C_T(c_t0);
   ldp_raw20(sb, p, r);
   ldp_take17(sb, p, r, a0, a1, a2, a3, a4);
   const u32 h = lz4_hash_seq<U16>(a0, a1);
-  /* racing with the walker's stores is fine: whatever this read misses is in the walker's ring */
+  /* racing with the walker's stores (and, at a stream's start, with its clearing of the table) is fine:
+   * the walker takes the verdict only if the live entry still equals snap */
   const int snap = U16 ? (int)((const volatile u16*)tabmem)[h] : (int)((const volatile u32*)tabmem)[h];
-  u32 vx = 0;
-  if (snap < p) {                                      /* always true for entries the serial code could see here */
+  u32 vx = h << 8, sn = LZ4T_END;
+  if ((unsigned)snap < (unsigned)p) {                  /* always true for entries the serial code could see here */
     LZ4C_T(c_t1);
     LZ4C_ADD(LZ4C_PREP_OWN, c_t1 - c_t0);
     ldp_gather17(sb, snap, c0, c1, c2, c3, c4);
@@ -313,32 +338,60 @@ DEV void lz4_team_prepare_tile(Lz4Team* tm, const void* tabmem, const u8* s, int
     else if (x3) m = 8u + ((u32)(__ffs((int)x3) - 1) >> 3);
     else m = a4 != c4 ? 12u : (u32)LZ4T_LONG;
     const bool hit = (U16 || snap + 65535 >= p) && c0 == a0;
-    vx = (hit ? 1u : 0u) | (m << 2) | ((u32)((p - snap) & 0xffff) << 8);
+    vx |= (hit ? 1u : 0u) | (m << 2);
+    sn = (u32)snap;
     LZ4C_SPAN(LZ4C_PREP_GATHER, c_t1);
   }
-  tm->vd[e] = make_uint2(vx, h);
+  tm->vd[e] = make_uint2(vx, sn);
 }
 
-/* body of preparer warp i (0..2); returns when the walker posts LZ4T_QUIT */
+/* body of preparer warp i (0..2): per stream, tiles i, i+3, i+6, ... from GO(i) until the walker posts
+ * LZ4T_STOP; returns when the walker posts LZ4T_QUIT */
 DEV void lz4_team_preparer(Lz4Team* tm, const void* tabmem, int i) {
-  int gen_seen = -1, tile = i;
   for (;;) {
     bar_sync(LZ4T_BAR_GO(i), 64);
     if (lz4t_ld_i32(&tm->cmd) == LZ4T_QUIT) return;
-    LZ4C_T(c_go);
-    const int gen = lz4t_ld_i32(&tm->gen);
-    if (gen != gen_seen) { gen_seen = gen; tile = i; }
     const u8* s = *(const u8* const volatile*)&tm->s;
-    const int n = lz4t_ld_i32(&tm->n), w0 = lz4t_ld_i32(&tm->base) + 32 * tile;
-    lz4d_prefetch(s, w0 + LZ4T_PREFETCH + lane_id(), n);
-    if (lz4t_ld_i32(&tm->u16)) lz4_team_prepare_tile<true>(tm, tabmem, s, n, w0);
-    else lz4_team_prepare_tile<false>(tm, tabmem, s, n, w0);
-    tile += 3;
-    LZ4C_SPAN(LZ4C_PREP_BUSY, c_go);
-    LZ4C_ADD(LZ4C_PREP_TILES, 1);
-    __threadfence_block();
-    bar_arrive(LZ4T_BAR_FULL(i), 64);
+    const int n = lz4t_ld_i32(&tm->n), u16 = lz4t_ld_i32(&tm->u16);
+    for (int tile = i;; tile += 3) {
+      int w;
+      for (;;) {                                       /* until the tile may be prepared */
+        w = __shfl_sync(FULLMASK, lz4t_ld_i32(&tm->wt), 0);
+        if (w == LZ4T_STOP) break;
+        if (tile < w) tile = w + (i + 3 - w % 3) % 3;  /* the walker is past it: first own tile from w on */
+        if (tile <= w + LZ4T_AHEAD) break;             /* slot of tile - LZ4T_TILES (< w) is no longer read */
+        __nanosleep(LZ4T_NAP);
+      }
+      if (w == LZ4T_STOP) break;
+      LZ4C_T(c_go);
+      lz4d_prefetch(s, 32 * tile + LZ4T_PREFETCH + lane_id(), n);
+      if (u16) lz4_team_prepare_tile<true>(tm, tabmem, s, n, tile);
+      else lz4_team_prepare_tile<false>(tm, tabmem, s, n, tile);
+      __syncwarp();
+      if (lane_id() == 0) { __threadfence_block(); lz4t_st_i32(&tm->rdy[tile % LZ4T_TILES], tile + 1); }
+      LZ4C_SPAN(LZ4C_PREP_BUSY, c_go);
+      LZ4C_ADD(LZ4C_PREP_TILES, 1);
+    }
+    __syncwarp();
+    bar_arrive(LZ4T_BAR_IDLE(i), 64);
   }
+}
+
+/* walker: the chain needs the tiles of ip-2 and ip.  Publishes the tile of ip-2 as `wt` (moving it past
+ * the tiles the preparers may have started re-bases them there) and waits for the ready words of the
+ * tiles up to that of ip not yet checked (vt = highest tile checked). */
+DEV void lz4t_reach(Lz4Team* tm, int ip, int& wt, int& vt) {
+  const int lo = (ip - 2) >> 5, hi = ip >> 5;
+  if (lo > wt + LZ4T_AHEAD) LZ4T_DBG(g_dbg_lz4t_x[2]);
+  if (lo != wt) { wt = lo; lz4t_st_i32(&tm->wt, lo); }
+  for (int t = vt + 1 > lo ? vt + 1 : lo; t <= hi; t++) {
+    const int* r = &tm->rdy[t % LZ4T_TILES];
+    if (lz4t_ld_i32(r) != t + 1) {
+      LZ4T_DBG(g_dbg_lz4t_x[5]);
+      do { __syncwarp(); } while (__any_sync(FULLMASK, lz4t_ld_i32(r) != t + 1));
+    }
+  }
+  if (hi > vt) vt = hi;
 }
 
 /* Returns the compressed size, or 0 when the stream does not fit in `cap`
@@ -357,9 +410,9 @@ DEV void lz4_team_preparer(Lz4Team* tm, const void* tabmem, int i) {
  * the table is kept as 4096 x u16 plus one bit per entry -- 8.5 KiB instead of 16 KiB, i.e. twice as
  * many streams per SM.  It costs a few instructions per probe; measured with 4 chunks in flight it wins
  * at typesize 2 and 8 and loses at typesize 4, so the host only uses it on request (BLOSC_B200_LZ4_PACK=1). */
-template <bool U16, bool PACK = false, bool TEAM = false>
-DEV int lz4_encode_warp(const u8* __restrict__ s, const int n, u8* __restrict__ d, const int cap,
-                        const int accel, void* tabmem, int* need_out, Lz4Team* tm = nullptr) {
+template <bool U16, bool PACK, bool TEAM>
+DEV int lz4_encode_stream(const u8* __restrict__ s, const int n, u8* __restrict__ d, const int cap,
+                          const int accel, void* tabmem, int* need_out, Lz4Team* tm) {
   const int lane = lane_id();
   const StreamBase sb = make_stream_base(s);
   u16* tab16 = (u16*)tabmem;
@@ -393,6 +446,7 @@ DEV int lz4_encode_warp(const u8* __restrict__ s, const int n, u8* __restrict__ 
   u32 pq0 = 0, pq1 = 0, pq2 = 0, pq3 = 0;    /* its raw aligned words */
   int nrec = 0, recop = 0;
   u32 rec = 0;
+  int twt = 0, tvt = -1;                     /* TEAM: `wt` as last published, highest tile whose ready word was checked */
 #define LZ4_FLUSH_CHECKED() do { if (nrec) { LZ4_LIMIT(op + (1 + LZ4_LASTLITERALS)); } LZ4_FLUSH(); } while (0)
 #define LZ4_FLUSH() do { if (lane < nrec) { d[recop] = (u8)rec; d[recop + 1] = (u8)(rec >> 8); d[recop + 2] = (u8)(rec >> 16); \
                                              if ((rec & 15u) == 15u) d[recop + 3] = (u8)(rec >> 24); } nrec = 0; } while (0)
@@ -410,53 +464,41 @@ DEV int lz4_encode_warp(const u8* __restrict__ s, const int n, u8* __restrict__ 
         /* ---- chained "test next position" (lz4.c:1236-1294) with the verdicts prepared by the helper
          * warps (see "team mode" above) ---- */
         scalar_post = false;
-        bool finished = false, reanchor = false;
+        bool finished = false;
         if (nrec >= 24) LZ4_FLUSH_CHECKED();
         LZ4T_DBG(g_dbg_lz4t_sessions);
         LZ4C_T(c_s0);
         LZ4C_ADD(LZ4C_SESSIONS, 1);
-        const int base = ip - 2;
-        if (lane == 0) {
-          tm->s = s; tm->n = n; tm->u16 = U16 ? 1 : 0; tm->base = base;
-          tm->gen = lz4t_ld_i32(&tm->gen) + 1;
-        }
-        __syncwarp();
-        __threadfence_block();
-        bar_arrive(LZ4T_BAR_GO(0), 64); bar_arrive(LZ4T_BAR_GO(1), 64); bar_arrive(LZ4T_BAR_GO(2), 64);
-        u32 out = 7u;                         /* preparers that were told to go and whose tile has not been taken yet */
-        int t = 0, li = 2;                    /* current tile of the session and position inside it: ip == base + 32 t + li */
-        u32 ring_h = 0xffffffffu;             /* lane l: hash of the (l mod 32)-th most recent table store, or invalid */
-        int ring_n = 0, rs_lo = 0, rs_1 = 0, rs_2 = 0;   /* stores so far; ring_n when tile t-2 / t-1 / t began */
-        bool ovf = false;                     /* more than 32 stores inside the window: every verdict counts as stale */
-        bar_sync(LZ4T_BAR_FULL(0), 64); out &= ~1u;
+        if ((ip - 2) >> 5 <= twt + LZ4T_AHEAD) LZ4T_DBG(g_dbg_lz4t_x[3]);     /* its tiles are prepared or in flight */
+        lz4t_reach(tm, ip, twt, tvt);
+        __syncwarp();                         /* table stores of the scalar code (lane 0) are seen by every lane */
         LZ4C_SPAN(LZ4C_START, c_s0);
         LZ4C_T(c_s1);
         const smem_addr_t vda = smem_addr(tm->vd);
+        u32 e = (u32)ip % (u32)LZ4T_RING;     /* ring entry of ip: slot (ip >> 5) mod LZ4T_TILES, lane ip & 31 */
         for (;;) {
-          const u32 e = (u32)(32 * t + li);
-          u32 pk, h;
-          smem_ld_u32x2(vda, (e & (LZ4T_RING - 1)) << 3, pk, h);
-          const u32 h2 = smem_ld_u32(vda, (((e - 2u) & (LZ4T_RING - 1)) << 3) + 4u);
+          u32 pk, snap;
+          smem_ld_u32x2(vda, e << 3, pk, snap);
+          const u32 h2 = smem_ld_u32(vda, (e >= 2u ? e - 2u : e - 2u + LZ4T_RING) << 3) >> 8;
+          const u32 h = pk >> 8;
           LZ4_TPUT(h2, ip - 2);                                            /* every lane the same word: no hand-off between lanes */
-          if (ring_n - rs_lo >= 32) ovf = true;
-          if (lane == (ring_n & 31)) ring_h = h2;
-          ring_n++;
-          const unsigned stale = __ballot_sync(FULLMASK, ring_h == h);
-          if (stale || ovf || pk == LZ4T_END) { LZ4T_DBG(g_dbg_lz4t_stale); scalar_post = true; break; }      /* the plain probe below looks this one up itself */
+          const int cand = LZ4_TGET(h);
+          __syncwarp();                                                    /* every lane has read the entry before any overwrites it */
+          if (cand != (int)snap) {                                         /* the verdict was computed from another candidate */
+            LZ4T_DBG(g_dbg_lz4t_stale); LZ4C_ADD(LZ4C_STALE, 1);
+            scalar_post = true; break;                                     /* the plain probe below looks this one up itself */
+          }
           LZ4_TPUT(h, ip);                                                 /* lz4.c:1291: ip goes into the table, hit or not */
-          if (ring_n - rs_lo >= 32) ovf = true;
-          if (lane == (ring_n & 31)) ring_h = h;
-          ring_n++;
-          if (!(pk & 1u)) { LZ4T_DBG(g_dbg_lz4t_x[0]); ip++; break; }                                 /* lz4.c:1298; on to the search below */
-          const int off = (int)(pk >> 8);
+          if (!(pk & 1u)) { LZ4T_DBG(g_dbg_lz4t_x[4]); ip++; break; }                                 /* lz4.c:1298; on to the search below */
+          const int off = ip - (int)snap;
           int mc = (int)((pk >> 2) & 15u);
           if (mc == LZ4T_LONG) {
-            LZ4T_DBG(g_dbg_lz4t_x[1]);
+            LZ4T_DBG(g_dbg_lz4t_x[0]);
             mc = LZ4T_LONG + lz4_count_tail(sb, s, ip + 4 + LZ4T_LONG, ip - off + 4 + LZ4T_LONG, matchlimit, n);   /* ip+64 <= n: far from matchlimit */
             if (mc >= 15 + 255) {                                          /* very long match: general emission below */
               hit = true; imm = true; match = ip - off;
               have_mc = true; mc_carry = mc;
-              LZ4T_DBG(g_dbg_lz4t_x[2]);
+              LZ4T_DBG(g_dbg_lz4t_x[1]);
               break;
             }
           }
@@ -471,43 +513,23 @@ DEV int lz4_encode_warp(const u8* __restrict__ s, const int n, u8* __restrict__ 
           nrec++;
           op += ext ? 4 : 3;
           ip += mc + 4;
-          li += mc + 4;
+          e += (u32)(mc + 4);                                              /* mc + 4 < 15 + 255 + 4 < LZ4T_RING */
+          if (e >= (u32)LZ4T_RING) e -= (u32)LZ4T_RING;
           anchor = ip;
           if (ip + 64 > n) {                                               /* a match ended close to the end of the stream */
             if (ip >= mfl1) finished = true;                               /* lz4.c:1230-1233 */
             else scalar_post = true;                                       /* the plain probe below takes over */
             break;
           }
-          if (li >= 128) { LZ4T_DBG(g_dbg_lz4t_x[3]); reanchor = true; break; }                       /* jumped past everything that is being prepared */
-          while (li >= 32) {                                               /* on to the next tile */
-            __threadfence_block();
-            bar_arrive(LZ4T_BAR_GO(t % 3), 64); out |= 1u << (t % 3);      /* its preparer may start tile t+3 */
-            t++; li -= 32;
-            rs_lo = rs_1; rs_1 = rs_2; rs_2 = ring_n;                      /* the window is now the stores of tiles t-2 .. t */
-            {
-              const int k = ring_n - 1 - ((ring_n - 1 - lane) & 31);       /* index of the store this lane holds */
-              if (ring_n == 0 || k < rs_lo) ring_h = 0xffffffffu;
-              ovf = ring_n - rs_lo > 32;
-            }
-            {
-              LZ4C_T(c_w);
-              bar_sync(LZ4T_BAR_FULL(t % 3), 64); out &= ~(1u << (t % 3));
-              LZ4C_SPAN(LZ4C_FULLWAIT, c_w);
-            }
-            if (nrec >= 24) LZ4_FLUSH_CHECKED();
+          if ((ip >> 5) > tvt) {                                           /* on to a tile not checked yet */
+            LZ4C_T(c_w);
+            lz4t_reach(tm, ip, twt, tvt);
+            LZ4C_SPAN(LZ4C_FULLWAIT, c_w);
+            if (nrec >= 24) LZ4_FLUSH_CHECKED();                           /* at most 8 sequences start inside one tile */
           }
-        }
-        /* leave the session: take the tiles that are still being prepared, so that every preparer is
-         * parked at its GO barrier again */
-        {
-          LZ4C_T(c_w);
-          for (int i = 0; i < 3; i++)
-            if (out & (1u << i)) bar_sync(LZ4T_BAR_FULL(i), 64);
-          LZ4C_SPAN(LZ4C_FULLWAIT, c_w);
         }
         LZ4C_SPAN(LZ4C_SESSION, c_s1);
         if (finished) break;
-        if (reanchor) continue;
       }
       if (!TEAM && post && ip + 64 <= n) {
         scalar_post = false;
@@ -779,6 +801,35 @@ DEV int lz4_encode_warp(const u8* __restrict__ s, const int n, u8* __restrict__ 
 #undef LZ4_LIMIT
 #undef LZ4_TGET
 #undef LZ4_TPUT
+}
+
+/* Team mode, walker side, around each stream: the preparers start with wt = 0 and fresh ready words; at
+ * the end the walker posts LZ4T_STOP and waits until all three are parked at their GO barriers again,
+ * so that the next stream may change the stream fields and clear the ready words.  The kernel ends
+ * the preparers after its last stream by posting LZ4T_QUIT and arriving at GO(0..2). */
+DEV void lz4t_begin(Lz4Team* tm, const u8* s, int n, bool u16) {
+  const int lane = lane_id();
+  for (int i = lane; i < LZ4T_TILES; i += 32) tm->rdy[i] = 0;
+  if (lane == 0) { tm->s = s; tm->n = n; tm->u16 = u16 ? 1 : 0; tm->wt = 0; tm->gen = tm->gen + 1; }
+  __syncwarp();
+  __threadfence_block();
+  bar_arrive(LZ4T_BAR_GO(0), 64); bar_arrive(LZ4T_BAR_GO(1), 64); bar_arrive(LZ4T_BAR_GO(2), 64);
+}
+DEV void lz4t_end(Lz4Team* tm) {
+  if (lane_id() == 0) lz4t_st_i32(&tm->wt, LZ4T_STOP);
+  __syncwarp();
+  bar_sync(LZ4T_BAR_IDLE(0), 64); bar_sync(LZ4T_BAR_IDLE(1), 64); bar_sync(LZ4T_BAR_IDLE(2), 64);
+}
+
+/* Returns the compressed size, or 0 when the stream does not fit in `cap` (see lz4_encode_stream).
+ * TEAM: the calling warp is the walker of the team `tm` (one stream from start to end, on every return). */
+template <bool U16, bool PACK = false, bool TEAM = false>
+DEV int lz4_encode_warp(const u8* __restrict__ s, const int n, u8* __restrict__ d, const int cap,
+                        const int accel, void* tabmem, int* need_out, Lz4Team* tm = nullptr) {
+  if (TEAM) lz4t_begin(tm, s, n, U16);
+  const int c = lz4_encode_stream<U16, PACK, TEAM>(s, n, d, cap, accel, tabmem, need_out, tm);
+  if (TEAM) lz4t_end(tm);
+  return c;
 }
 
 /* ---- decoder ---- */

@@ -8,14 +8,16 @@ Builds the library with -DB2_LZ4_CYCLES into a temporary directory (or takes an 
 given with --lib), compresses the buffer in team mode (one warm-up call, then the measured one) and
 prints, per split of a block, the streams' sequence counts and clock64() cycles, then the phase
 breakdown of the hard streams (more than 1000 sequences) per sequence.  Phases (dev_lz4.cuh, LZ4C_*):
-  start    GO to the preparers until the session's first tile is ready
-  chain    the walker's own work in a session (session time minus its FULL waits)
-  fullwait the walker waiting at bar_sync(FULL) for a tile
+  start    chain start: publishing the walker's tile until the chain's first tiles are ready
+  chain    the walker's own work in a chain (chain time minus its tile waits)
+  fullwait the walker waiting for the ready word of a tile inside a chain
   reprobe  stale verdicts and post-match probes done by the scalar code
   search   the search after a chain break (scalar probes, 32-wide rounds, catch-up)
   other    the rest of the call (emission of searched sequences, table init, last literals)
-and, for the preparers, the cycles from GO to FULL per tile, split into the load of the tile's own
-bytes (with hash and table read) and the candidate gather (with compare)."""
+and, for the preparers, the cycles per tile from being allowed to prepare it to posting its ready word,
+split into the load of the tile's own bytes (with hash and table read) and the candidate gather (with
+compare); and the share of chained positions whose verdict was stale (its snap differed from the live
+table), which the scalar code probes again."""
 import argparse
 import ctypes as C
 import os
@@ -28,7 +30,7 @@ sys.path.insert(0, ROOT)
 
 # dev_lz4.cuh, enum LZ4C_*
 TOTAL, START, SESSION, FULLWAIT, REPROBE, SEARCH, SESSIONS, SEQS, CHAIN_SEQS, PREP_BUSY, PREP_OWN, PREP_GATHER, \
-    PREP_TILES, SMID, SUBP = range(15)
+    PREP_TILES, SMID, SUBP, STALE = range(16)
 NCOL = 16
 MAXSTREAMS = 16384
 
@@ -100,7 +102,7 @@ def main():
     chain = h[:, SESSION] - h[:, FULLWAIT]
     other = h[:, TOTAL] - h[:, START] - h[:, SESSION] - h[:, REPROBE] - h[:, SEARCH]
     print(f"hard streams: {hard.sum()}, {seqs / hard.sum():.0f} sequences each ({h[:, CHAIN_SEQS].sum() / seqs:.1%} in a chain), "
-          f"{h[:, SESSIONS].sum() / hard.sum():.0f} sessions each; "
+          f"{h[:, SESSIONS].sum() / hard.sum():.0f} chains each; "
           f"{len(set(zip(h[:, SMID].astype(int), h[:, SUBP].astype(int))))} distinct (SM, sub-partition) walker slots, "
           f"{len(set(h[:, SMID].astype(int)))} SMs")
     print("walker phase   cycles/seq   share")
@@ -110,8 +112,12 @@ def main():
                     ("total", tot)):
         print(f"  {name:10s} {v / seqs:10.1f} {v / tot:7.1%}")
     tiles = h[:, PREP_TILES].sum()
-    print(f"preparers: {tiles / hard.sum():.0f} tiles per stream; cycles per tile: GO..FULL {h[:, PREP_BUSY].sum() / tiles:.0f}, "
+    print(f"preparers: {tiles / hard.sum():.0f} tiles per stream; cycles per tile: allowed..ready {h[:, PREP_BUSY].sum() / tiles:.0f}, "
           f"own bytes {h[:, PREP_OWN].sum() / tiles:.0f}, gather {h[:, PREP_GATHER].sum() / tiles:.0f}")
+    looked = h[:, CHAIN_SEQS].sum() + h[:, STALE].sum()
+    print(f"stale verdicts re-probed: {h[:, STALE].sum() / hard.sum():.0f} per stream, "
+          f"{h[:, STALE].sum() / seqs:.2%} of all sequences, {h[:, STALE].sum() / max(looked, 1):.2%} of chained lookups; "
+          f"chain cycles per chained sequence {chain.sum() / max(h[:, CHAIN_SEQS].sum(), 1):.1f}")
 
 
 if __name__ == "__main__":
