@@ -23,7 +23,8 @@ LIB_PATH = os.path.join(_HERE, "lib", "libblosc_b200.so")
 BLOSC_NOSHUFFLE, BLOSC_SHUFFLE, BLOSC_BITSHUFFLE = 0, 1, 2
 BLOSC_MAX_OVERHEAD = 16
 FILT_SHUFFLE, FILT_UNSHUFFLE, FILT_BITSHUFFLE, FILT_BITUNSHUFFLE = 0, 1, 2, 3
-KERNEL_KINDS = ("filter", "encode", "scan", "compact", "decode", "unfilter", "index", "parse", "zenc", "denc", "senc")
+KERNEL_KINDS = ("filter", "encode", "scan", "compact", "decode", "unfilter", "index", "parse", "zenc", "denc", "senc",
+                "gather")
 HAS_FAST_PARSE = True      # BLOSC_B200_PARSE=fast: segment-parallel LZ4 parse (csrc/dev_lz4fast.cuh)
 
 
@@ -62,6 +63,10 @@ def _load(path: str) -> C.CDLL:
     lib.blosc_b200_frame_decompress.argtypes = [vp, sz, vp, sz, ci]
     lib.blosc_b200_frame_getitem.restype = ll
     lib.blosc_b200_frame_getitem.argtypes = [vp, sz, sz, sz, vp]
+    lib.blosc_b200_getitems.restype = ll
+    lib.blosc_b200_getitems.argtypes = [vp, ci, vp, vp, vp]
+    lib.blosc_b200_frame_getitems.restype = ll
+    lib.blosc_b200_frame_getitems.argtypes = [vp, sz, sz, vp, vp, vp]
     lib.blosc_b200_frame_info.restype = ci
     lib.blosc_b200_frame_info.argtypes = [vp, sz, C.POINTER(sz), C.POINTER(sz), C.POINTER(sz), C.POINTER(sz)]
     lib.blosc_b200_frame_chunk.restype = ll
@@ -106,6 +111,24 @@ def getitem(src, start, nitems, dest):
     return lib.blosc_getitem(_ptr(src), start, nitems, _ptr(dest))
 
 
+def _ranges(starts, nitems, dtype):
+    """starts / nitems (sequences or numpy arrays) as two C-contiguous arrays of `dtype`, checked to have one length."""
+    import numpy as np
+    st = np.ascontiguousarray(starts, dtype=dtype).reshape(-1)
+    n = np.ascontiguousarray(nitems, dtype=dtype).reshape(-1)
+    if st.shape != n.shape:
+        raise ValueError(f"{st.size} starts but {n.size} counts")
+    return st, n
+
+
+def getitems(src, starts, nitems, dest):
+    """Many item ranges of one chunk in one call (blosc_b200_getitems): range r is items
+    [starts[r], starts[r] + nitems[r]); they land back to back in `dest`, in request order.  Returns the bytes
+    written, or blosc_getitem's code for the first bad range (dest is then untouched)."""
+    st, n = _ranges(starts, nitems, "int32")
+    return int(lib.blosc_b200_getitems(_ptr(src), st.size, st.ctypes.data, n.ctypes.data, _ptr(dest)))
+
+
 def _name(compressor):
     return compressor.encode() if isinstance(compressor, str) else compressor
 
@@ -128,6 +151,12 @@ def frame_decompress(frame, framesize, dest, destsize, numinternalthreads=1):
 
 def frame_getitem(frame, framesize, start, nitems, dest):
     return int(lib.blosc_b200_frame_getitem(_ptr(frame), framesize, start, nitems, _ptr(dest)))
+
+
+def frame_getitems(frame, framesize, starts, nitems, dest):
+    """getitems over a frame (blosc_b200_frame_getitems); ranges may cross chunk boundaries."""
+    st, n = _ranges(starts, nitems, "uint64")
+    return int(lib.blosc_b200_frame_getitems(_ptr(frame), framesize, st.size, st.ctypes.data, n.ctypes.data, _ptr(dest)))
 
 
 def frame_info(frame, framesize):

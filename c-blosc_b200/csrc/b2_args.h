@@ -153,7 +153,28 @@ typedef struct DecodeArgs {
   int* done;             /* zero-initialised count of finished streams */
   int* status_out;       /* the last warp publishes the verdict here and zeroes the three words above */
   int many;              /* other calls are running on this device: streams per SM matter more than latency */
+  const int* blocks;     /* NULL: the selected blocks are [first_block, first_block + nfull (+1)) of map.  Otherwise a
+                          * device list of block numbers (getitems; map.first_block and out_shift are 0): the j-th
+                          * listed block decodes to j * blocksize of a compact output, and a short last block can
+                          * only be the last entry.  It is not part of StreamMap so that the encoders' arguments,
+                          * and the code compiled from them, stay as they are. */
 } DecodeArgs;
+
+/* One item range of a getitems request: `len` = next.pos - pos bytes from src + `src` to dst + `dst`.  `pos` is the
+ * exclusive prefix of the lengths, so the gather splits its work by bytes; the table ends with an entry whose pos is
+ * the total.  Only non-empty ranges are listed. */
+typedef struct GatherRange {
+  long long src, dst, pos;
+} GatherRange;
+
+typedef struct GatherArgs {
+  const uint8_t* src;         /* decoded (unfiltered) scratch, or a memcpyed chunk's payload */
+  uint8_t* dst;
+  const GatherRange* ranges;  /* [nranges + 1] */
+  int nranges;
+  long long total;            /* bytes to copy = ranges[nranges].pos */
+  const int* status;          /* NULL, or the decode verdict: the gather writes nothing when it is negative */
+} GatherArgs;
 
 #ifdef __cplusplus
 }

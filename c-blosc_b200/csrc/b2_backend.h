@@ -51,9 +51,10 @@ int  b2_launch_fast(const FastArgs* a, b2_stream_t s);      /* index_kernel + pa
                                                              * a->zstd: index_kernel + zparse_kernel + zenc_kernel (zstd);
                                                              * a->deflate: index_kernel + dparse_kernel + denc_kernel (zlib);
                                                              * a->snappy: index_kernel + zparse_kernel + senc_kernel */
+int  b2_launch_gather(const GatherArgs* a, b2_stream_t s);  /* gather_kernel (getitems) */
 
 /* profiling: per-kernel-kind CUDA-event timing (off by default) */
-enum { B2_K_FILTER = 0, B2_K_ENCODE, B2_K_SCAN, B2_K_COMPACT, B2_K_DECODE, B2_K_UNFILTER, B2_K_INDEX, B2_K_PARSE, B2_K_ZENC, B2_K_DENC, B2_K_SENC, B2_K_COUNT };
+enum { B2_K_FILTER = 0, B2_K_ENCODE, B2_K_SCAN, B2_K_COMPACT, B2_K_DECODE, B2_K_UNFILTER, B2_K_INDEX, B2_K_PARSE, B2_K_ZENC, B2_K_DENC, B2_K_SENC, B2_K_GATHER, B2_K_COUNT };
 void b2_prof_enable(int on);
 void b2_prof_reset(void);
 int  b2_prof_get(int kind, double* ms_total, long long* launches);

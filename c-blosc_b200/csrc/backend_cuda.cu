@@ -374,3 +374,13 @@ extern "C" int b2_launch_decode(const DecodeArgs* a, b2_stream_t s) {
   CK(cudaGetLastError());
   return 0;
 }
+
+extern "C" int b2_launch_gather(const GatherArgs* a, b2_stream_t s) {
+  if (a->total <= 0) return 0;
+  long long ctas = (a->total + (long long)GATHER_WARPS * GATHER_SPAN - 1) / ((long long)GATHER_WARPS * GATHER_SPAN);
+  if (ctas > (long long)num_sms() * 8) ctas = (long long)num_sms() * 8;
+  ProfScope ps(B2_K_GATHER, s->s);
+  gather_kernel<<<(unsigned)ctas, GATHER_WARPS * 32, 0, s->s>>>(*a);
+  CK(cudaGetLastError());
+  return 0;
+}

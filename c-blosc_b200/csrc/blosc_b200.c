@@ -852,31 +852,33 @@ static int codec_from_header(const b2_hdr* h, int* codec) {                /* bl
   return -5;
 }
 
-/* Decode blocks [first, first+count) of a chunk that is already on the device into `d_out`
- * (device), which represents buffer offsets [first*blocksize, ...).  Shared by decompress and getitem. */
-static int decode_blocks(b2_ws* w, const b2_hdr* h, int codec, const uint8_t* d_chunk, int first, int count,
-                         uint8_t* d_out) {
+/* Launch the decode (and unfilter) of `count` blocks of a chunk that is already on the device into `d_out` (device).
+ * d_blocks NULL: blocks [first, first+count), and d_out represents buffer offsets [first*blocksize, ...).  Otherwise
+ * d_blocks is a device list of `count` ascending block numbers and the j-th decodes to d_out + j*blocksize; has_left
+ * says whether the last of them is the chunk's short last block.  The verdict lands in B2_R_STATUS_OUT. */
+static int launch_decode_blocks(b2_ws* w, const b2_hdr* h, int codec, const uint8_t* d_chunk, int first, int count,
+                                const int* d_blocks, int has_left, uint8_t* d_out) {
   DecodeArgs da;
   FilterArgs fa;
   const int ts = h->typesize, bs = h->blocksize;
   const int dont_split = (h->flags & 0x10) >> 4;
   const int doshuffle = (h->flags & BLOSC_DOSHUFFLE) && ts > 1;
   const int dobitshuffle = !doshuffle && (h->flags & BLOSC_DOBITSHUFFLE);
-  const int has_left = h->leftover > 0 && first + count == h->nblocks;
   const int nfull = count - has_left;
   const long long span = (long long)nfull * bs + (has_left ? h->leftover : 0);
   uint8_t* d_codec_out = d_out;
   memset(&da, 0, sizeof da);
   /* blosc.c:749-757: split only if typesize <= 16 and >= 128 elements per block */
   da.map.nsplits = (!dont_split && ts <= MAX_SPLITS && bs / ts >= MIN_BUFFERSIZE) ? ts : 1;
-  da.map.nbytes = h->nbytes; da.map.blocksize = bs; da.map.first_block = first; da.map.nfull = nfull;
+  da.map.nbytes = h->nbytes; da.map.blocksize = bs; da.map.first_block = d_blocks ? 0 : first; da.map.nfull = nfull;
   da.map.leftover = has_left ? h->leftover : 0;
   da.map.nstreams = nfull * da.map.nsplits + (has_left ? 1 : 0);
+  da.blocks = d_blocks;
   if (doshuffle || dobitshuffle) {
     if (buf_ensure(&w->filt, (size_t)span + 64)) return -1;
     d_codec_out = (uint8_t*)w->filt.p;
   }
-  da.chunk = d_chunk; da.cbytes = h->cbytes; da.out = d_codec_out; da.out_shift = (long long)first * bs;
+  da.chunk = d_chunk; da.cbytes = h->cbytes; da.out = d_codec_out; da.out_shift = d_blocks ? 0 : (long long)first * bs;
   da.codec = codec; da.status = w->d_result + B2_R_STATUS; da.queue = w->d_result + B2_R_QUEUE;
   da.queue_base_host = &w->queue_base;
   da.done = w->d_result + B2_R_DONE; da.status_out = w->d_result + B2_R_STATUS_OUT;
@@ -887,6 +889,15 @@ static int decode_blocks(b2_ws* w, const b2_hdr* h, int codec, const uint8_t* d_
     fa.mode = doshuffle ? FILT_UNSHUFFLE : FILT_BITUNSHUFFLE;
     if (b2_launch_filter(&fa, w->stream)) { ws_reset_counters(w); return -1; }
   }
+  return 0;
+}
+
+/* Decode blocks [first, first+count) of a chunk that is already on the device into `d_out`
+ * (device), which represents buffer offsets [first*blocksize, ...).  Shared by decompress and getitem. */
+static int decode_blocks(b2_ws* w, const b2_hdr* h, int codec, const uint8_t* d_chunk, int first, int count,
+                         uint8_t* d_out) {
+  const int has_left = h->leftover > 0 && first + count == h->nblocks;
+  if (launch_decode_blocks(w, h, codec, d_chunk, first, count, NULL, has_left, d_out)) return -1;
   if (b2_copy_d2h(w->h_result + B2_R_STATUS_OUT, w->d_result + B2_R_STATUS_OUT, 4, w->stream) || b2_stream_sync(w->stream)) {
     ws_reset_counters(w);
     return -1;
@@ -972,39 +983,53 @@ int blosc_decompress_ctx(const void* src, void* dest, size_t destsize, int numin
   return decompress_impl(src, dest, destsize, numinternalthreads, -1, -1);
 }
 
-static int getitem_impl(const void* src, int start, int nitems, void* dest, long long max_cbytes) {    /* blosc.c:1574-1703 */
+/* the chunk-header checks of blosc_getitem (blosc.c:1574-1631), with its return codes; 0 when the chunk is readable */
+static int getitem_header(const void* src, int src_dev, long long max_cbytes, b2_hdr* h, int* codec) {
   uint8_t hb[16];
-  b2_hdr h;
-  int src_dev, dest_dev, codec = 0, rc, result = -1;
-  const int stop = start + nitems;
-  b2_ws* w;
-  long long b_lo, b_hi, first, last;
-
-  src_dev = b2_ptr_is_device(src);
+  int rc;
   if (src_dev) {
-    w = ws_acquire();
+    b2_ws* w = ws_acquire();
     if (!w) return -1;
     rc = copy_any(hb, 0, src, 1, 16, w->stream);
     ws_release(w);
     if (rc) return -1;
   } else memcpy(hb, src, 16);
-  parse_header(hb, &h);
-  if (max_cbytes >= 0 && (h.cbytes < BLOSC_MAX_OVERHEAD || h.cbytes > max_cbytes)) return -1;
-  if (h.version != BLOSC_VERSION_FORMAT) return -9;
-  if (h.blocksize <= 0 || h.blocksize > h.nbytes || (size_t)h.blocksize > BLOSC_MAX_BLOCKSIZE || h.typesize <= 0)
+  parse_header(hb, h);
+  if (max_cbytes >= 0 && (h->cbytes < BLOSC_MAX_OVERHEAD || h->cbytes > max_cbytes)) return -1;
+  if (h->version != BLOSC_VERSION_FORMAT) return -9;
+  if (h->blocksize <= 0 || h->blocksize > h->nbytes || (size_t)h->blocksize > BLOSC_MAX_BLOCKSIZE || h->typesize <= 0)
     return -1;
-  h.nblocks = h.nbytes / h.blocksize; h.leftover = h.nbytes % h.blocksize;
-  if (h.leftover > 0) h.nblocks++;
-  if (h.flags & BLOSC_MEMCPYED) {
-    if (h.nbytes + BLOSC_MAX_OVERHEAD != h.cbytes) return -1;
+  h->nblocks = h->nbytes / h->blocksize; h->leftover = h->nbytes % h->blocksize;
+  if (h->leftover > 0) h->nblocks++;
+  if (h->flags & BLOSC_MEMCPYED) {
+    if (h->nbytes + BLOSC_MAX_OVERHEAD != h->cbytes) return -1;
   } else {
-    rc = codec_from_header(&h, &codec);
+    rc = codec_from_header(h, codec);
     if (rc) return rc;
-    if (h.nblocks >= (h.cbytes - 16) / 4) return -1;                       /* :1630 */
+    if (h->nblocks >= (h->cbytes - 16) / 4) return -1;                     /* :1630 */
   }
-  if (start < 0 || (long long)start * h.typesize > h.nbytes) { fprintf(stderr, "`start` out of bounds"); return -1; }
-  if (stop < 0 || (long long)stop * h.typesize > h.nbytes) { fprintf(stderr, "`start`+`nitems` out of bounds"); return -1; }
-  b_lo = (long long)start * h.typesize; b_hi = (long long)stop * h.typesize;
+  return 0;
+}
+
+/* blosc_getitem's bounds checks of one range (blosc.c:1633-1644): its bytes [*b_lo, *b_hi), empty when b_hi <= b_lo */
+static int getitem_range(const b2_hdr* h, int start, int nitems, long long* b_lo, long long* b_hi) {
+  const int stop = (int)((unsigned)start + (unsigned)nitems);
+  if (start < 0 || (long long)start * h->typesize > h->nbytes) { fprintf(stderr, "`start` out of bounds"); return -1; }
+  if (stop < 0 || (long long)stop * h->typesize > h->nbytes) { fprintf(stderr, "`start`+`nitems` out of bounds"); return -1; }
+  *b_lo = (long long)start * h->typesize; *b_hi = (long long)stop * h->typesize;
+  return 0;
+}
+
+static int getitem_impl(const void* src, int start, int nitems, void* dest, long long max_cbytes) {    /* blosc.c:1574-1703 */
+  b2_hdr h;
+  int src_dev, dest_dev, codec = 0, rc, result = -1;
+  b2_ws* w;
+  long long b_lo, b_hi, first, last;
+
+  src_dev = b2_ptr_is_device(src);
+  rc = getitem_header(src, src_dev, max_cbytes, &h, &codec);
+  if (rc) return rc;
+  if (getitem_range(&h, start, nitems, &b_lo, &b_hi)) return -1;
   if (b_hi <= b_lo) return 0;                                              /* no block overlaps: loop copies nothing */
   dest_dev = b2_ptr_is_device(dest);
 
@@ -1059,6 +1084,210 @@ static int getitem_impl(const void* src, int start, int nitems, void* dest, long
 }
 
 int blosc_getitem(const void* src, int start, int nitems, void* dest) { return getitem_impl(src, start, nitems, dest, -1); }
+
+/* ------------------------------------------------------------------------- */
+/* many item ranges of one chunk in one pass (blosc_b200_getitems)             */
+/* ------------------------------------------------------------------------- */
+/* Every block that some range overlaps is decoded exactly once, by one decode launch over the sorted list of those
+ * blocks: the j-th listed block decodes to j * blocksize of a compact scratch (StreamMap.blocks).  A range covers a
+ * run of consecutive blocks, which stay adjacent in the list, so it is one contiguous span of the scratch.  One
+ * unfilter launch and one gather launch (gather_kernel) then copy every range to its place in dest. */
+typedef struct { long long lo, hi; } b2_iv;
+
+static int cmp_iv(const void* a, const void* b) {
+  const b2_iv *x = (const b2_iv*)a, *y = (const b2_iv*)b;
+  return x->lo < y->lo ? -1 : x->lo > y->lo;
+}
+static int cmp_i32(const void* a, const void* b) {
+  const int32_t x = *(const int32_t*)a, y = *(const int32_t*)b;
+  return x < y ? -1 : x > y;
+}
+
+/* sorts iv[0..n) by lo and merges the intervals that overlap or touch (hi is exclusive); returns the new count */
+static int merge_ivs(b2_iv* iv, int n) {
+  int k = 0, i;
+  if (n == 0) return 0;
+  qsort(iv, (size_t)n, sizeof *iv, cmp_iv);
+  for (i = 1; i < n; i++) {
+    if (iv[i].lo <= iv[k].hi) { if (iv[i].hi > iv[k].hi) iv[k].hi = iv[i].hi; }
+    else iv[++k] = iv[i];
+  }
+  return k + 1;
+}
+
+/* Stage what the decoder reads of a host-resident chunk: the header with bstarts[] and, for every listed block, its
+ * bytes from its bstart to the next bstart above it (as getitem_impl does for one span); adjacent spans are copied as
+ * one.  -1 when a listed block's bstart is out of bounds (blosc_d would refuse it, blosc.c:761). */
+static int stage_blocks(b2_ws* w, const b2_hdr* h, const uint8_t* hs, const int* blocks, int count) {
+  const size_t index_end = 16 + 4 * (size_t)h->nblocks;
+  int32_t* sorted = (int32_t*)malloc(4 * (size_t)h->nblocks + 4);
+  b2_iv* iv = (b2_iv*)malloc(sizeof(b2_iv) * (size_t)count + sizeof(b2_iv));
+  int i, n = 0, rc = -1;
+  do {
+    if (!sorted || !iv) break;
+    for (i = 0; i < h->nblocks; i++) sorted[i] = rd_i32(hs + 16 + 4 * (size_t)i);
+    qsort(sorted, (size_t)h->nblocks, 4, cmp_i32);
+    for (i = 0; i < count; i++) {
+      const int32_t bs_b = rd_i32(hs + 16 + 4 * (size_t)blocks[i]);
+      int lo = 0, hi = h->nblocks;
+      if (bs_b < (int32_t)index_end || bs_b > h->cbytes) break;
+      while (lo < hi) { const int m = (lo + hi) / 2; if (sorted[m] <= bs_b) lo = m + 1; else hi = m; }   /* first above */
+      iv[n].lo = bs_b;
+      iv[n].hi = (lo < h->nblocks && sorted[lo] < h->cbytes) ? sorted[lo] : h->cbytes;
+      n++;
+    }
+    if (i < count) break;
+    n = merge_ivs(iv, n);
+    if (buf_ensure(&w->in, (size_t)h->cbytes + 64)) break;
+    if (h2d_any(w, w->in.p, hs, index_end)) break;
+    for (i = 0; i < n; i++)
+      if (h2d_any(w, (uint8_t*)w->in.p + iv[i].lo, hs + iv[i].lo, (size_t)(iv[i].hi - iv[i].lo))) break;
+    rc = i < n ? -1 : 0;
+  } while (0);
+  free(sorted); free(iv);
+  return rc;
+}
+
+/* The range table of the gather, in one copy.  A host dest receives the ranges packed, from a device staging buffer
+ * (w->slots), so their destinations become their positions in it. */
+static int upload_ranges(b2_ws* w, GatherRange* tab, int nr, long long total, int dest_dev) {
+  int r;
+  if (!dest_dev) {
+    for (r = 0; r < nr; r++) tab[r].dst = tab[r].pos;
+    if (buf_ensure(&w->slots, (size_t)total + 64)) return -1;
+  }
+  if (buf_ensure(&w->segs, sizeof(GatherRange) * ((size_t)nr + 1) + 64)) return -1;
+  return b2_copy_h2d(w->segs.p, tab, sizeof(GatherRange) * ((size_t)nr + 1), w->stream);
+}
+
+/* `n` ranges of one chunk; range r goes to dest + dsts[r] (back to back in request order when dsts is NULL).  The
+ * header and every range are validated before anything is launched or written.  Returns the bytes written. */
+static long long getitems_chunk(const void* src, long long max_cbytes, int n, const int* starts, const int* nitems,
+                                const long long* dsts, void* dest) {
+  b2_hdr h;
+  int src_dev, dest_dev, codec = 0, rc, r, nr = 0, contiguous = 1;
+  long long total = 0, result = -1;
+  b2_ws* w = NULL;
+  GatherRange* tab = NULL;       /* [nr + 1] non-empty ranges; src: offset in the gather's source, set once that is known */
+  long long* lo_b = NULL;        /* [2n]: first byte of each listed range inside the chunk, then its dest offset */
+  long long* at_b;
+  b2_iv* iv = NULL;
+  int* blocks = NULL;
+  uint8_t* tmp = NULL;
+
+  if (n <= 0) return 0;
+  src_dev = b2_ptr_is_device(src);
+  rc = getitem_header(src, src_dev, max_cbytes, &h, &codec);
+  if (rc) return rc;
+  tab = (GatherRange*)malloc(sizeof(GatherRange) * ((size_t)n + 1));
+  lo_b = (long long*)malloc(2 * sizeof(long long) * (size_t)n);
+  if (!tab || !lo_b) { free(tab); free(lo_b); return -1; }
+  at_b = lo_b + n;
+  for (r = 0; r < n; r++) {
+    long long b_lo, b_hi;
+    const long long at = dsts ? dsts[r] : total;
+    if (getitem_range(&h, starts[r], nitems[r], &b_lo, &b_hi)) { free(tab); free(lo_b); return -1; }
+    if (b_hi <= b_lo) continue;                                            /* empty: 0 bytes, as blosc_getitem */
+    tab[nr].src = b_lo; tab[nr].dst = at; tab[nr].pos = total;
+    lo_b[nr] = b_lo; at_b[nr] = at;
+    contiguous &= at - tab[0].dst == total;
+    total += b_hi - b_lo;
+    nr++;
+  }
+  tab[nr].src = tab[nr].dst = 0; tab[nr].pos = total;
+  if (nr == 0) { free(tab); free(lo_b); return 0; }
+  dest_dev = b2_ptr_is_device(dest);
+
+  if ((h.flags & BLOSC_MEMCPYED) && !src_dev && !dest_dev) {               /* :1678-1683, host to host */
+    for (r = 0; r < nr; r++)
+      memcpy((uint8_t*)dest + tab[r].dst, (const uint8_t*)src + 16 + tab[r].src, (size_t)(tab[r + 1].pos - tab[r].pos));
+    free(tab); free(lo_b);
+    return total;
+  }
+
+  w = ws_acquire();
+  if (!w) { free(tab); free(lo_b); return -1; }
+  do {
+    GatherArgs ga;
+    const uint8_t* d_src;
+    const int* status = NULL;
+    memset(&ga, 0, sizeof ga);
+    if (h.flags & BLOSC_MEMCPYED) {
+      if (src_dev) d_src = (const uint8_t*)src + 16;                       /* ranges read the payload in place */
+      else {                                                               /* the ranges, packed, cross PCIe once */
+        if (!(tmp = (uint8_t*)malloc((size_t)total))) break;
+        for (r = 0; r < nr; r++) {
+          memcpy(tmp + tab[r].pos, (const uint8_t*)src + 16 + tab[r].src, (size_t)(tab[r + 1].pos - tab[r].pos));
+          tab[r].src = tab[r].pos;
+        }
+        if (buf_ensure(&w->in, (size_t)total + 64) || h2d_any(w, w->in.p, tmp, (size_t)total)) break;
+        d_src = (const uint8_t*)w->in.p;
+      }
+    } else {
+      /* the touched blocks: one interval of block numbers per range, merged, then listed in ascending order */
+      const int bs = h.blocksize;
+      int nv, count = 0, k;
+      const uint8_t* d_chunk;
+      if (!(iv = (b2_iv*)malloc(sizeof(b2_iv) * (size_t)nr))) break;
+      for (r = 0; r < nr; r++) {
+        iv[r].lo = lo_b[r] / bs;
+        iv[r].hi = (lo_b[r] + (tab[r + 1].pos - tab[r].pos) - 1) / bs + 1;
+      }
+      nv = merge_ivs(iv, nr);
+      for (k = 0; k < nv; k++) count += (int)(iv[k].hi - iv[k].lo);
+      if (!(blocks = (int*)malloc(sizeof(int) * (size_t)count))) break;
+      for (k = 0, count = 0; k < nv; k++) {
+        long long b;
+        for (b = iv[k].lo; b < iv[k].hi; b++) blocks[count++] = (int)b;
+      }
+      for (r = 0; r < nr; r++) {                                           /* range r -> its span of the scratch */
+        const long long first = lo_b[r] / bs;
+        int lo = 0, hi = count - 1;
+        while (lo < hi) { const int m = (lo + hi + 1) / 2; if (blocks[m] <= first) lo = m; else hi = m - 1; }
+        tab[r].src = (long long)lo * bs + (lo_b[r] - first * bs);
+      }
+      if (src_dev) d_chunk = (const uint8_t*)src;
+      else {
+        if (stage_blocks(w, &h, (const uint8_t*)src, blocks, count)) break;
+        d_chunk = (const uint8_t*)w->in.p;
+      }
+      if (buf_ensure(&w->bstarts, sizeof(int) * (size_t)count + 64)) break;
+      if (b2_copy_h2d(w->bstarts.p, blocks, sizeof(int) * (size_t)count, w->stream)) break;
+      if (buf_ensure(&w->out, (size_t)count * (size_t)bs + 64)) break;
+      if (upload_ranges(w, tab, nr, total, dest_dev)) break;      /* before the decode: a pageable copy would wait for it */
+      if (launch_decode_blocks(w, &h, codec, d_chunk, 0, count, (const int*)w->bstarts.p,
+                               h.leftover > 0 && blocks[count - 1] == h.nblocks - 1, (uint8_t*)w->out.p)) break;
+      d_src = (const uint8_t*)w->out.p;
+      status = w->d_result + B2_R_STATUS_OUT;
+    }
+    if (h.flags & BLOSC_MEMCPYED && upload_ranges(w, tab, nr, total, dest_dev)) break;
+    ga.src = d_src; ga.dst = dest_dev ? (uint8_t*)dest : (uint8_t*)w->slots.p; ga.ranges = (const GatherRange*)w->segs.p;
+    ga.nranges = nr; ga.total = total; ga.status = status;
+    if (b2_launch_gather(&ga, w->stream)) { ws_reset_counters(w); break; }
+    if (b2_copy_d2h(w->h_result + B2_R_STATUS_OUT, w->d_result + B2_R_STATUS_OUT, 4, w->stream) || b2_stream_sync(w->stream)) {
+      ws_reset_counters(w);
+      break;
+    }
+    if (status && w->h_result[B2_R_STATUS_OUT] < 0) { result = w->h_result[B2_R_STATUS_OUT]; break; }
+    if (!dest_dev) {
+      if (contiguous) {
+        if (d2h_any(w, (uint8_t*)dest + at_b[0], w->slots.p, (size_t)total)) break;
+      } else {                                                             /* scattered (frame pieces) */
+        if (!tmp && !(tmp = (uint8_t*)malloc((size_t)total))) break;
+        if (d2h_any(w, tmp, w->slots.p, (size_t)total)) break;
+        for (r = 0; r < nr; r++) memcpy((uint8_t*)dest + at_b[r], tmp + tab[r].pos, (size_t)(tab[r + 1].pos - tab[r].pos));
+      }
+    }
+    result = total;
+  } while (0);
+  ws_release(w);
+  free(tab); free(lo_b); free(iv); free(blocks); free(tmp);
+  return result;
+}
+
+long long blosc_b200_getitems(const void* src, int nranges, const int* starts, const int* nitems, void* dest) {
+  return getitems_chunk(src, -1, nranges, starts, nitems, NULL, dest);
+}
 
 /* ------------------------------------------------------------------------- */
 /* frames: buffers larger than one chunk (SURVEY.md section 8, row f3)           */
@@ -1376,6 +1605,85 @@ long long blosc_b200_frame_getitem(const void* frame, size_t framesize, size_t s
     }
   } while (0);
   free(off);
+  return result;
+}
+
+/* One piece of a frame range: the part that falls in one chunk */
+typedef struct { size_t chunk, order; int start, nitems; long long dst; } b2_piece;
+
+static int cmp_piece(const void* a, const void* b) {
+  const b2_piece *x = (const b2_piece*)a, *y = (const b2_piece*)b;
+  if (x->chunk != y->chunk) return x->chunk < y->chunk ? -1 : 1;
+  return x->order < y->order ? -1 : x->order > y->order;
+}
+
+/* Every range is checked as blosc_b200_frame_getitem checks one before anything is read; then the ranges are cut at
+ * chunk boundaries and each touched chunk runs the chunk plan once, each piece landing at its own dest offset. */
+long long blosc_b200_frame_getitems(const void* frame, size_t framesize, size_t nranges, const size_t* starts,
+                                    const size_t* nitems, void* dest) {
+  size_t nb = 0, cs = 0, nc = 0, ts = 0, ipc, r, npieces = 0, i, j;
+  uint64_t* off = NULL;
+  uint8_t hb[16];
+  b2_piece* pieces = NULL;
+  long long result = -1, at = 0;
+  if (nranges == 0) return 0;
+  if (!backend_ready()) return -1;
+  if (frame_open(frame, framesize, &nb, &cs, &nc, &off)) return -1;
+  do {
+    if (nc == 0) {
+      for (r = 0; r < nranges && nitems[r] == 0; r++) {}
+      result = r == nranges ? 0 : -1;
+      break;
+    }
+    if (b2_ptr_is_device(frame)) {
+      b2_ws* w = ws_acquire();
+      int rc = w ? copy_any(hb, 0, (const uint8_t*)frame + off[0], 1, 16, w->stream) : -1;
+      if (w) ws_release(w);
+      if (rc) break;
+    } else memcpy(hb, (const uint8_t*)frame + off[0], 16);
+    ts = hb[3];
+    if (ts == 0 || cs % ts) break;
+    ipc = cs / ts;                                     /* items per chunk */
+    for (r = 0; r < nranges; r++) {
+      if (starts[r] > nb / ts || nitems[r] > nb / ts - starts[r]) { fprintf(stderr, "`start`+`nitems` out of bounds"); break; }
+      npieces += nitems[r] ? (starts[r] + nitems[r] - 1) / ipc - starts[r] / ipc + 1 : 0;
+    }
+    if (r < nranges) break;
+    if (npieces == 0) { result = 0; break; }
+    if (!(pieces = (b2_piece*)malloc(sizeof(b2_piece) * npieces))) break;
+    for (r = 0, npieces = 0; r < nranges; r++) {
+      size_t done = 0;
+      while (done < nitems[r]) {
+        const size_t c = (starts[r] + done) / ipc, first = (starts[r] + done) % ipc;
+        const size_t take = nitems[r] - done < ipc - first ? nitems[r] - done : ipc - first;
+        pieces[npieces].chunk = c; pieces[npieces].order = npieces;
+        pieces[npieces].start = (int)first; pieces[npieces].nitems = (int)take;
+        pieces[npieces].dst = at + (long long)(done * ts);
+        npieces++;
+        done += take;
+      }
+      at += (long long)(nitems[r] * ts);
+    }
+    qsort(pieces, npieces, sizeof *pieces, cmp_piece);
+    result = 0;
+    for (i = 0; i < npieces; i = j) {
+      int* st;
+      long long* dsts;
+      long long want = 0, rc;
+      size_t k;
+      for (j = i; j < npieces && pieces[j].chunk == pieces[i].chunk; j++) want += (long long)pieces[j].nitems * (long long)ts;
+      st = (int*)malloc(2 * sizeof(int) * (j - i));
+      dsts = (long long*)malloc(sizeof(long long) * (j - i));
+      if (!st || !dsts) { free(st); free(dsts); result = -1; break; }
+      for (k = i; k < j; k++) { st[k - i] = pieces[k].start; st[j - i + k - i] = pieces[k].nitems; dsts[k - i] = pieces[k].dst; }
+      rc = getitems_chunk((const uint8_t*)frame + off[pieces[i].chunk], (long long)(off[pieces[i].chunk + 1] - off[pieces[i].chunk]),
+                          (int)(j - i), st, st + (j - i), dsts, dest);
+      free(st); free(dsts);
+      if (rc != want) { result = rc < 0 ? rc : -1; break; }
+      result += rc;
+    }
+  } while (0);
+  free(pieces); free(off);
   return result;
 }
 

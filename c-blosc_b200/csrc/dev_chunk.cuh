@@ -48,8 +48,11 @@ DEV int next_stream(int* queue, unsigned base, const StreamMap& m) {
   return b * m.nsplits + s;
 }
 
-/* stream index -> (block, offset inside the uncompressed buffer, length) */
-DEV void stream_locate(const StreamMap& m, int idx, int* block, long long* off, int* len, int* split) {
+/* stream index -> (block, offset inside the uncompressed buffer, length).  With a block list (DecodeArgs.blocks,
+ * getitems) first_block is 0, so the offset computed for the j-th selected block is already j * blocksize of the
+ * compact output (the caller's out_shift is 0); only the block number comes from the list. */
+DEV void stream_locate(const StreamMap& m, int idx, int* block, long long* off, int* len, int* split,
+                       const int* blocks = nullptr) {
   const int nfs = m.nfull * m.nsplits;
   if (idx < nfs) {
     const int b = idx / m.nsplits, s = idx - b * m.nsplits;
@@ -64,6 +67,7 @@ DEV void stream_locate(const StreamMap& m, int idx, int* block, long long* off, 
     *len = m.leftover;
     *split = 0;
   }
+  if (blocks) *block = blocks[*block];
 }
 
 
@@ -764,7 +768,7 @@ DEV void decode_streams(const DecodeArgs& a, Codec codec) {
     if (idx < 0) break;
     int block, len, split;
     long long off;
-    stream_locate(a.map, idx, &block, &off, &len, &split);
+    stream_locate(a.map, idx, &block, &off, &len, &split, a.blocks);
     int so = ld_i32(a.chunk + 16 + 4ll * block);
     int cs = 0, err = 0;
     for (int s = 0; s <= split; s++) {
@@ -817,6 +821,65 @@ __global__ void __launch_bounds__(DECODE_WARPS * 32) decode_kernel(DecodeArgs a)
     return blz_decode_warp(src, cs, out, len);
   });
 }
+
+
+/* getitems: copies every requested range out of the compact scratch that one decode (and unfilter) launch made of
+ * the touched blocks.  Work is cut by bytes, not by range, so a long range does not serialise the launch: warp job k
+ * covers bytes [k * GATHER_SPAN, (k + 1) * GATHER_SPAN) of the concatenated ranges and binary-searches the prefix of
+ * range lengths for its first range.  Each piece is copied 16 bytes per lane when source and destination share their
+ * alignment mod 16, bytewise at the edges and otherwise. */
+#define GATHER_WARPS 8
+#define GATHER_SPAN 8192
+DEV void warp_copy_vec(u8* __restrict__ dst, const u8* __restrict__ src, int n) {
+  const int lane = lane_id();
+  if ((((uintptr_t)dst ^ (uintptr_t)src) & 15u) == 0 && n >= 32) {
+    const int head = (int)((16u - ((uintptr_t)dst & 15u)) & 15u);
+    if (lane < head) dst[lane] = src[lane];
+    const int nv = (n - head) >> 4;
+    const uint4* s4 = (const uint4*)(src + head);
+    uint4* d4 = (uint4*)(dst + head);
+    for (int i = lane; i < nv; i += 32) d4[i] = s4[i];
+    for (int i = head + (nv << 4) + lane; i < n; i += 32) dst[i] = src[i];
+  } else {
+    for (int i = lane; i < n; i += 32) dst[i] = src[i];
+  }
+}
+
+__global__ void __launch_bounds__(GATHER_WARPS * 32) gather_kernel(GatherArgs a) {
+  if (a.status && ld_cg_i32(a.status) < 0) return;       /* a stream failed to decode: dest stays untouched */
+  const long long warps = (long long)gridDim.x * GATHER_WARPS;
+  for (long long lo = ((long long)blockIdx.x * GATHER_WARPS + (threadIdx.x >> 5)) * GATHER_SPAN; lo < a.total;
+       lo += warps * GATHER_SPAN) {
+    const long long hi = lo + GATHER_SPAN < a.total ? lo + GATHER_SPAN : a.total;
+    int l = 0, h = a.nranges - 1;                          /* the last range with pos <= lo */
+    while (l < h) {
+      const int m = (l + h + 1) >> 1;
+      if (a.ranges[m].pos <= lo) l = m; else h = m - 1;
+    }
+    for (int r = l; r < a.nranges; r++) {
+      const GatherRange g = a.ranges[r];
+      if (g.pos >= hi) break;
+      const long long end = a.ranges[r + 1].pos;
+      const long long p0 = lo > g.pos ? lo : g.pos, p1 = hi < end ? hi : end;
+      warp_copy_vec(a.dst + g.dst + (p0 - g.pos), a.src + g.src + (p0 - g.pos), (int)(p1 - p0));
+    }
+  }
+}
+
+#ifdef SIMT_EMU
+/* The CPU emulator's launcher of gather_kernel (the other kernels are launched by tests/emu/backend_emu.cpp, which
+ * includes this header): a few CTAs, so that every warp goes through several spans.  It counts its own launches. */
+static long long g_emu_gather_launches = 0;
+extern "C" int b2_launch_gather(const GatherArgs* a, b2_stream_t) {
+  if (a->total <= 0) return 0;
+  long long ctas = (a->total + (long long)GATHER_WARPS * GATHER_SPAN - 1) / ((long long)GATHER_WARPS * GATHER_SPAN);
+  if (ctas > 3) ctas = 3;
+  g_emu_gather_launches++;
+  GatherArgs args = *a;
+  simt::launch(simt::Dim3((unsigned)ctas), simt::Dim3(GATHER_WARPS * 32), 0, [&] { gather_kernel(args); });
+  return 0;
+}
+#endif
 
 
 /* LZ4 chunks: one CTA of two warps per stream -- a parser that walks the tokens and a copier that owns the output

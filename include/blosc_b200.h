@@ -147,6 +147,14 @@ const char* blosc_cbuffer_complib(const void* cbuffer);                         
  * src/dest host or device.  Returns 0, or -1 on device failure. */
 int blosc_b200_filter(int mode, size_t typesize, size_t blocksize, const void* src, void* dest);
 
+/* Many item ranges of one chunk in one call.  Range r covers items [starts[r], starts[r] + nitems[r]) in elements of
+ * the chunk's typesize.  Each range is validated exactly as blosc_getitem validates one.  Ranges may be unsorted,
+ * overlap or repeat.  They are written back to back into dest in request order.  starts / nitems are host arrays;
+ * src / dest are host or device.  Every block that some range overlaps is decoded once, by one decode launch, however
+ * many ranges touch it.  Returns the total bytes written, or the code blosc_getitem would return for the first range
+ * that fails; in that case nothing is written to dest.  nranges == 0 returns 0. */
+long long blosc_b200_getitems(const void* src, int nranges, const int* starts, const int* nitems, void* dest);
+
 /* Frames: buffers larger than one chunk (a Blosc-1 chunk holds at most BLOSC_MAX_BUFFERSIZE
  * bytes, blosc.h:40).  The buffer is cut into `chunksize`-byte pieces (0 = 256 MiB; rounded down
  * to a multiple of typesize), each compressed exactly as blosc_compress_ctx() would with
@@ -163,6 +171,10 @@ long long blosc_b200_frame_compress(int clevel, int doshuffle, size_t typesize, 
 long long blosc_b200_frame_decompress(const void* frame, size_t framesize, void* dest, size_t destsize,
                                       int numinternalthreads);
 long long blosc_b200_frame_getitem(const void* frame, size_t framesize, size_t start, size_t nitems, void* dest);
+/* blosc_b200_getitems over a frame: ranges may cross chunk boundaries, as in blosc_b200_frame_getitem, and are
+ * written back to back into dest in request order.  Every range is checked before anything is read. */
+long long blosc_b200_frame_getitems(const void* frame, size_t framesize, size_t nranges, const size_t* starts,
+                                    const size_t* nitems, void* dest);
 int       blosc_b200_frame_info(const void* frame, size_t framesize, size_t* nbytes, size_t* cbytes,
                                 size_t* chunksize, size_t* nchunks);
 long long blosc_b200_frame_chunk(const void* frame, size_t framesize, size_t i, size_t* chunk_cbytes);
@@ -172,7 +184,8 @@ long long blosc_b200_frame_chunk(const void* frame, size_t framesize, size_t i, 
 int blosc_b200_set_device(int dev);
 
 /* Per-kernel CUDA-event timing of the calls made since the last reset (bench.py's roofline
- * leg).  kind: 0 filter, 1 encode, 2 scan, 3 compact, 4 decode, 5 unfilter. */
+ * leg).  kind: 0 filter, 1 encode, 2 scan, 3 compact, 4 decode, 5 unfilter, 6 index, 7 parse, 8 zenc, 9 denc,
+ * 10 senc, 11 gather. */
 void blosc_b200_set_profiling(int on);
 void blosc_b200_prof_reset(void);
 int  blosc_b200_prof_get(int kind, double* ms_total, long long* launches);
