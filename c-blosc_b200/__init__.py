@@ -24,7 +24,7 @@ BLOSC_NOSHUFFLE, BLOSC_SHUFFLE, BLOSC_BITSHUFFLE = 0, 1, 2
 BLOSC_MAX_OVERHEAD = 16
 FILT_SHUFFLE, FILT_UNSHUFFLE, FILT_BITSHUFFLE, FILT_BITUNSHUFFLE = 0, 1, 2, 3
 KERNEL_KINDS = ("filter", "encode", "scan", "compact", "decode", "unfilter", "index", "parse", "zenc", "denc", "senc",
-                "gather")
+                "gather", "plan")
 HAS_FAST_PARSE = True      # BLOSC_B200_PARSE=fast: segment-parallel LZ4 parse (csrc/dev_lz4fast.cuh)
 
 
@@ -111,22 +111,39 @@ def getitem(src, start, nitems, dest):
     return lib.blosc_getitem(_ptr(src), start, nitems, _ptr(dest))
 
 
-def _ranges(starts, nitems, dtype):
-    """starts / nitems (sequences or numpy arrays) as two C-contiguous arrays of `dtype`, checked to have one length."""
+def _is_cuda(a):
+    return getattr(a, "is_cuda", False)
+
+
+def _range_list(a, dtype, cuda_dtypes):
+    """One range list as (array or tensor to keep alive, its address, its length).  A CUDA tensor stays on its device
+    (made contiguous there) and must already have one of `cuda_dtypes`: a cast on the device could silently truncate.
+    Sequences and numpy arrays become C-contiguous host arrays of `dtype`."""
+    if _is_cuda(a):
+        if str(a.dtype) not in cuda_dtypes:
+            raise TypeError(f"CUDA range lists must be {' or '.join(cuda_dtypes)}, not {a.dtype}")
+        t = a.contiguous().reshape(-1)
+        return t, t.data_ptr(), t.numel()
     import numpy as np
-    st = np.ascontiguousarray(starts, dtype=dtype).reshape(-1)
-    n = np.ascontiguousarray(nitems, dtype=dtype).reshape(-1)
-    if st.shape != n.shape:
-        raise ValueError(f"{st.size} starts but {n.size} counts")
+    h = np.ascontiguousarray(a, dtype=dtype).reshape(-1)
+    return h, h.ctypes.data, h.size
+
+
+def _ranges(starts, nitems, dtype, cuda_dtypes):
+    """starts / nitems (sequences, numpy arrays or CUDA tensors) as two lists checked to have one length"""
+    st, n = _range_list(starts, dtype, cuda_dtypes), _range_list(nitems, dtype, cuda_dtypes)
+    if st[2] != n[2]:
+        raise ValueError(f"{st[2]} starts but {n[2]} counts")
     return st, n
 
 
 def getitems(src, starts, nitems, dest):
     """Many item ranges of one chunk in one call (blosc_b200_getitems): range r is items
     [starts[r], starts[r] + nitems[r]); they land back to back in `dest`, in request order.  Returns the bytes
-    written, or blosc_getitem's code for the first bad range (dest is then untouched)."""
-    st, n = _ranges(starts, nitems, "int32")
-    return int(lib.blosc_b200_getitems(_ptr(src), st.size, st.ctypes.data, n.ctypes.data, _ptr(dest)))
+    written, or blosc_getitem's code for the first bad range (dest is then untouched).  starts / nitems may be
+    int32 CUDA tensors, on the device of the call: the read is then planned on the GPU."""
+    st, n = _ranges(starts, nitems, "int32", ("torch.int32",))
+    return int(lib.blosc_b200_getitems(_ptr(src), st[2], st[1], n[1], _ptr(dest)))
 
 
 def _name(compressor):
@@ -154,9 +171,10 @@ def frame_getitem(frame, framesize, start, nitems, dest):
 
 
 def frame_getitems(frame, framesize, starts, nitems, dest):
-    """getitems over a frame (blosc_b200_frame_getitems); ranges may cross chunk boundaries."""
-    st, n = _ranges(starts, nitems, "uint64")
-    return int(lib.blosc_b200_frame_getitems(_ptr(frame), framesize, st.size, st.ctypes.data, n.ctypes.data, _ptr(dest)))
+    """getitems over a frame (blosc_b200_frame_getitems); ranges may cross chunk boundaries.  starts / nitems may be
+    int64 or uint64 CUDA tensors (copied to the host for the plan)."""
+    st, n = _ranges(starts, nitems, "uint64", ("torch.int64", "torch.uint64"))
+    return int(lib.blosc_b200_frame_getitems(_ptr(frame), framesize, st[2], st[1], n[1], _ptr(dest)))
 
 
 def frame_info(frame, framesize):

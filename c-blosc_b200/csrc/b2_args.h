@@ -162,7 +162,8 @@ typedef struct DecodeArgs {
 
 /* One item range of a getitems request: `len` = next.pos - pos bytes from src + `src` to dst + `dst`.  `pos` is the
  * exclusive prefix of the lengths, so the gather splits its work by bytes; the table ends with an entry whose pos is
- * the total.  Only non-empty ranges are listed. */
+ * the total.  The host plan lists only non-empty ranges; the GPU plan keeps empty ones, which copy nothing (next.pos ==
+ * pos). */
 typedef struct GatherRange {
   long long src, dst, pos;
 } GatherRange;
@@ -175,6 +176,65 @@ typedef struct GatherArgs {
   long long total;            /* bytes to copy = ranges[nranges].pos */
   const int* status;          /* NULL, or the decode verdict: the gather writes nothing when it is negative */
 } GatherArgs;
+
+/* blosc_getitem's bounds checks of one range (blosc.c:1633-1644), the one statement of them: the host plan of getitems
+ * (blosc_b200.c getitem_range) and its GPU plan (dev_chunk.cuh plan_check_kernel) both call it.  0: the range is
+ * valid and covers bytes [*b_lo, *b_hi), empty when b_hi <= b_lo; 1: `start` is out of bounds; 2: `start`+`nitems` is.
+ * The stop wraps as the reference's int sum does. */
+#ifdef __CUDACC__
+#define B2_HD __host__ __device__
+#else
+#define B2_HD
+#endif
+static inline B2_HD int b2_range_check(int start, int nitems, int typesize, long long nbytes, long long* b_lo,
+                                       long long* b_hi) {
+  const int stop = (int)((unsigned)start + (unsigned)nitems);
+  if (start < 0 || (long long)start * typesize > nbytes) return 1;
+  if (stop < 0 || (long long)stop * typesize > nbytes) return 2;
+  *b_lo = (long long)start * typesize; *b_hi = (long long)stop * typesize;
+  return 0;
+}
+
+/* What the GPU plan of getitems leaves for the host, read back with one small copy */
+typedef struct GetitemsPlan {
+  unsigned bad;          /* index of the first failing range; 0xffffffff when every range is valid */
+  int nlisted;           /* touched blocks, listed in ascending order */
+  int has_left;          /* whether the chunk's short last block is one of them */
+  int pad;
+  long long total;       /* bytes of all ranges */
+} GetitemsPlan;
+
+/* The tile state of one device-wide scan (dev_chunk.cuh plan_scan_kernel, single pass with decoupled look-back) */
+typedef struct PlanScan {
+  unsigned* ticket;      /* zeroed: CTAs take tiles in the order they start, so a tile only waits for running ones */
+  unsigned* flag;        /* [tiles], zeroed: 1 when the tile's aggregate is published, 2 when its inclusive prefix is */
+  void* agg;             /* [tiles] of the scan's value type */
+  void* inc;             /* [tiles] */
+} PlanScan;
+
+/* getitems planned on the GPU from device-resident range lists: the gather table and the touched-block list the host
+ * plan would build.  Kernels: plan_check_kernel, then (unless in_place) the block scans PLAN_COVER and PLAN_SLOT over
+ * nblocks, then PLAN_POS over the ranges, which also fills the table. */
+typedef struct PlanArgs {
+  const int* starts;
+  const int* nitems;
+  int nranges;
+  int typesize, blocksize, nblocks;
+  int leftover;          /* the chunk has a short last block */
+  long long nbytes;
+  int in_place;          /* a memcpyed chunk in device memory: the gather reads the payload itself, no block list */
+  long long* len;        /* [nranges] bytes of each range; 0 when it is empty or fails */
+  int* cover;            /* [nblocks + 1], zeroed: +1 at each range's first block, -1 after its last; then coverage */
+  int* slot;             /* [nblocks] position of a touched block in the list */
+  int* blocks;           /* [nblocks] the touched blocks, ascending */
+  GatherRange* ranges;   /* [nranges + 1] the gather table, in request order, empty ranges included */
+  GetitemsPlan* rec;     /* zeroed but for rec->bad = 0xffffffff */
+  PlanScan scan[3];      /* PLAN_COVER, PLAN_SLOT, PLAN_POS */
+} PlanArgs;
+enum { PLAN_COVER = 0, PLAN_SLOT = 1, PLAN_POS = 2 };
+#define PLAN_THREADS 256
+#define PLAN_ITEMS 8
+#define PLAN_TILE (PLAN_THREADS * PLAN_ITEMS)
 
 #ifdef __cplusplus
 }

@@ -30,6 +30,7 @@ int  b2_pinned_alloc(void** p, size_t n);           /* host memory the device ca
 void b2_pinned_free(void* p);
 int  b2_ptr_is_device(const void* p);               /* 1 device/managed, 0 host */
 int  b2_ptr_is_pinned(const void* p);               /* 1 page-locked / registered host memory */
+int  b2_ptr_device(const void* p);                  /* the device that holds device memory p; -1 for host memory */
 
 typedef struct b2_event_s* b2_event_t;
 int  b2_event_create(b2_event_t* e);
@@ -52,9 +53,11 @@ int  b2_launch_fast(const FastArgs* a, b2_stream_t s);      /* index_kernel + pa
                                                              * a->deflate: index_kernel + dparse_kernel + denc_kernel (zlib);
                                                              * a->snappy: index_kernel + zparse_kernel + senc_kernel */
 int  b2_launch_gather(const GatherArgs* a, b2_stream_t s);  /* gather_kernel (getitems) */
+int  b2_launch_plan(const PlanArgs* a, b2_stream_t s);      /* plan_check_kernel + plan_scan_kernel x 3 (x 1 in place):
+                                                             * getitems planned from device-resident range lists */
 
 /* profiling: per-kernel-kind CUDA-event timing (off by default) */
-enum { B2_K_FILTER = 0, B2_K_ENCODE, B2_K_SCAN, B2_K_COMPACT, B2_K_DECODE, B2_K_UNFILTER, B2_K_INDEX, B2_K_PARSE, B2_K_ZENC, B2_K_DENC, B2_K_SENC, B2_K_GATHER, B2_K_COUNT };
+enum { B2_K_FILTER = 0, B2_K_ENCODE, B2_K_SCAN, B2_K_COMPACT, B2_K_DECODE, B2_K_UNFILTER, B2_K_INDEX, B2_K_PARSE, B2_K_ZENC, B2_K_DENC, B2_K_SENC, B2_K_GATHER, B2_K_PLAN, B2_K_COUNT };
 void b2_prof_enable(int on);
 void b2_prof_reset(void);
 int  b2_prof_get(int kind, double* ms_total, long long* launches);

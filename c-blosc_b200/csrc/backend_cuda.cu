@@ -104,6 +104,13 @@ extern "C" int b2_ptr_is_device(const void* p) {
   return a.type == cudaMemoryTypeDevice || a.type == cudaMemoryTypeManaged;
 }
 
+extern "C" int b2_ptr_device(const void* p) {
+  cudaPointerAttributes a;
+  if (p == NULL) return -1;
+  if (cudaPointerGetAttributes(&a, p) != cudaSuccess) { cudaGetLastError(); return -1; }
+  return (a.type == cudaMemoryTypeDevice || a.type == cudaMemoryTypeManaged) ? a.device : -1;
+}
+
 extern "C" int b2_ptr_is_pinned(const void* p) {
   cudaPointerAttributes a;
   if (p == NULL) return 0;
@@ -381,6 +388,37 @@ extern "C" int b2_launch_gather(const GatherArgs* a, b2_stream_t s) {
   if (ctas > (long long)num_sms() * 8) ctas = (long long)num_sms() * 8;
   ProfScope ps(B2_K_GATHER, s->s);
   gather_kernel<<<(unsigned)ctas, GATHER_WARPS * 32, 0, s->s>>>(*a);
+  CK(cudaGetLastError());
+  return 0;
+}
+
+/* the GPU plan of getitems: the per-range check, then one launch per scan (one CTA per tile of PLAN_TILE items) */
+extern "C" int b2_launch_plan(const PlanArgs* a, b2_stream_t s) {
+  if (a->nranges <= 0) return 0;
+  {
+    long long ctas = ((long long)a->nranges + PLAN_THREADS - 1) / PLAN_THREADS;
+    if (ctas > (long long)num_sms() * 8) ctas = (long long)num_sms() * 8;
+    ProfScope ps(B2_K_PLAN, s->s);
+    plan_check_kernel<<<(unsigned)ctas, PLAN_THREADS, 0, s->s>>>(*a);
+    CK(cudaGetLastError());
+  }
+  if (!a->in_place) {
+    const long long nb = a->nblocks;
+    const unsigned tiles = (unsigned)((nb + PLAN_TILE - 1) / PLAN_TILE);
+    {
+      ProfScope ps(B2_K_PLAN, s->s);
+      plan_scan_kernel<PLAN_COVER><<<tiles, PLAN_THREADS, 0, s->s>>>(*a, nb);
+      CK(cudaGetLastError());
+    }
+    {
+      ProfScope ps(B2_K_PLAN, s->s);
+      plan_scan_kernel<PLAN_SLOT><<<tiles, PLAN_THREADS, 0, s->s>>>(*a, nb);
+      CK(cudaGetLastError());
+    }
+  }
+  const long long nr = a->nranges;
+  ProfScope ps(B2_K_PLAN, s->s);
+  plan_scan_kernel<PLAN_POS><<<(unsigned)((nr + PLAN_TILE - 1) / PLAN_TILE), PLAN_THREADS, 0, s->s>>>(*a, nr);
   CK(cudaGetLastError());
   return 0;
 }

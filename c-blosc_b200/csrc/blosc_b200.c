@@ -132,6 +132,7 @@ typedef struct {
   b2_stream_t stream;
   b2_buf in, filt, slots, out, csizes, needs, bstarts;
   b2_buf prev, segs, seg_done, ptail;   /* segment-parallel LZ4 parse (dev_lz4fast.cuh) */
+  b2_buf plan;          /* getitems planned on the GPU: its scratch */
   int* d_result;        /* B2_R_* words (b2_args.h): cbytes, fits, status, work-queue and done counters */
   int* h_result;        /* pinned mirror */
   unsigned queue_base;  /* tickets drawn from the B2_R_QUEUE counter so far (dev_chunk.cuh next_stream) */
@@ -164,7 +165,7 @@ static void ws_teardown(b2_ws* w) {
   int k;
   buf_free(&w->in); buf_free(&w->filt); buf_free(&w->slots); buf_free(&w->out);
   buf_free(&w->csizes); buf_free(&w->needs); buf_free(&w->bstarts);
-  buf_free(&w->prev); buf_free(&w->segs); buf_free(&w->seg_done); buf_free(&w->ptail);
+  buf_free(&w->prev); buf_free(&w->segs); buf_free(&w->seg_done); buf_free(&w->ptail); buf_free(&w->plan);
   for (k = 0; k < B2_STAGE_DEPTH; k++) {
     if (w->stage[k]) b2_pinned_free(w->stage[k]);
     if (w->stage_ev[k]) b2_event_destroy(w->stage_ev[k]);
@@ -271,7 +272,7 @@ int blosc_free_resources(void) {                              /* blosc.h:411 */
     if (w->in_use || !w->ready) continue;
     buf_free(&w->in); buf_free(&w->filt); buf_free(&w->slots); buf_free(&w->out);
     buf_free(&w->csizes); buf_free(&w->needs); buf_free(&w->bstarts);
-    buf_free(&w->prev); buf_free(&w->segs); buf_free(&w->seg_done); buf_free(&w->ptail);
+    buf_free(&w->prev); buf_free(&w->segs); buf_free(&w->seg_done); buf_free(&w->ptail); buf_free(&w->plan);
   }
   pthread_mutex_unlock(&g_ws_mutex);
   return 0;
@@ -1013,10 +1014,9 @@ static int getitem_header(const void* src, int src_dev, long long max_cbytes, b2
 
 /* blosc_getitem's bounds checks of one range (blosc.c:1633-1644): its bytes [*b_lo, *b_hi), empty when b_hi <= b_lo */
 static int getitem_range(const b2_hdr* h, int start, int nitems, long long* b_lo, long long* b_hi) {
-  const int stop = (int)((unsigned)start + (unsigned)nitems);
-  if (start < 0 || (long long)start * h->typesize > h->nbytes) { fprintf(stderr, "`start` out of bounds"); return -1; }
-  if (stop < 0 || (long long)stop * h->typesize > h->nbytes) { fprintf(stderr, "`start`+`nitems` out of bounds"); return -1; }
-  *b_lo = (long long)start * h->typesize; *b_hi = (long long)stop * h->typesize;
+  const int rc = b2_range_check(start, nitems, h->typesize, h->nbytes, b_lo, b_hi);
+  if (rc == 1) { fprintf(stderr, "`start` out of bounds"); return -1; }
+  if (rc == 2) { fprintf(stderr, "`start`+`nitems` out of bounds"); return -1; }
   return 0;
 }
 
@@ -1160,8 +1160,55 @@ static int upload_ranges(b2_ws* w, GatherRange* tab, int nr, long long total, in
   return b2_copy_h2d(w->segs.p, tab, sizeof(GatherRange) * ((size_t)nr + 1), w->stream);
 }
 
-/* `n` ranges of one chunk; range r goes to dest + dsts[r] (back to back in request order when dsts is NULL).  The
- * header and every range are validated before anything is launched or written.  Returns the bytes written. */
+/* The execution tail of getitems, shared by its host plan and its GPU plan.  On entry the gather table (nr + 1
+ * entries; dst = pos when dest is host memory) is in w->segs, and w->slots has room for `total` bytes when dest is host
+ * memory.  d_src is the gather's source when it is already on the device (a memcpyed chunk); when it is NULL the
+ * `count` blocks listed in w->bstarts (ascending; has_left: the last is the chunk's short last block) are decoded and
+ * unfiltered from d_chunk into a compact scratch.  A host dest then receives the ranges from w->slots: at dest +
+ * at_b[0] when `contiguous`, else range r at dest + at_b[r] (tab: the table on the host).  Returns total, or blosc_d's
+ * code when a stream fails to decode (dest is then untouched). */
+static long long getitems_run(b2_ws* w, const b2_hdr* h, int codec, const uint8_t* d_src, const uint8_t* d_chunk,
+                              int count, int has_left, int nr, long long total, void* dest, int dest_dev,
+                              const GatherRange* tab, const long long* at_b, int contiguous) {
+  GatherArgs ga;
+  const int* status = NULL;
+  long long result = -1;
+  uint8_t* tmp = NULL;
+  int r;
+  memset(&ga, 0, sizeof ga);
+  do {
+    if (!d_src) {
+      if (buf_ensure(&w->out, (size_t)count * (size_t)h->blocksize + 64)) break;
+      if (launch_decode_blocks(w, h, codec, d_chunk, 0, count, (const int*)w->bstarts.p, has_left, (uint8_t*)w->out.p)) break;
+      d_src = (const uint8_t*)w->out.p;
+      status = w->d_result + B2_R_STATUS_OUT;
+    }
+    ga.src = d_src; ga.dst = dest_dev ? (uint8_t*)dest : (uint8_t*)w->slots.p; ga.ranges = (const GatherRange*)w->segs.p;
+    ga.nranges = nr; ga.total = total; ga.status = status;
+    if (b2_launch_gather(&ga, w->stream)) { ws_reset_counters(w); break; }
+    if (b2_copy_d2h(w->h_result + B2_R_STATUS_OUT, w->d_result + B2_R_STATUS_OUT, 4, w->stream) || b2_stream_sync(w->stream)) {
+      ws_reset_counters(w);
+      break;
+    }
+    if (status && w->h_result[B2_R_STATUS_OUT] < 0) { result = w->h_result[B2_R_STATUS_OUT]; break; }
+    if (!dest_dev) {
+      if (contiguous) {
+        if (d2h_any(w, (uint8_t*)dest + at_b[0], w->slots.p, (size_t)total)) break;
+      } else {                                                             /* scattered (frame pieces) */
+        if (!(tmp = (uint8_t*)malloc((size_t)total))) break;
+        if (d2h_any(w, tmp, w->slots.p, (size_t)total)) break;
+        for (r = 0; r < nr; r++) memcpy((uint8_t*)dest + at_b[r], tmp + tab[r].pos, (size_t)(tab[r + 1].pos - tab[r].pos));
+      }
+    }
+    result = total;
+  } while (0);
+  free(tmp);
+  return result;
+}
+
+/* The host plan: `n` ranges of one chunk, in host memory; range r goes to dest + dsts[r] (back to back in request order
+ * when dsts is NULL).  The header and every range are validated before anything is launched or written.  Returns the
+ * bytes written. */
 static long long getitems_chunk(const void* src, long long max_cbytes, int n, const int* starts, const int* nitems,
                                 const long long* dsts, void* dest) {
   b2_hdr h;
@@ -1208,10 +1255,9 @@ static long long getitems_chunk(const void* src, long long max_cbytes, int n, co
   w = ws_acquire();
   if (!w) { free(tab); free(lo_b); return -1; }
   do {
-    GatherArgs ga;
-    const uint8_t* d_src;
-    const int* status = NULL;
-    memset(&ga, 0, sizeof ga);
+    const uint8_t* d_src = NULL;
+    const uint8_t* d_chunk = NULL;
+    int count = 0, has_left = 0;
     if (h.flags & BLOSC_MEMCPYED) {
       if (src_dev) d_src = (const uint8_t*)src + 16;                       /* ranges read the payload in place */
       else {                                                               /* the ranges, packed, cross PCIe once */
@@ -1223,11 +1269,11 @@ static long long getitems_chunk(const void* src, long long max_cbytes, int n, co
         if (buf_ensure(&w->in, (size_t)total + 64) || h2d_any(w, w->in.p, tmp, (size_t)total)) break;
         d_src = (const uint8_t*)w->in.p;
       }
+      if (upload_ranges(w, tab, nr, total, dest_dev)) break;
     } else {
       /* the touched blocks: one interval of block numbers per range, merged, then listed in ascending order */
       const int bs = h.blocksize;
-      int nv, count = 0, k;
-      const uint8_t* d_chunk;
+      int nv, k;
       if (!(iv = (b2_iv*)malloc(sizeof(b2_iv) * (size_t)nr))) break;
       for (r = 0; r < nr; r++) {
         iv[r].lo = lo_b[r] / bs;
@@ -1253,40 +1299,138 @@ static long long getitems_chunk(const void* src, long long max_cbytes, int n, co
       }
       if (buf_ensure(&w->bstarts, sizeof(int) * (size_t)count + 64)) break;
       if (b2_copy_h2d(w->bstarts.p, blocks, sizeof(int) * (size_t)count, w->stream)) break;
-      if (buf_ensure(&w->out, (size_t)count * (size_t)bs + 64)) break;
       if (upload_ranges(w, tab, nr, total, dest_dev)) break;      /* before the decode: a pageable copy would wait for it */
-      if (launch_decode_blocks(w, &h, codec, d_chunk, 0, count, (const int*)w->bstarts.p,
-                               h.leftover > 0 && blocks[count - 1] == h.nblocks - 1, (uint8_t*)w->out.p)) break;
-      d_src = (const uint8_t*)w->out.p;
-      status = w->d_result + B2_R_STATUS_OUT;
+      has_left = h.leftover > 0 && blocks[count - 1] == h.nblocks - 1;
     }
-    if (h.flags & BLOSC_MEMCPYED && upload_ranges(w, tab, nr, total, dest_dev)) break;
-    ga.src = d_src; ga.dst = dest_dev ? (uint8_t*)dest : (uint8_t*)w->slots.p; ga.ranges = (const GatherRange*)w->segs.p;
-    ga.nranges = nr; ga.total = total; ga.status = status;
-    if (b2_launch_gather(&ga, w->stream)) { ws_reset_counters(w); break; }
-    if (b2_copy_d2h(w->h_result + B2_R_STATUS_OUT, w->d_result + B2_R_STATUS_OUT, 4, w->stream) || b2_stream_sync(w->stream)) {
-      ws_reset_counters(w);
-      break;
-    }
-    if (status && w->h_result[B2_R_STATUS_OUT] < 0) { result = w->h_result[B2_R_STATUS_OUT]; break; }
-    if (!dest_dev) {
-      if (contiguous) {
-        if (d2h_any(w, (uint8_t*)dest + at_b[0], w->slots.p, (size_t)total)) break;
-      } else {                                                             /* scattered (frame pieces) */
-        if (!tmp && !(tmp = (uint8_t*)malloc((size_t)total))) break;
-        if (d2h_any(w, tmp, w->slots.p, (size_t)total)) break;
-        for (r = 0; r < nr; r++) memcpy((uint8_t*)dest + at_b[r], tmp + tab[r].pos, (size_t)(tab[r + 1].pos - tab[r].pos));
-      }
-    }
-    result = total;
+    result = getitems_run(w, &h, codec, d_src, d_chunk, count, has_left, nr, total, dest, dest_dev, tab, at_b, contiguous);
   } while (0);
   ws_release(w);
   free(tab); free(lo_b); free(iv); free(blocks); free(tmp);
   return result;
 }
 
+/* Stage the payload of a memcpyed host chunk that the listed blocks cover, block j of the list at j * blocksize of
+ * w->in; runs of consecutive blocks are copied as one. */
+static int stage_memcpyed_blocks(b2_ws* w, const b2_hdr* h, const uint8_t* hs, const int* blocks, int count) {
+  const long long bs = h->blocksize;
+  int i = 0, j;
+  if (buf_ensure(&w->in, (size_t)count * (size_t)bs + 64)) return -1;
+  while (i < count) {
+    long long end;
+    for (j = i + 1; j < count && blocks[j] == blocks[j - 1] + 1; j++) {}
+    end = ((long long)blocks[j - 1] + 1) * bs;
+    if (end > h->nbytes) end = h->nbytes;
+    if (h2d_any(w, (uint8_t*)w->in.p + i * bs, hs + 16 + blocks[i] * bs, (size_t)(end - blocks[i] * bs))) return -1;
+    i = j;
+  }
+  return 0;
+}
+
+#define B2_R_PLAN 8   /* h_result words 8..13 receive the GPU plan's record (GetitemsPlan) */
+#define B2_AL(x) (((x) + 15) & ~(size_t)15)
+
+/* The GPU plan (dev_chunk.cuh plan_*_kernel), for range lists of which at least one is in device memory (a host one is
+ * uploaded).  It builds the gather table in w->segs and the touched-block list in w->bstarts, both as the host plan
+ * would (the table keeps empty ranges, which copy nothing), and the host reads back one small record.  A failing range
+ * is reported by getitem_range on that range alone, so the code and the message are the host plan's.  A host chunk
+ * also has the block list read back, to stage only the touched blocks. */
+static long long getitems_gpu(const void* src, int src_dev, const b2_hdr* h, int codec, int n, const int* starts,
+                              int starts_dev, const int* nitems, int nitems_dev, void* dest) {
+  const int dest_dev = b2_ptr_is_device(dest);
+  const int memcpyed = (h->flags & BLOSC_MEMCPYED) != 0, in_place = memcpyed && src_dev;
+  const size_t tb = ((size_t)h->nblocks + PLAN_TILE - 1) / PLAN_TILE, tr = ((size_t)n + PLAN_TILE - 1) / PLAN_TILE;
+  /* one scratch: the record, the tickets, the tile flags and the difference array, all zeroed; then the tiles' values,
+   * the range lengths, the block slots and an uploaded host list */
+  const size_t o_tk = 32, o_flag = 64, o_cover = B2_AL(o_flag + 4 * (2 * tb + tr));
+  const size_t zeroed = B2_AL(o_cover + 4 * ((size_t)h->nblocks + 1));
+  const size_t o_vals = zeroed, o_len = B2_AL(o_vals + 4 * 4 * tb + 8 * 2 * tr);
+  const size_t o_slot = B2_AL(o_len + 8 * (size_t)n), o_up = B2_AL(o_slot + 4 * (size_t)h->nblocks);
+  const size_t need = o_up + 4 * (size_t)n;
+  const long long at0 = 0;
+  long long result = -1;
+  int* hblocks = NULL;
+  b2_ws* w = ws_acquire();
+  if (!w) return -1;
+  do {
+    PlanArgs pa;
+    GetitemsPlan rec;
+    uint8_t* base;
+    const uint8_t* d_src = NULL;
+    const uint8_t* d_chunk = NULL;
+    int k;
+    if (buf_ensure(&w->plan, need) || buf_ensure(&w->segs, sizeof(GatherRange) * ((size_t)n + 1) + 64)) break;
+    if (!in_place && buf_ensure(&w->bstarts, 4 * (size_t)h->nblocks + 64)) break;
+    base = (uint8_t*)w->plan.p;
+    memset(&pa, 0, sizeof pa);
+    pa.starts = starts; pa.nitems = nitems;
+    if (!starts_dev || !nitems_dev) {                                      /* the host list joins the device one */
+      if (h2d_any(w, base + o_up, starts_dev ? (const void*)nitems : (const void*)starts, 4 * (size_t)n)) break;
+      if (starts_dev) pa.nitems = (const int*)(base + o_up); else pa.starts = (const int*)(base + o_up);
+    }
+    if (b2_memset_dev(base, 0, zeroed, w->stream) || b2_memset_dev(base, 0xff, 4, w->stream)) break;
+    pa.nranges = n; pa.typesize = h->typesize; pa.blocksize = h->blocksize; pa.nblocks = h->nblocks;
+    pa.leftover = h->leftover > 0; pa.nbytes = h->nbytes; pa.in_place = in_place;
+    pa.len = (long long*)(base + o_len); pa.cover = (int*)(base + o_cover); pa.slot = (int*)(base + o_slot);
+    pa.blocks = (int*)w->bstarts.p; pa.ranges = (GatherRange*)w->segs.p; pa.rec = (GetitemsPlan*)base;
+    for (k = 0; k < 3; k++) {
+      const size_t tiles = k < 2 ? tb : tr;
+      const size_t flags_at = o_flag + 4 * (k < 2 ? k * tb : 2 * tb);
+      const size_t vals_at = o_vals + (k < 2 ? 2 * 4 * k * tb : 4 * 4 * tb), width = k < 2 ? 4 : 8;
+      pa.scan[k].ticket = (unsigned*)(base + o_tk) + k;
+      pa.scan[k].flag = (unsigned*)(base + flags_at);
+      pa.scan[k].agg = base + vals_at;
+      pa.scan[k].inc = base + vals_at + width * tiles;
+    }
+    if (b2_launch_plan(&pa, w->stream)) break;
+    if (b2_copy_d2h(w->h_result + B2_R_PLAN, base, sizeof rec, w->stream) || b2_stream_sync(w->stream)) break;
+    memcpy(&rec, w->h_result + B2_R_PLAN, sizeof rec);
+    if (rec.bad != 0xffffffffu) {                                          /* blosc_getitem's verdict on that range */
+      int s, c;
+      long long lo, hi;
+      if (copy_any(&s, 0, starts + rec.bad, starts_dev, 4, w->stream) ||
+          copy_any(&c, 0, nitems + rec.bad, nitems_dev, 4, w->stream)) break;
+      getitem_range(h, s, c, &lo, &hi);
+      break;
+    }
+    if (rec.total == 0) { result = 0; break; }
+    if (!dest_dev && buf_ensure(&w->slots, (size_t)rec.total + 64)) break;
+    if (in_place) d_src = (const uint8_t*)src + 16;
+    else if (src_dev) d_chunk = (const uint8_t*)src;
+    else {                                                                 /* stage the touched blocks only */
+      if (!(hblocks = (int*)malloc(4 * (size_t)rec.nlisted))) break;
+      if (d2h_any(w, hblocks, w->bstarts.p, 4 * (size_t)rec.nlisted)) break;
+      if (memcpyed) {
+        if (stage_memcpyed_blocks(w, h, (const uint8_t*)src, hblocks, rec.nlisted)) break;
+        d_src = (const uint8_t*)w->in.p;
+      } else {
+        if (stage_blocks(w, h, (const uint8_t*)src, hblocks, rec.nlisted)) break;
+        d_chunk = (const uint8_t*)w->in.p;
+      }
+    }
+    result = getitems_run(w, h, codec, d_src, d_chunk, rec.nlisted, rec.has_left, n, rec.total, dest, dest_dev, NULL,
+                          &at0, 1);
+  } while (0);
+  ws_release(w);
+  free(hblocks);
+  return result;
+}
+
 long long blosc_b200_getitems(const void* src, int nranges, const int* starts, const int* nitems, void* dest) {
-  return getitems_chunk(src, -1, nranges, starts, nitems, NULL, dest);
+  b2_hdr h;
+  int starts_dev, nitems_dev, src_dev, dev, codec = 0, rc;
+  if (nranges <= 0) return 0;
+  starts_dev = b2_ptr_is_device(starts); nitems_dev = b2_ptr_is_device(nitems);
+  if (!starts_dev && !nitems_dev) return getitems_chunk(src, -1, nranges, starts, nitems, NULL, dest);
+  /* device lists: on the device the call runs on, that of src or dest when either is device memory */
+  src_dev = b2_ptr_is_device(src);
+  dev = src_dev ? b2_ptr_device(src) : b2_ptr_is_device(dest) ? b2_ptr_device(dest) : b2_get_device();
+  if ((starts_dev && b2_ptr_device(starts) != dev) || (nitems_dev && b2_ptr_device(nitems) != dev)) {
+    fprintf(stderr, "blosc_b200: starts / nitems are not on device %d, where the call runs\n", dev);
+    return -1;
+  }
+  rc = getitem_header(src, src_dev, -1, &h, &codec);
+  if (rc) return rc;
+  return getitems_gpu(src, src_dev, &h, codec, nranges, starts, starts_dev, nitems, nitems_dev, dest);
 }
 
 /* ------------------------------------------------------------------------- */
@@ -1617,17 +1761,41 @@ static int cmp_piece(const void* a, const void* b) {
   return x->order < y->order ? -1 : x->order > y->order;
 }
 
-/* Every range is checked as blosc_b200_frame_getitem checks one before anything is read; then the ranges are cut at
- * chunk boundaries and each touched chunk runs the chunk plan once, each piece landing at its own dest offset. */
+static long long frame_getitems_host(const void* frame, size_t framesize, size_t nranges, const size_t* starts,
+                                     const size_t* nitems, void* dest);
+
+/* Range lists in device memory are copied to the host (one copy each), and the frame is planned there */
 long long blosc_b200_frame_getitems(const void* frame, size_t framesize, size_t nranges, const size_t* starts,
                                     const size_t* nitems, void* dest) {
+  size_t* h = NULL;
+  b2_ws* w;
+  long long result = -1;
+  int starts_dev, nitems_dev;
+  if (nranges == 0) return 0;
+  if (!backend_ready()) return -1;
+  starts_dev = b2_ptr_is_device(starts); nitems_dev = b2_ptr_is_device(nitems);
+  if (!starts_dev && !nitems_dev) return frame_getitems_host(frame, framesize, nranges, starts, nitems, dest);
+  if (nranges > ((size_t)-1) / (2 * sizeof(size_t)) || !(h = (size_t*)malloc(2 * sizeof(size_t) * nranges))) return -1;
+  if ((w = ws_acquire()) != NULL) {
+    if (!copy_any(h, 0, starts, starts_dev, sizeof(size_t) * nranges, w->stream) &&
+        !copy_any(h + nranges, 0, nitems, nitems_dev, sizeof(size_t) * nranges, w->stream))
+      result = 0;
+    ws_release(w);
+  }
+  if (result == 0) result = frame_getitems_host(frame, framesize, nranges, h, h + nranges, dest);
+  free(h);
+  return result;
+}
+
+/* Every range is checked as blosc_b200_frame_getitem checks one before anything is read; then the ranges are cut at
+ * chunk boundaries and each touched chunk runs the chunk plan once, each piece landing at its own dest offset. */
+static long long frame_getitems_host(const void* frame, size_t framesize, size_t nranges, const size_t* starts,
+                                     const size_t* nitems, void* dest) {
   size_t nb = 0, cs = 0, nc = 0, ts = 0, ipc, r, npieces = 0, i, j;
   uint64_t* off = NULL;
   uint8_t hb[16];
   b2_piece* pieces = NULL;
   long long result = -1, at = 0;
-  if (nranges == 0) return 0;
-  if (!backend_ready()) return -1;
   if (frame_open(frame, framesize, &nb, &cs, &nc, &off)) return -1;
   do {
     if (nc == 0) {

@@ -11,6 +11,9 @@
  *                   payloads at their final offsets (:1148-1247, :715, :1860)
  *   decode_kernel   one warp per LZ stream: bounds-checked walk of the size prefixes
  *                   (:761-770), raw-split copy or codec (:773-783)
+ *   gather_kernel, plan_check_kernel, plan_scan_kernel
+ *                   many item ranges of one chunk (blosc_b200_getitems): the copy out of
+ *                   the decoded blocks, and its plan when the range lists are device memory
  */
 #pragma once
 #include "b2_args.h"
@@ -879,6 +882,175 @@ extern "C" int b2_launch_gather(const GatherArgs* a, b2_stream_t) {
   simt::launch(simt::Dim3((unsigned)ctas), simt::Dim3(GATHER_WARPS * 32), 0, [&] { gather_kernel(args); });
   return 0;
 }
+#endif
+
+
+/* getitems planned on the GPU (PlanArgs), for range lists in device memory: the same gather table and block list the
+ * host plan builds, with no copy of the lists to the host.  plan_check_kernel, one thread per range: blosc_getitem's
+ * checks (b2_range_check), the first failing index by atomicMin, each range's byte length, and its block interval
+ * marked in a difference array (+1 at the first block, -1 after the last), so a whole-chunk range costs two atomics. */
+__global__ void __launch_bounds__(PLAN_THREADS) plan_check_kernel(PlanArgs a) {
+  for (long long r = (long long)blockIdx.x * PLAN_THREADS + threadIdx.x; r < a.nranges;
+       r += (long long)gridDim.x * PLAN_THREADS) {
+    long long lo = 0, hi = 0;
+    if (b2_range_check(a.starts[r], a.nitems[r], a.typesize, a.nbytes, &lo, &hi)) {
+      atomicMin(&a.rec->bad, (unsigned)r);
+      a.len[r] = 0;
+      continue;
+    }
+    const long long n = hi > lo ? hi - lo : 0;
+    a.len[r] = n;
+    if (n > 0 && !a.in_place) {
+      atomicAdd(a.cover + lo / a.blocksize, 1);
+      atomicAdd(a.cover + (hi - 1) / a.blocksize + 1, -1);
+    }
+  }
+}
+
+/* The three scans of the plan, one device-wide exclusive scan each: PLAN_COVER turns the difference array into each
+ * block's coverage (in place), PLAN_SLOT numbers the covered blocks and lists them, PLAN_POS makes each range's
+ * position in dest from its length and writes its gather entry. */
+template <int MODE> struct PlanVal { typedef int T; };
+template <> struct PlanVal<PLAN_POS> { typedef long long T; };
+
+template <int MODE> DEV typename PlanVal<MODE>::T plan_load(const PlanArgs& a, long long i) {
+  if constexpr (MODE == PLAN_COVER) return a.cover[i];
+  else if constexpr (MODE == PLAN_SLOT) return a.cover[i] > 0;
+  else return a.len[i];
+}
+
+template <int MODE, typename T> DEV void plan_store(const PlanArgs& a, long long i, long long n, T excl, T x) {
+  if constexpr (MODE == PLAN_COVER) {
+    a.cover[i] = excl + x;
+  } else if constexpr (MODE == PLAN_SLOT) {
+    if (x) { a.slot[i] = excl; a.blocks[excl] = (int)i; }
+    if (i == n - 1) { a.rec->nlisted = excl + x; a.rec->has_left = x && a.leftover; }
+  } else {
+    GatherRange g;
+    g.pos = g.dst = excl;
+    g.src = 0;
+    if (x > 0) {                       /* where the range starts in the gather's source */
+      const long long lo = (long long)a.starts[i] * a.typesize;
+      if (a.in_place) g.src = lo;
+      else {
+        const long long first = lo / a.blocksize;
+        g.src = (long long)a.slot[first] * a.blocksize + (lo - first * a.blocksize);
+      }
+    }
+    a.ranges[i] = g;
+    if (i == n - 1) {
+      GatherRange e;
+      e.src = e.dst = 0; e.pos = excl + x;
+      a.ranges[n] = e;
+      a.rec->total = excl + x;
+    }
+  }
+}
+
+/* Single pass with decoupled look-back: each CTA takes the next tile (PLAN_TILE items, PLAN_ITEMS consecutive ones
+ * per thread) from a counter, so the tiles before it have started; it publishes its aggregate, then warp 0 walks back
+ * 32 tiles at a time, summing aggregates up to the nearest tile that has published its inclusive prefix. */
+template <int MODE>
+__global__ void __launch_bounds__(PLAN_THREADS) plan_scan_kernel(PlanArgs a, long long n) {
+  typedef typename PlanVal<MODE>::T T;
+  const PlanScan& st = a.scan[MODE];
+  __shared__ T s_warp[PLAN_THREADS / 32];
+  __shared__ T s_prefix;
+  __shared__ unsigned s_tile;
+  const int lane = lane_id(), warp = (int)(threadIdx.x >> 5);
+  if (threadIdx.x == 0) s_tile = atomicAdd(st.ticket, 1u);
+  __syncthreads();
+  const long long tile = s_tile;
+  const long long base = tile * PLAN_TILE + (long long)threadIdx.x * PLAN_ITEMS;
+  T v[PLAN_ITEMS], sum = 0;
+#pragma unroll
+  for (int k = 0; k < PLAN_ITEMS; k++) {
+    v[k] = base + k < n ? plan_load<MODE>(a, base + k) : (T)0;
+    sum += v[k];
+  }
+  T inc = sum;
+#pragma unroll
+  for (int d = 1; d < 32; d <<= 1) {
+    const T t = __shfl_up_sync(FULLMASK, inc, d);
+    if (lane >= d) inc += t;
+  }
+  if (lane == 31) s_warp[warp] = inc;
+  __syncthreads();
+  if (warp == 0) {
+    T* agg = (T*)st.agg;
+    T* incl = (T*)st.inc;
+    volatile unsigned* flag = st.flag;
+    const T w = lane < PLAN_THREADS / 32 ? s_warp[lane] : (T)0;
+    T wi = w;
+#pragma unroll
+    for (int d = 1; d < 32; d <<= 1) {
+      const T t = __shfl_up_sync(FULLMASK, wi, d);
+      if (lane >= d) wi += t;
+    }
+    const T total = __shfl_sync(FULLMASK, wi, 31);
+    if (lane < PLAN_THREADS / 32) s_warp[lane] = wi - w;
+    if (lane == 0) {
+      if (tile == 0) { incl[0] = total; __threadfence(); flag[0] = 2; }
+      else { agg[tile] = total; __threadfence(); flag[tile] = 1; }
+    }
+    T prefix = 0;
+    if (tile > 0) {
+      for (long long p = tile - 1;; p -= 32) {
+        const long long q = p - lane;
+        unsigned f = 2;
+        T val = 0;
+        if (q >= 0) {
+          while ((f = flag[q]) == 0) {}
+          __threadfence();
+          val = f == 2 ? ((volatile T*)incl)[q] : ((volatile T*)agg)[q];
+        }
+        const unsigned done = __ballot_sync(FULLMASK, f == 2);
+        const int stop = done ? __ffs((int)done) - 1 : 31;     /* lanes up to the nearest inclusive prefix count */
+        T c = lane <= stop ? val : (T)0;
+#pragma unroll
+        for (int d = 16; d; d >>= 1) c += __shfl_xor_sync(FULLMASK, c, d);
+        prefix += c;
+        if (done) break;
+      }
+      if (lane == 0) { incl[tile] = prefix + total; __threadfence(); flag[tile] = 2; }
+    }
+    if (lane == 0) s_prefix = prefix;
+  }
+  __syncthreads();
+  T excl = s_prefix + s_warp[warp] + inc - sum;
+#pragma unroll
+  for (int k = 0; k < PLAN_ITEMS; k++) {
+    if (base + k < n) plan_store<MODE, T>(a, base + k, n, excl, v[k]);
+    excl += v[k];
+  }
+}
+
+#ifdef SIMT_EMU
+/* The emulator's launcher of the plan kernels: a few CTAs for the per-range check, so that the grid-stride loop runs;
+ * every tile of a scan is its own CTA, as on the GPU.  The emulator has one device. */
+static long long g_emu_plan_launches = 0;
+extern "C" int b2_launch_plan(const PlanArgs* a, b2_stream_t) {
+  if (a->nranges <= 0) return 0;
+  PlanArgs args = *a;
+  long long ctas = ((long long)a->nranges + PLAN_THREADS - 1) / PLAN_THREADS;
+  if (ctas > 3) ctas = 3;
+  simt::launch(simt::Dim3((unsigned)ctas), simt::Dim3(PLAN_THREADS), 0, [&] { plan_check_kernel(args); });
+  g_emu_plan_launches++;
+  if (!a->in_place) {
+    const long long nb = a->nblocks;
+    simt::launch(simt::Dim3((unsigned)((nb + PLAN_TILE - 1) / PLAN_TILE)), simt::Dim3(PLAN_THREADS), 0,
+                 [&] { plan_scan_kernel<PLAN_COVER>(args, nb); });
+    simt::launch(simt::Dim3((unsigned)((nb + PLAN_TILE - 1) / PLAN_TILE)), simt::Dim3(PLAN_THREADS), 0,
+                 [&] { plan_scan_kernel<PLAN_SLOT>(args, nb); });
+    g_emu_plan_launches += 2;
+  }
+  const long long nr = a->nranges;
+  simt::launch(simt::Dim3((unsigned)((nr + PLAN_TILE - 1) / PLAN_TILE)), simt::Dim3(PLAN_THREADS), 0,
+               [&] { plan_scan_kernel<PLAN_POS>(args, nr); });
+  g_emu_plan_launches++;
+  return 0;
+}
+extern "C" int b2_ptr_device(const void*) { return 0; }
 #endif
 
 

@@ -149,10 +149,17 @@ int blosc_b200_filter(int mode, size_t typesize, size_t blocksize, const void* s
 
 /* Many item ranges of one chunk in one call.  Range r covers items [starts[r], starts[r] + nitems[r]) in elements of
  * the chunk's typesize.  Each range is validated exactly as blosc_getitem validates one.  Ranges may be unsorted,
- * overlap or repeat.  They are written back to back into dest in request order.  starts / nitems are host arrays;
- * src / dest are host or device.  Every block that some range overlaps is decoded once, by one decode launch, however
- * many ranges touch it.  Returns the total bytes written, or the code blosc_getitem would return for the first range
- * that fails; in that case nothing is written to dest.  nranges == 0 returns 0. */
+ * overlap or repeat.  They are written back to back into dest in request order.  src / dest are host or device.
+ * Every block that some range overlaps is decoded once, by one decode launch, however many ranges touch it.  Returns
+ * the total bytes written, or the code blosc_getitem would return for the first range that fails (with its stderr
+ * message); in that case nothing is written to dest.  nranges == 0 returns 0 and reads neither list.
+ *
+ * starts / nitems may each be host or device memory.  When either is device memory the read is planned on the GPU
+ * (a host list is uploaded with the other), so the lists never come back to the host; the results are the same as
+ * with host lists.  Device lists must be on the device the call runs on: that of src or dest when either is device
+ * memory, else the one chosen with blosc_b200_set_device; otherwise the call returns -1 before anything is read or
+ * written.  The call runs on blocking streams, ordered after work on the legacy default stream; lists produced on
+ * other non-blocking streams must be synchronised first, as src must. */
 long long blosc_b200_getitems(const void* src, int nranges, const int* starts, const int* nitems, void* dest);
 
 /* Frames: buffers larger than one chunk (a Blosc-1 chunk holds at most BLOSC_MAX_BUFFERSIZE
@@ -172,7 +179,8 @@ long long blosc_b200_frame_decompress(const void* frame, size_t framesize, void*
                                       int numinternalthreads);
 long long blosc_b200_frame_getitem(const void* frame, size_t framesize, size_t start, size_t nitems, void* dest);
 /* blosc_b200_getitems over a frame: ranges may cross chunk boundaries, as in blosc_b200_frame_getitem, and are
- * written back to back into dest in request order.  Every range is checked before anything is read. */
+ * written back to back into dest in request order.  Every range is checked before anything is read.  starts / nitems
+ * may be host or device memory; device lists are copied to the host, where the frame is planned. */
 long long blosc_b200_frame_getitems(const void* frame, size_t framesize, size_t nranges, const size_t* starts,
                                     const size_t* nitems, void* dest);
 int       blosc_b200_frame_info(const void* frame, size_t framesize, size_t* nbytes, size_t* cbytes,
@@ -185,7 +193,7 @@ int blosc_b200_set_device(int dev);
 
 /* Per-kernel CUDA-event timing of the calls made since the last reset (bench.py's roofline
  * leg).  kind: 0 filter, 1 encode, 2 scan, 3 compact, 4 decode, 5 unfilter, 6 index, 7 parse, 8 zenc, 9 denc,
- * 10 senc, 11 gather. */
+ * 10 senc, 11 gather, 12 plan (getitems planned on the GPU). */
 void blosc_b200_set_profiling(int on);
 void blosc_b200_prof_reset(void);
 int  blosc_b200_prof_get(int kind, double* ms_total, long long* launches);
