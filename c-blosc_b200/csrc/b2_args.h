@@ -92,7 +92,6 @@ typedef struct FastArgs {
   uint8_t* slots;
   uint16_t* prev;          /* [nbytes] hash-chain index written by index_kernel */
   FastSeg* segs;           /* stream-major: stream idx starts at idx * segs_full (the leftover stream comes last) */
-  int* seg_done;           /* [nstreams] zero-initialised count of parsed groups; the warp that completes a stream scans it */
   int* ptail;              /* [nstreams] literals after the stream's last match */
   int* csizes;
   int* needs;
@@ -109,18 +108,15 @@ typedef struct FastArgs {
   int* done;
   int fold_scan;
   ScanArgs scan;
-  /* zstd encoder (dev_zstdenc.cuh): the same index and windows, sequence records instead of LZ4 bytes, then one warp
-   * per stream writes its zstd frame; segs / seg_done / ptail are not used */
-  int zstd;
+  /* B2_CODEC_LZ4: the parse writes LZ4 bytes and segs, one warp per stream merges them (fscan_kernel).  The others
+   * parse into sequence records (recs / nrec; segs and ptail are not used), then one warp per stream writes it:
+   *   B2_CODEC_ZSTD    a zstd frame (dev_zstdenc.cuh);
+   *   B2_CODEC_ZLIB    a zlib stream, from records with offsets <= 32768 (dev_deflate.cuh);
+   *   B2_CODEC_SNAPPY  a snappy stream (dev_snappy.cuh); the last warp's block scan applies blosc_c's snappy maxout rule */
+  int codec;
   uint32_t* recs;                  /* 64 records per segment, segment-major as segs */
   uint32_t* nrec;                  /* records per segment */
-  /* DEFLATE encoder (dev_deflate.cuh): the zstd encoder's records, offsets <= 32768, then one warp per stream writes
-   * its zlib stream (zstd is 0) */
-  int deflate;
   int flevel;                      /* zlib's FLEVEL for the clevel (deflate.c), in the stream header */
-  /* snappy encoder (dev_snappy.cuh): the zstd encoder's records, then one warp per stream writes its snappy stream
-   * (zstd and deflate are 0); the last warp's block scan applies blosc_c's snappy maxout rule */
-  int snappy;
   int ebsize;                      /* blocksize + 4 typesize: the per-block maxbytes of t_blosc's pool (blosc.c:1745) */
 } FastArgs;
 

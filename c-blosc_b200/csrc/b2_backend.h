@@ -48,10 +48,11 @@ int  b2_launch_encode(const EncodeArgs* a, b2_stream_t s);
 int  b2_launch_scan(const ScanArgs* a, b2_stream_t s);
 int  b2_launch_compact(const CompactArgs* a, b2_stream_t s);
 int  b2_launch_decode(const DecodeArgs* a, b2_stream_t s);
-int  b2_launch_fast(const FastArgs* a, b2_stream_t s);      /* index_kernel + parse_kernel (segment-parallel LZ4); with
-                                                             * a->zstd: index_kernel + zparse_kernel + zenc_kernel (zstd);
-                                                             * a->deflate: index_kernel + dparse_kernel + denc_kernel (zlib);
-                                                             * a->snappy: index_kernel + zparse_kernel + senc_kernel */
+int  b2_launch_fast(const FastArgs* a, b2_stream_t s);      /* by a->codec, index_kernel and then:
+                                                             * B2_CODEC_LZ4: parse_kernel + fscan_kernel (segment-parallel LZ4);
+                                                             * B2_CODEC_ZSTD: zparse_kernel + zenc_kernel (zstd);
+                                                             * B2_CODEC_ZLIB: dparse_kernel + denc_kernel (zlib);
+                                                             * B2_CODEC_SNAPPY: zparse_kernel + senc_kernel */
 int  b2_launch_gather(const GatherArgs* a, b2_stream_t s);  /* gather_kernel (getitems) */
 int  b2_launch_plan(const PlanArgs* a, b2_stream_t s);      /* plan_check_kernel + plan_scan_kernel x 3 (x 1 in place):
                                                              * getitems planned from device-resident range lists */

@@ -226,6 +226,17 @@ extern "C" int b2_lz4_cycles_read(unsigned long long* dst, int nstreams) {
 }
 #endif
 
+/* The arguments of a launch that draws tickets from the workspace's queue counter (dev_chunk.cuh next_stream, and the
+ * parse's job counter): it consumes `jobs` tickets and one more per drawing warp or thread, which draws once past the
+ * end.  The launch starts at the running base, which moves on past it. */
+template <class Args>
+static Args take_tickets(const Args* a, long long jobs, long long drawers) {
+  Args args = *a;
+  args.queue_base = *a->queue_base_host;
+  *a->queue_base_host += (unsigned)jobs + (unsigned)drawers;
+  return args;
+}
+
 extern "C" int b2_launch_encode(const EncodeArgs* a, b2_stream_t s) {
   if (team_wanted(a)) {
     int ctas = a->map.nstreams;
@@ -233,10 +244,8 @@ extern "C" int b2_launch_encode(const EncodeArgs* a, b2_stream_t s) {
     if (ctas > cap) ctas = cap;
     if (ctas <= 0) return 0;
     ProfScope ps(B2_K_ENCODE, s->s);
-    EncodeArgs args = *a;
+    EncodeArgs args = take_tickets(a, a->map.nstreams, ctas);      /* one ticket-drawing warp per CTA */
     args.num_sms = num_sms();
-    args.queue_base = *a->queue_base_host;
-    *a->queue_base_host += (unsigned)a->map.nstreams + (unsigned)ctas;      /* one ticket-drawing warp per CTA */
     encode_team_kernel<<<ctas, TEAM_WARPS * 32, TEAM_SMEM_BYTES, s->s>>>(args);
     CK(cudaGetLastError());
     return 0;
@@ -247,78 +256,47 @@ extern "C" int b2_launch_encode(const EncodeArgs* a, b2_stream_t s) {
   const int ctas = (a->map.nstreams + wpc - 1) / wpc;
   if (ctas <= 0) return 0;
   ProfScope ps(B2_K_ENCODE, s->s);
-  EncodeArgs args = *a;
-  args.queue_base = *a->queue_base_host;
-  *a->queue_base_host += (unsigned)a->map.nstreams + (unsigned)ctas * (unsigned)wpc;
-  encode_kernel<<<ctas, wpc * 32, (size_t)wpc * a->table_bytes, s->s>>>(args);
+  encode_kernel<<<ctas, wpc * 32, (size_t)wpc * a->table_bytes, s->s>>>(take_tickets(a, a->map.nstreams, ctas * wpc));
   CK(cudaGetLastError());
   return 0;
 }
 
-/* the front half of every segment-parallel encoder: the hash-chain index of every stream, then one lane per segment --
- * LZ4 bytes (parse_kernel), or zstd sequence records (`records`: zparse_kernel; a->deflate: dparse_kernel, offsets
- * <= 32768) */
-static int launch_fast_front(const FastArgs* a, bool records, b2_stream_t s) {
+/* Every segment-parallel encoder: the hash-chain index of every stream, then one lane per segment parses it, then one
+ * warp per stream finishes it (FastArgs.codec).  The parse writes LZ4 bytes (parse_kernel) or sequence records
+ * (zparse_kernel; dparse_kernel for DEFLATE, offsets <= 32768).  The back half merges the LZ4 segments (fscan_kernel)
+ * or writes a zstd frame (zenc_kernel), a zlib stream (denc_kernel) or a snappy stream (senc_kernel). */
+extern "C" int b2_launch_fast(const FastArgs* a, b2_stream_t s) {
+  if (a->map.nstreams <= 0) return 0;
   {
     int ctas = (a->map.nstreams + INDEX_WARPS - 1) / INDEX_WARPS;
     ProfScope ps(B2_K_INDEX, s->s);
     index_kernel<<<ctas, INDEX_WARPS * 32, INDEX_WARPS * FAST_TAB_BYTES, s->s>>>(*a);
     CK(cudaGetLastError());
   }
-  const long long njobs = (long long)a->map.nfull * a->map.nsplits * a->groups_full + a->groups_left;
-  const int threads = a->threads;
-  const size_t smem = (size_t)a->win_bytes + 64;
-  int per_sm = (int)((size_t)220 * 1024 / (smem + 1024));
-  if (per_sm * threads > 2048) per_sm = 2048 / threads;
-  if (per_sm < 1) per_sm = 1;
-  long long ctas = njobs;
-  const long long cap = (long long)num_sms() * per_sm;
-  if (ctas > cap) ctas = cap;
-  ProfScope ps(B2_K_PARSE, s->s);
-  FastArgs args = *a;
-  args.queue_base = *a->queue_base_host;
-  *a->queue_base_host += (unsigned)njobs + (unsigned)ctas;      /* one ticket-drawing thread per CTA */
-  if (a->deflate) dparse_kernel<<<(unsigned)ctas, threads, smem, s->s>>>(args);
-  else if (records) zparse_kernel<<<(unsigned)ctas, threads, smem, s->s>>>(args);
-  else parse_kernel<<<(unsigned)ctas, threads, smem, s->s>>>(args);
-  CK(cudaGetLastError());
-  return 0;
-}
-
-/* segment-parallel LZ4: the front half, then the stream scan; a->zstd: the front half with records, then one warp per
- * zstd frame (dev_zstdenc.cuh); a->deflate: the same records with offsets <= 32768, then one warp per zlib stream
- * (dev_deflate.cuh); a->snappy: the zstd records, then one warp per snappy stream (dev_snappy.cuh), whose last warp
- * runs the block scan with blosc_c's snappy maxout rule */
-extern "C" int b2_launch_fast(const FastArgs* a, b2_stream_t s) {
-  if (a->map.nstreams <= 0) return 0;
-  if (launch_fast_front(a, a->zstd || a->snappy, s)) return -1;
-  if (a->snappy) {                                                /* one warp per snappy stream */
-    const int ctas = (a->map.nstreams + SN_WARPS - 1) / SN_WARPS;
-    ProfScope ps(B2_K_SENC, s->s);
-    senc_kernel<<<ctas, SN_WARPS * 32, 0, s->s>>>(*a);
-    CK(cudaGetLastError());
-    return 0;
-  }
-  if (a->zstd) {                                                  /* one warp per zstd frame */
-    const int ctas = (a->map.nstreams + ZE_WARPS - 1) / ZE_WARPS;
-    ProfScope ps(B2_K_ZENC, s->s);
-    zenc_kernel<<<ctas, ZE_WARPS * 32, ZE_WARPS * ZE_SMEM_BYTES, s->s>>>(*a);
-    CK(cudaGetLastError());
-    return 0;
-  }
-  if (a->deflate) {                                               /* one warp per zlib stream */
-    const int ctas = (a->map.nstreams + DZ_WARPS - 1) / DZ_WARPS;
-    ProfScope ps(B2_K_DENC, s->s);
-    denc_kernel<<<ctas, DZ_WARPS * 32, DZ_WARPS * DZ_SMEM_BYTES, s->s>>>(*a);
-    CK(cudaGetLastError());
-    return 0;
-  }
   {
-    const int ctas = (a->map.nstreams + FSCAN_WARPS - 1) / FSCAN_WARPS;
-    ProfScope ps(B2_K_SCAN, s->s);
-    fscan_kernel<<<ctas, FSCAN_WARPS * 32, 0, s->s>>>(*a);
+    void (*parse)(FastArgs) = a->codec == B2_CODEC_LZ4 ? parse_kernel : a->codec == B2_CODEC_ZLIB ? dparse_kernel : zparse_kernel;
+    const long long njobs = (long long)a->map.nfull * a->map.nsplits * a->groups_full + a->groups_left;
+    const int threads = a->threads;
+    const size_t smem = (size_t)a->win_bytes + 64;
+    int per_sm = (int)((size_t)220 * 1024 / (smem + 1024));
+    if (per_sm * threads > 2048) per_sm = 2048 / threads;
+    if (per_sm < 1) per_sm = 1;
+    long long ctas = njobs;
+    const long long cap = (long long)num_sms() * per_sm;
+    if (ctas > cap) ctas = cap;
+    ProfScope ps(B2_K_PARSE, s->s);
+    parse<<<(unsigned)ctas, threads, smem, s->s>>>(take_tickets(a, njobs, ctas));      /* one ticket-drawing thread per CTA */
     CK(cudaGetLastError());
   }
+  void (*back)(FastArgs) = fscan_kernel;
+  int warps = FSCAN_WARPS, kind = B2_K_SCAN;
+  size_t smem = 0;
+  if (a->codec == B2_CODEC_ZSTD) { back = zenc_kernel; warps = ZE_WARPS; smem = ZE_WARPS * ZE_SMEM_BYTES; kind = B2_K_ZENC; }
+  if (a->codec == B2_CODEC_ZLIB) { back = denc_kernel; warps = DZ_WARPS; smem = DZ_WARPS * DZ_SMEM_BYTES; kind = B2_K_DENC; }
+  if (a->codec == B2_CODEC_SNAPPY) { back = senc_kernel; warps = SN_WARPS; kind = B2_K_SENC; }
+  ProfScope ps(kind, s->s);
+  back<<<(a->map.nstreams + warps - 1) / warps, warps * 32, smem, s->s>>>(*a);
+  CK(cudaGetLastError());
   return 0;
 }
 
@@ -358,10 +336,7 @@ extern "C" int b2_launch_decode(const DecodeArgs* a, b2_stream_t s) {
     if (ctas > cap) ctas = cap;
     if (ctas <= 0) return 0;
     ProfScope ps(B2_K_DECODE, s->s);
-    DecodeArgs args = *a;
-    args.queue_base = *a->queue_base_host;
-    *a->queue_base_host += (unsigned)a->map.nstreams + (unsigned)ctas;      /* one ticket-drawing warp per CTA */
-    decode_pair_kernel<<<ctas, 64, LZ4P_SMEM, s->s>>>(args);
+    decode_pair_kernel<<<ctas, 64, LZ4P_SMEM, s->s>>>(take_tickets(a, a->map.nstreams, ctas));      /* one ticket-drawing warp per CTA */
     CK(cudaGetLastError());
     return 0;
   }
@@ -370,9 +345,7 @@ extern "C" int b2_launch_decode(const DecodeArgs* a, b2_stream_t s) {
   if (ctas <= 0) return 0;
   ProfScope ps(B2_K_DECODE, s->s);
   const size_t sm = (size_t)wpc * LZ4D_SMEM;
-  DecodeArgs args = *a;
-  args.queue_base = *a->queue_base_host;
-  *a->queue_base_host += (unsigned)a->map.nstreams + (unsigned)ctas * (unsigned)wpc;
+  const DecodeArgs args = take_tickets(a, a->map.nstreams, ctas * wpc);
   if (a->codec == B2_CODEC_LZ4) decode_kernel<B2_CODEC_LZ4><<<ctas, wpc * 32, sm, s->s>>>(args);
   else if (a->codec == B2_CODEC_ZLIB) decode_kernel<B2_CODEC_ZLIB><<<ctas, wpc * 32, sm, s->s>>>(args);
   else if (a->codec == B2_CODEC_ZSTD) decode_kernel<B2_CODEC_ZSTD><<<ctas, wpc * 32, sm, s->s>>>(args);

@@ -131,7 +131,7 @@ typedef struct {
   int in_use, ready, dev;
   b2_stream_t stream;
   b2_buf in, filt, slots, out, csizes, needs, bstarts;
-  b2_buf prev, segs, seg_done, ptail;   /* segment-parallel LZ4 parse (dev_lz4fast.cuh) */
+  b2_buf prev, segs, ptail;   /* segment-parallel LZ4 parse (dev_lz4fast.cuh) */
   b2_buf plan;          /* getitems planned on the GPU: its scratch */
   int* d_result;        /* B2_R_* words (b2_args.h): cbytes, fits, status, work-queue and done counters */
   int* h_result;        /* pinned mirror */
@@ -165,7 +165,7 @@ static void ws_teardown(b2_ws* w) {
   int k;
   buf_free(&w->in); buf_free(&w->filt); buf_free(&w->slots); buf_free(&w->out);
   buf_free(&w->csizes); buf_free(&w->needs); buf_free(&w->bstarts);
-  buf_free(&w->prev); buf_free(&w->segs); buf_free(&w->seg_done); buf_free(&w->ptail); buf_free(&w->plan);
+  buf_free(&w->prev); buf_free(&w->segs); buf_free(&w->ptail); buf_free(&w->plan);
   for (k = 0; k < B2_STAGE_DEPTH; k++) {
     if (w->stage[k]) b2_pinned_free(w->stage[k]);
     if (w->stage_ev[k]) b2_event_destroy(w->stage_ev[k]);
@@ -183,7 +183,6 @@ static void ws_teardown(b2_ws* w) {
 static void ws_reset_counters(b2_ws* w) {
   b2_stream_sync(w->stream);
   b2_memset_dev(w->d_result, 0, 4 * B2_R_WORDS, w->stream);
-  if (w->seg_done.p) b2_memset_dev(w->seg_done.p, 0, w->seg_done.cap, w->stream);
   b2_stream_sync(w->stream);
   w->queue_base = 0;
 }
@@ -257,13 +256,6 @@ static int buf_ensure(b2_buf* b, size_t need) {
   return 0;
 }
 
-/* a buffer of counters that the kernels leave at zero: cleared only when it is (re)allocated */
-static int buf_ensure_zeroed(b2_ws* w, b2_buf* b, size_t need) {
-  if (need <= b->cap) return 0;
-  if (buf_ensure(b, need)) return -1;
-  return b2_memset_dev(b->p, 0, b->cap, w->stream);
-}
-
 int blosc_free_resources(void) {                              /* blosc.h:411 */
   int i;
   pthread_mutex_lock(&g_ws_mutex);
@@ -272,7 +264,7 @@ int blosc_free_resources(void) {                              /* blosc.h:411 */
     if (w->in_use || !w->ready) continue;
     buf_free(&w->in); buf_free(&w->filt); buf_free(&w->slots); buf_free(&w->out);
     buf_free(&w->csizes); buf_free(&w->needs); buf_free(&w->bstarts);
-    buf_free(&w->prev); buf_free(&w->segs); buf_free(&w->seg_done); buf_free(&w->ptail); buf_free(&w->plan);
+    buf_free(&w->prev); buf_free(&w->segs); buf_free(&w->ptail); buf_free(&w->plan);
   }
   pthread_mutex_unlock(&g_ws_mutex);
   return 0;
@@ -710,76 +702,55 @@ static int compress_impl(int clevel, int doshuffle, size_t typesize, size_t nbyt
     ea.scan = sa;
     launched = 1;
     memset(&ca, 0, sizeof ca);
-    if (compcode == BLOSC_ZSTD || compcode == BLOSC_ZLIB || compcode == BLOSC_SNAPPY) {
-      /* the zstd encoder (dev_zstdenc.cuh): the index and windows of the segment-parallel parse, sequence records
-       * instead of LZ4 bytes, then one warp per zstd frame.  The DEFLATE encoder (dev_deflate.cuh) shares the parse,
-       * with offsets <= 32768, then one warp writes each zlib stream.  The snappy encoder (dev_snappy.cuh) takes the
-       * zstd records as they are, then one warp writes each snappy stream. */
+    if (compcode == BLOSC_ZSTD || compcode == BLOSC_ZLIB || compcode == BLOSC_SNAPPY || compcode == BLOSC_LZ4HC ||
+        (compcode == BLOSC_LZ4 && lz4_fast_wanted())) {
+      /* The segment-parallel encoders (b2_launch_fast): a hash-chain index, one parse CTA per window with one lane per
+       * segment, then one warp per stream.  LZ4 and lz4hc parse into LZ4 bytes that compaction stitches together; the
+       * zstd (dev_zstdenc.cuh), DEFLATE (dev_deflate.cuh, offsets <= 32768) and snappy (dev_snappy.cuh) encoders parse
+       * into sequence records, then one warp writes each stream. */
       FastArgs fx;
       const int neblock = bs / nsplits;
       const int longest = neblock > leftover ? neblock : leftover;
+      /* a window is the whole stream when it fits in B2_FAST_WIN_MAX, rounded up to whole warps of segments */
       int win = (longest + 32 * B2_FAST_SEG - 1) / (32 * B2_FAST_SEG) * (32 * B2_FAST_SEG);
       long long nsegs;
-      b2_buf* recs;
-      memset(&fx, 0, sizeof fx);
       if (win > B2_FAST_WIN_MAX) win = B2_FAST_WIN_MAX;
+      memset(&fx, 0, sizeof fx);
       fx.map = ea.map; fx.in = ea.in; fx.slots = ea.slots; fx.csizes = ea.csizes; fx.needs = ea.needs;
       fx.segs_full = (neblock + B2_FAST_SEG - 1) / B2_FAST_SEG; fx.segs_left = (leftover + B2_FAST_SEG - 1) / B2_FAST_SEG;
       fx.win_bytes = win; fx.threads = win / B2_FAST_SEG;
       fx.groups_full = (neblock + win - 1) / win; fx.groups_left = (leftover + win - 1) / win;
-      /* effort: the chain depth and laziness of "lz4hc" (blosc.c:499-511 maps clevel to zstd levels 1..22) */
-      fx.depth = clevel <= 2 ? 4 : (clevel >= 8 ? 128 : (1 << (clevel - 1))); fx.accel = 1;
-      fx.hash_mask = 0xffff; fx.lazy = 64;
       nsegs = (long long)nfull * nsplits * fx.segs_full + fx.segs_left;
-      /* the records need 256 bytes per segment; whichever of the staging / filter buffers does not hold the
-       * codec input is free for them */
-      recs = d_codec_in == (const uint8_t*)w->in.p ? &w->filt : &w->in;
-      if (buf_ensure(&w->prev, 2 * (size_t)nb + 64)) break;
-      if (buf_ensure(recs, (size_t)nsegs * B2_FAST_SEG + 64)) break;
-      if (buf_ensure(&w->segs, (size_t)nsegs * 4 + 64)) break;
-      fx.zstd = compcode == BLOSC_ZSTD; fx.deflate = compcode == BLOSC_ZLIB;
-      /* snappy is a speed codec: the effort of the segment-parallel LZ4 parse (chain depth 3 clevel + 1, no lazy
-       * matching) */
-      if (compcode == BLOSC_SNAPPY) { fx.depth = 3 * clevel + 1; fx.lazy = 0; }
+      fx.codec = compcode == BLOSC_ZSTD ? B2_CODEC_ZSTD : compcode == BLOSC_ZLIB ? B2_CODEC_ZLIB
+               : compcode == BLOSC_SNAPPY ? B2_CODEC_SNAPPY : B2_CODEC_LZ4;
+      /* effort (chain depth, accel, lazy matching).  "lz4hc" (blosc.c:422-433 hands clevel to LZ4_compress_HC) takes
+       * LZ4HC's search effort -- 2^(level-1) candidates, capped -- and no skipping over literals; so do zstd
+       * (blosc.c:499-511 maps clevel to zstd levels 1..22) and zlib.  Snappy is a speed codec: fast LZ4's effort. */
+      fx.hash_mask = 0xffff;
+      if (compcode == BLOSC_LZ4) { fx.depth = 3 * clevel + 1; fx.accel = ea.accel; fx.lazy = 0; }
+      else if (compcode == BLOSC_SNAPPY) { fx.depth = 3 * clevel + 1; fx.accel = 1; fx.lazy = 0; }
+      else { fx.depth = clevel <= 2 ? 4 : (clevel >= 8 ? 128 : (1 << (clevel - 1))); fx.accel = 1; fx.lazy = 64; }
       /* zlib's FLEVEL for compress2(.., clevel) (blosc.c:472-483, deflate.c) */
       fx.flevel = clevel < 2 ? 0 : (clevel < 6 ? 1 : (clevel == 6 ? 2 : 3));
-      fx.prev = (uint16_t*)w->prev.p; fx.recs = (uint32_t*)recs->p; fx.nrec = (uint32_t*)w->segs.p;
-      fx.queue = ea.queue; fx.queue_base_host = ea.queue_base_host; fx.done = ea.done;
-      fx.fold_scan = ea.fold_scan; fx.scan = sa;
-      fx.snappy = compcode == BLOSC_SNAPPY; fx.ebsize = bs + 4 * ts;
-      if (b2_launch_fast(&fx, w->stream)) break;
-    } else if (ea.codec == B2_CODEC_LZ4 && (compcode == BLOSC_LZ4HC || lz4_fast_wanted())) {
-      FastArgs fx;
-      const int neblock = bs / nsplits;
-      memset(&fx, 0, sizeof fx);
-      fx.map = ea.map; fx.in = ea.in; fx.slots = ea.slots; fx.csizes = ea.csizes; fx.needs = ea.needs;
-      fx.segs_full = (neblock + B2_FAST_SEG - 1) / B2_FAST_SEG; fx.segs_left = (leftover + B2_FAST_SEG - 1) / B2_FAST_SEG;
-      {
-        /* one parse CTA per window: the whole stream when it fits in B2_FAST_WIN_MAX, rounded up to whole warps of segments */
-        const int longest = neblock > leftover ? neblock : leftover;
-        int win = (longest + 32 * B2_FAST_SEG - 1) / (32 * B2_FAST_SEG) * (32 * B2_FAST_SEG);
-        if (win > B2_FAST_WIN_MAX) win = B2_FAST_WIN_MAX;
-        fx.win_bytes = win;
-        fx.threads = win / B2_FAST_SEG;
-        fx.groups_full = (neblock + win - 1) / win; fx.groups_left = (leftover + win - 1) / win;
-      }
-      fx.depth = 3 * clevel + 1; fx.accel = ea.accel;
-      /* "lz4hc" (blosc.c:422-433 hands clevel to LZ4_compress_HC): the same hash-chain parser, with LZ4HC's search
-       * effort -- 2^(level-1) candidates, capped -- and no skipping over literals */
-      fx.hash_mask = 0xffff; fx.lazy = 0;
-      if (compcode == BLOSC_LZ4HC) {
-        fx.depth = clevel <= 2 ? 4 : (clevel >= 8 ? 128 : (1 << (clevel - 1))); fx.accel = 1;
-        fx.hash_mask = 0xffff; fx.lazy = 64;
-      }
+      fx.ebsize = bs + 4 * ts;
       if (buf_ensure(&w->prev, 2 * (size_t)nb + 64)) break;
-      if (buf_ensure(&w->segs, ((size_t)nfull * nsplits * fx.segs_full + fx.segs_left + 8) * sizeof(FastSeg))) break;
-      if (buf_ensure_zeroed(w, &w->seg_done, (size_t)ea.map.nstreams * 4 + 64)) break;
-      if (buf_ensure(&w->ptail, (size_t)ea.map.nstreams * 4 + 64)) break;
-      fx.prev = (uint16_t*)w->prev.p; fx.segs = (FastSeg*)w->segs.p; fx.seg_done = (int*)w->seg_done.p; fx.ptail = (int*)w->ptail.p;
+      fx.prev = (uint16_t*)w->prev.p;
+      if (fx.codec == B2_CODEC_LZ4) {
+        if (buf_ensure(&w->segs, ((size_t)nsegs + 8) * sizeof(FastSeg))) break;
+        if (buf_ensure(&w->ptail, (size_t)ea.map.nstreams * 4 + 64)) break;
+        fx.segs = (FastSeg*)w->segs.p; fx.ptail = (int*)w->ptail.p;
+        ca.segs = fx.segs; ca.ptail = fx.ptail; ca.segs_full = fx.segs_full; ca.segs_left = fx.segs_left;
+      } else {
+        /* the records need 256 bytes per segment; whichever of the staging / filter buffers does not hold the
+         * codec input is free for them */
+        b2_buf* recs = d_codec_in == (const uint8_t*)w->in.p ? &w->filt : &w->in;
+        if (buf_ensure(recs, (size_t)nsegs * B2_FAST_SEG + 64)) break;
+        if (buf_ensure(&w->segs, (size_t)nsegs * 4 + 64)) break;
+        fx.recs = (uint32_t*)recs->p; fx.nrec = (uint32_t*)w->segs.p;
+      }
       fx.queue = ea.queue; fx.queue_base_host = ea.queue_base_host; fx.done = ea.done;
       fx.fold_scan = ea.fold_scan; fx.scan = sa;
       if (b2_launch_fast(&fx, w->stream)) break;
-      ca.segs = fx.segs; ca.ptail = fx.ptail; ca.segs_full = fx.segs_full; ca.segs_left = fx.segs_left;
     } else if (b2_launch_encode(&ea, w->stream)) break;
     if (!ea.fold_scan && b2_launch_scan(&sa, w->stream)) break;
     if (dest_dev && !pl) d_dest = (uint8_t*)dest;

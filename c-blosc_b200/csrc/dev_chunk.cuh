@@ -73,6 +73,23 @@ DEV void stream_locate(const StreamMap& m, int idx, int* block, long long* off, 
   if (blocks) *block = blocks[*block];
 }
 
+/* The end of every encode and decode launch, for one warp that finished `mine` streams: the warp that completes the
+ * count of finished streams runs `last` and puts the count back to zero for the next launch on this workspace (the
+ * ticket counter is never reset: warps that got no stream may still be polling it). */
+template <class Last>
+DEV void streams_done(int* done, const int nstreams, const int mine, Last last) {
+  if (mine == 0) return;
+  __threadfence();
+  int is_last = 0;
+  if (lane_id() == 0) is_last = atomicAdd(done, mine) + mine == nstreams;
+  is_last = __shfl_sync(FULLMASK, is_last, 0);
+  if (!is_last) return;
+  __threadfence();
+  last();
+  __syncwarp();
+  if (lane_id() == 0) *done = 0;
+}
+
 
 /* L2 loads for words written by other SMs during this launch */
 DEV int ld_cg_i32(const int* p) {
@@ -83,27 +100,30 @@ DEV int ld_cg_i32(const int* p) {
 #endif
 }
 
-/* The block scan of t_blosc's ordered copy-out (blosc.c:1843-1856) by ONE warp: exclusive scan of the
- * per-block compressed sizes -> bstarts, total cbytes and the "does it fit" verdict.  Run by the warp
- * that finishes the last stream of an encode launch, so compression needs no separate scan launch
- * (a 1-CTA launch queues behind the encoders of every other chunk in flight). */
-DEV void warp_scan_blocks(const ScanArgs& a) {
-  const int lane = lane_id();
-  const int nblocks = a.nfull + (a.has_leftover ? 1 : 0);
-  const int per = (nblocks + 31) / 32;
-  const int b0 = lane * per < nblocks ? lane * per : nblocks, b1 = b0 + per < nblocks ? b0 + per : nblocks;
+/* The bytes that blocks [b0, b1) take in the chunk: every split's size prefix and its compressed (or raw) bytes */
+DEV long long scan_sum(const ScanArgs& a, const int* csizes, const int b0, const int b1) {
   long long sum = 0;
   for (int b = b0; b < b1; b++) {
-    if (b < a.nfull) for (int s = 0; s < a.nsplits; s++) sum += 4 + (long long)ld_cg_i32(&a.csizes[(long long)b * a.nsplits + s]);
-    else sum += 4 + (long long)ld_cg_i32(&a.csizes[(long long)a.nfull * a.nsplits]);
+    if (b < a.nfull) for (int s = 0; s < a.nsplits; s++) sum += 4 + (long long)ld_cg_i32(&csizes[(long long)b * a.nsplits + s]);
+    else sum += 4 + (long long)ld_cg_i32(&csizes[(long long)a.nfull * a.nsplits]);
   }
-  long long incl = sum;
+  return sum;
+}
+
+/* Inclusive prefix sum over the warp */
+DEV long long warp_prefix(const long long v) {
+  long long incl = v;
 #pragma unroll
   for (int d = 1; d < 32; d <<= 1) {
     const long long t = __shfl_up_sync(FULLMASK, incl, d);
-    if (lane >= d) incl += t;
+    if (lane_id() >= d) incl += t;
   }
-  long long pos = 16 + 4ll * nblocks + (incl - sum);
+  return incl;
+}
+
+/* Blocks [b0, b1), the first of which starts at `pos`: writes their bstarts and returns 1 if serial_blosc would give
+ * up on one of their splits */
+DEV int scan_place(const ScanArgs& a, const int b0, const int b1, long long pos) {
   int bad = 0;
   for (int b = b0; b < b1; b++) {
     a.bstarts[b] = (int)(pos > 0x7fffffffll ? 0x7fffffffll : pos);
@@ -122,12 +142,49 @@ DEV void warp_scan_blocks(const ScanArgs& a) {
       pos += 4 + (long long)c;
     }
   }
+  return bad;
+}
+
+/* The block scan of t_blosc's ordered copy-out (blosc.c:1843-1856) by ONE warp: exclusive scan of the
+ * per-block compressed sizes -> bstarts, total cbytes and the "does it fit" verdict.  Run by the warp
+ * that finishes the last stream of an encode launch, so compression needs no separate scan launch
+ * (a 1-CTA launch queues behind the encoders of every other chunk in flight). */
+DEV void warp_scan_blocks(const ScanArgs& a) {
+  const int lane = lane_id();
+  const int nblocks = a.nfull + (a.has_leftover ? 1 : 0);
+  const int per = (nblocks + 31) / 32;
+  const int b0 = lane * per < nblocks ? lane * per : nblocks, b1 = b0 + per < nblocks ? b0 + per : nblocks;
+  const long long sum = scan_sum(a, a.csizes, b0, b1);
+  const long long incl = warp_prefix(sum);
+  const int bad = scan_place(a, b0, b1, 16 + 4ll * nblocks + (incl - sum));
   const unsigned anybad = __ballot_sync(FULLMASK, bad);
   const long long total = 16 + 4ll * nblocks + __shfl_sync(FULLMASK, incl, 31);
   if (lane == 0) {
     a.result[B2_R_CBYTES] = (int)(total > 0x7fffffffll ? 0x7fffffffll : total);
     a.result[B2_R_FITS] = (total <= a.destsize && anybad == 0u) ? 1 : 0;       /* blosc.c:1848 / :836-839 give up */
   }
+}
+
+/* The stream loop of an exact encode launch, for one warp: every stream it draws goes to
+ * `codec(idx, in, len, out, &need)`, which writes at most len bytes to out and returns the compressed size.
+ * Returns the number of streams this warp finished. */
+template <class Codec>
+DEV int encode_streams(const EncodeArgs& a, Codec codec) {
+  int mine = 0;
+  for (;;) {
+    const int idx = next_stream(a.queue, a.queue_base, a.map);
+    if (idx < 0) break;
+    int block, len, split;
+    long long off;
+    stream_locate(a.map, idx, &block, &off, &len, &split);
+    int need = 0;
+    int c = codec(idx, a.in + off, len, a.slots + off, &need);
+    if (c <= 0 || c >= len) c = len;           /* blosc.c:705-714: incompressible split is stored raw */
+    if (lane_id() == 0) { a.csizes[idx] = c; a.needs[idx] = need; }
+    mine++;
+    __syncwarp();
+  }
+  return mine;
 }
 
 __global__ void encode_kernel(EncodeArgs a) {
@@ -138,39 +195,15 @@ __global__ void encode_kernel(EncodeArgs a) {
 #endif
   const int warp = (int)(threadIdx.x >> 5);
   void* tab = smem + (size_t)warp * a.table_bytes;
-  int mine = 0;
-  for (;;) {
-    const int idx = next_stream(a.queue, a.queue_base, a.map);
-    if (idx < 0) break;
-    int block, len, split;
-    long long off;
-    stream_locate(a.map, idx, &block, &off, &len, &split);
-    const u8* in = a.in + off;
-    u8* out = a.slots + off;
-    int c, need = 0;
+  const int mine = encode_streams(a, [&](int, const u8* in, int len, u8* out, int* need) {
     if (a.codec == B2_CODEC_LZ4) {
-      if (a.table_bytes == LZ4_TAB17_BYTES) c = lz4_encode_warp<false, true>(in, len, out, len, a.accel, tab, &need);   /* host guarantees the length range */
-      else if (len < 65536 + LZ4_MFLIMIT - 1) c = lz4_encode_warp<true>(in, len, out, len, a.accel, tab, &need);   /* lz4.c:710,1389 */
-      else c = lz4_encode_warp<false>(in, len, out, len, a.accel, tab, &need);
-    } else {
-      c = blz_encode_warp(a.clevel, in, len, out, len, a.split_flag, tab, a.table_bytes, &need);
+      if (a.table_bytes == LZ4_TAB17_BYTES) return lz4_encode_warp<false, true>(in, len, out, len, a.accel, tab, need);   /* host guarantees the length range */
+      if (len < 65536 + LZ4_MFLIMIT - 1) return lz4_encode_warp<true>(in, len, out, len, a.accel, tab, need);   /* lz4.c:710,1389 */
+      return lz4_encode_warp<false>(in, len, out, len, a.accel, tab, need);
     }
-    if (c <= 0 || c >= len) c = len;           /* blosc.c:705-714: incompressible split is stored raw */
-    if (lane_id() == 0) { a.csizes[idx] = c; a.needs[idx] = need; }
-    mine++;
-    __syncwarp();
-  }
-  /* whoever completes the stream count does the block scan and puts the counters back to zero */
-  if (mine == 0) return;
-  __threadfence();
-  int last = 0;
-  if (lane_id() == 0) last = atomicAdd(a.done, mine) + mine == a.map.nstreams;
-  last = __shfl_sync(FULLMASK, last, 0);
-  if (!last) return;
-  __threadfence();
-  if (a.fold_scan) warp_scan_blocks(a.scan);
-  __syncwarp();
-  if (lane_id() == 0) *a.done = 0;       /* (the ticket counter is never reset: warps that got no stream may still be polling it) */
+    return blz_encode_warp(a.clevel, in, len, out, len, a.split_flag, tab, a.table_bytes, need);
+  });
+  streams_done(a.done, a.map.nstreams, mine, [&] { if (a.fold_scan) warp_scan_blocks(a.scan); });
 }
 
 
@@ -214,19 +247,10 @@ __global__ void __launch_bounds__(TEAM_WARPS * 32, TEAM_CTAS_PER_SM) encode_team
   for (int k = 3; k >= 0; k--) if (tm->sub[k] == tm->slot) walker = k;
 #endif
   if (warp != walker) { lz4_team_preparer(tm, tab, (warp - walker - 1) & 3); return; }
-  int mine = 0;
-  for (;;) {
-    const int idx = next_stream(a.queue, a.queue_base, a.map);
-    if (idx < 0) break;
-    int block, len, split;
-    long long off;
-    stream_locate(a.map, idx, &block, &off, &len, &split);
-    const u8* in = a.in + off;
-    u8* out = a.slots + off;
-    int c, need = 0;
+  const int mine = encode_streams(a, [&](int idx, const u8* in, int len, u8* out, int* need) {
     LZ4C_T(c_total);
-    if (len < 65536 + LZ4_MFLIMIT - 1) c = lz4_encode_warp<true, false, true>(in, len, out, len, a.accel, tab, &need, tm);   /* lz4.c:710,1389 */
-    else c = lz4_encode_warp<false, false, true>(in, len, out, len, a.accel, tab, &need, tm);
+    const int c = len < 65536 + LZ4_MFLIMIT - 1 ? lz4_encode_warp<true, false, true>(in, len, out, len, a.accel, tab, need, tm)   /* lz4.c:710,1389 */
+                                                 : lz4_encode_warp<false, false, true>(in, len, out, len, a.accel, tab, need, tm);
 #ifdef B2_LZ4_CYCLES
     {
       const unsigned long long total = (unsigned long long)(clock64() - c_total);
@@ -241,25 +265,13 @@ __global__ void __launch_bounds__(TEAM_WARPS * 32, TEAM_CTAS_PER_SM) encode_team
       if (k < LZ4C_N) tm->cyc[k] = 0;
     }
 #endif
-    if (c <= 0 || c >= len) c = len;           /* blosc.c:705-714: incompressible split is stored raw */
-    if (lane_id() == 0) { a.csizes[idx] = c; a.needs[idx] = need; }
-    mine++;
-    __syncwarp();
-  }
+    return c;
+  });
   if (lane_id() == 0) *(volatile int*)&tm->cmd = LZ4T_QUIT;
   __syncwarp();
   __threadfence_block();
   bar_arrive(LZ4T_BAR_GO(0), 64); bar_arrive(LZ4T_BAR_GO(1), 64); bar_arrive(LZ4T_BAR_GO(2), 64);
-  if (mine == 0) return;
-  __threadfence();
-  int last = 0;
-  if (lane_id() == 0) last = atomicAdd(a.done, mine) + mine == a.map.nstreams;
-  last = __shfl_sync(FULLMASK, last, 0);
-  if (!last) return;
-  __threadfence();
-  if (a.fold_scan) warp_scan_blocks(a.scan);
-  __syncwarp();
-  if (lane_id() == 0) *a.done = 0;
+  streams_done(a.done, a.map.nstreams, mine, [&] { if (a.fold_scan) warp_scan_blocks(a.scan); });
 }
 
 
@@ -358,16 +370,16 @@ DEV void fast_parse_body(const FastArgs& a, u8* smem) {
 __global__ void __launch_bounds__(B2_FAST_WIN_MAX / FAST_SEG, 3) parse_kernel(FastArgs a) {
 #ifdef SIMT_EMU
   u8* smem = simt::g_dynsmem;
-  if (a.zstd) { fast_parse_body<true>(a, smem); return; }     /* the emulator launches the zstd parse under this name */
-  if (a.deflate) { fast_parse_body<true, DZ_MAXD>(a, smem); return; }   /* and the DEFLATE parse */
-  if (a.snappy) { fast_parse_body<true>(a, smem); return; }          /* and the snappy encoder's (zparse) */
+  if (a.codec == B2_CODEC_ZSTD) { fast_parse_body<true>(a, smem); return; }     /* the emulator launches the zstd parse under this name */
+  if (a.codec == B2_CODEC_ZLIB) { fast_parse_body<true, DZ_MAXD>(a, smem); return; }   /* and the DEFLATE parse */
+  if (a.codec == B2_CODEC_SNAPPY) { fast_parse_body<true>(a, smem); return; }          /* and the snappy encoder's (zparse) */
 #else
   extern __shared__ __align__(16) u8 smem[];
 #endif
   fast_parse_body<false>(a, smem);
 }
 
-/* FastArgs.zstd: the zstd encoder's parse (the backend launches it instead of parse_kernel) */
+/* the zstd and snappy encoders' parse (the backend launches it instead of parse_kernel) */
 __global__ void __launch_bounds__(B2_FAST_WIN_MAX / FAST_SEG, 3) zparse_kernel(FastArgs a) {
 #ifdef SIMT_EMU
   u8* smem = simt::g_dynsmem;
@@ -377,7 +389,7 @@ __global__ void __launch_bounds__(B2_FAST_WIN_MAX / FAST_SEG, 3) zparse_kernel(F
   fast_parse_body<true>(a, smem);
 }
 
-/* FastArgs.deflate: the DEFLATE encoder's parse, offsets <= 32768 (the backend launches it instead of parse_kernel) */
+/* the DEFLATE encoder's parse, offsets <= 32768 (the backend launches it instead of parse_kernel) */
 __global__ void __launch_bounds__(B2_FAST_WIN_MAX / FAST_SEG, 3) dparse_kernel(FastArgs a) {
 #ifdef SIMT_EMU
   u8* smem = simt::g_dynsmem;
@@ -385,6 +397,26 @@ __global__ void __launch_bounds__(B2_FAST_WIN_MAX / FAST_SEG, 3) dparse_kernel(F
   extern __shared__ __align__(16) u8 smem[];
 #endif
   fast_parse_body<true, DZ_MAXD>(a, smem);
+}
+
+/* The stream loop of a segment-parallel back half, for one warp: the warps take the streams in a grid stride, and
+ * `codec(idx, off, len)` writes stream idx (bytes [off, off + len) of the input) into at most len bytes of its slot and
+ * returns the compressed size.  Returns the number of streams this warp finished. */
+template <class Codec>
+DEV int fast_streams(const FastArgs& a, Codec codec) {
+  const int warp = (int)(threadIdx.x >> 5), nwarps = (int)(blockDim.x >> 5);
+  int mine = 0;
+  for (int idx = (int)blockIdx.x * nwarps + warp; idx < a.map.nstreams; idx += (int)gridDim.x * nwarps) {
+    int block, len, split;
+    long long off;
+    stream_locate(a.map, idx, &block, &off, &len, &split);
+    int c = codec(idx, off, len);
+    if (c <= 0 || c >= len) c = len;           /* blosc.c:705-714: incompressible split is stored raw */
+    if (lane_id() == 0) { a.csizes[idx] = c; a.needs[idx] = c; }
+    mine++;
+    __syncwarp();
+  }
+  return mine;
 }
 
 /* One warp per stream: scan of its segment records (pending literals, continued matches, output offsets, compressed
@@ -395,80 +427,39 @@ DEV void denc_body(const FastArgs& a, DzSm* S);
 DEV void senc_body(const FastArgs& a);
 __global__ void __launch_bounds__(FSCAN_WARPS * 32) fscan_kernel(FastArgs a) {
 #ifdef SIMT_EMU
-  if (a.zstd) {                                    /* the emulator launches the zstd entropy stage under this name */
+  if (a.codec == B2_CODEC_ZSTD) {                  /* the emulator launches the zstd entropy stage under this name */
     __shared__ ZeSm ztab[FSCAN_WARPS];
     zenc_body(a, &ztab[threadIdx.x >> 5]);
     return;
   }
-  if (a.deflate) {                                 /* and the DEFLATE one */
+  if (a.codec == B2_CODEC_ZLIB) {                  /* and the DEFLATE one */
     __shared__ DzSm dtab[FSCAN_WARPS];
     denc_body(a, &dtab[threadIdx.x >> 5]);
     return;
   }
-  if (a.snappy) { senc_body(a); return; }          /* and the snappy stream writer */
+  if (a.codec == B2_CODEC_SNAPPY) { senc_body(a); return; }          /* and the snappy stream writer */
 #endif
-  const int lane = lane_id();
   const int nfs = a.map.nfull * a.map.nsplits;
-  int mine = 0;
-  for (int idx = (int)blockIdx.x * FSCAN_WARPS + (int)(threadIdx.x >> 5); idx < a.map.nstreams; idx += (int)gridDim.x * FSCAN_WARPS) {
-    int block, len, split;
-    long long off;
-    stream_locate(a.map, idx, &block, &off, &len, &split);
+  const int mine = fast_streams(a, [&](int idx, long long, int len) {
     int ptail = 0;
-    int c = lz4f_stream_scan(a.segs + (long long)idx * a.segs_full, idx < nfs ? a.segs_full : a.segs_left, len, &ptail);
-    if (c >= len) c = len;                         /* blosc.c:705-714: incompressible split is stored raw */
-    if (lane == 0) { a.csizes[idx] = c; a.needs[idx] = c; a.ptail[idx] = ptail; }
-    mine++;
-    __syncwarp();
-  }
-  if (mine == 0) return;
-  __threadfence();
-  int last = 0;
-  if (lane == 0) last = atomicAdd(a.done, mine) + mine == a.map.nstreams;
-  last = __shfl_sync(FULLMASK, last, 0);
-  if (!last) return;
-  __threadfence();
-  if (a.fold_scan) warp_scan_blocks(a.scan);
-  __syncwarp();
-  if (lane == 0) *a.done = 0;
+    const int c = lz4f_stream_scan(a.segs + (long long)idx * a.segs_full, idx < nfs ? a.segs_full : a.segs_left, len, &ptail);
+    if (lane_id() == 0) a.ptail[idx] = ptail;
+    return c;
+  });
+  streams_done(a.done, a.map.nstreams, mine, [&] { if (a.fold_scan) warp_scan_blocks(a.scan); });
 }
 
 
 /* ---- segment-parallel zstd (dev_zstdenc.cuh): index_kernel, zparse_kernel, then one warp per frame ---- */
-DEV void fast_streams_done(const FastArgs& a, const int mine);
 DEV void zenc_body(const FastArgs& a, ZeSm* S) {
-  const int lane = lane_id(), warp = (int)(threadIdx.x >> 5), nwarps = (int)(blockDim.x >> 5);
-  int mine = 0;
-  for (int idx = (int)blockIdx.x * nwarps + warp; idx < a.map.nstreams; idx += (int)gridDim.x * nwarps) {
-    int block, len, split;
-    long long off;
-    stream_locate(a.map, idx, &block, &off, &len, &split);
+  const int mine = fast_streams(a, [&](int idx, long long off, int len) {
     const long long gseg = (long long)idx * a.segs_full;
     int c = 0;
-    if (lane == 0)
+    if (lane_id() == 0)
       c = zse_frame_serial(*S, a.in + off, len, a.recs + gseg * ZE_SEG_RECS, a.nrec + gseg, (u8*)(a.prev + off), a.slots + off);
-    c = __shfl_sync(FULLMASK, c, 0);
-    if (c >= len) c = len;                         /* blosc.c:705-714: incompressible split is stored raw */
-    if (lane == 0) { a.csizes[idx] = c; a.needs[idx] = c; }
-    mine++;
-    __syncwarp();
-  }
-  fast_streams_done(a, mine);
-}
-
-/* whoever completes the stream count does the block scan, exactly as in encode_kernel */
-DEV void fast_streams_done(const FastArgs& a, const int mine) {
-  const int lane = lane_id();
-  if (mine == 0) return;
-  __threadfence();
-  int last = 0;
-  if (lane == 0) last = atomicAdd(a.done, mine) + mine == a.map.nstreams;
-  last = __shfl_sync(FULLMASK, last, 0);
-  if (!last) return;
-  __threadfence();
-  if (a.fold_scan) warp_scan_blocks(a.scan);
-  __syncwarp();
-  if (lane == 0) *a.done = 0;
+    return __shfl_sync(FULLMASK, c, 0);
+  });
+  streams_done(a.done, a.map.nstreams, mine, [&] { if (a.fold_scan) warp_scan_blocks(a.scan); });
 }
 
 /* One warp per stream: its frame, lane 0 codes it; the tables live in the warp's ZE_SMEM_BYTES of shared memory */
@@ -483,20 +474,11 @@ __global__ void __launch_bounds__(ZE_WARPS * 32) zenc_kernel(FastArgs a) {
 
 /* ---- segment-parallel DEFLATE (dev_deflate.cuh): index_kernel, dparse_kernel, then one warp per zlib stream ---- */
 DEV void denc_body(const FastArgs& a, DzSm* S) {
-  const int lane = lane_id(), warp = (int)(threadIdx.x >> 5), nwarps = (int)(blockDim.x >> 5);
-  int mine = 0;
-  for (int idx = (int)blockIdx.x * nwarps + warp; idx < a.map.nstreams; idx += (int)gridDim.x * nwarps) {
-    int block, len, split;
-    long long off;
-    stream_locate(a.map, idx, &block, &off, &len, &split);
+  const int mine = fast_streams(a, [&](int idx, long long off, int len) {
     const long long gseg = (long long)idx * a.segs_full;
-    int c = dz_stream(*S, a.in + off, len, a.recs + gseg * ZE_SEG_RECS, a.nrec + gseg, (u8*)(a.prev + off), a.slots + off, a.flevel);
-    if (c >= len) c = len;                         /* blosc.c:705-714: incompressible split is stored raw */
-    if (lane == 0) { a.csizes[idx] = c; a.needs[idx] = c; }
-    mine++;
-    __syncwarp();
-  }
-  fast_streams_done(a, mine);
+    return dz_stream(*S, a.in + off, len, a.recs + gseg * ZE_SEG_RECS, a.nrec + gseg, (u8*)(a.prev + off), a.slots + off, a.flevel);
+  });
+  streams_done(a.done, a.map.nstreams, mine, [&] { if (a.fold_scan) warp_scan_blocks(a.scan); });
 }
 
 /* One warp per stream: its zlib stream; the tables and the bit window live in the warp's DZ_SMEM_BYTES */
@@ -561,17 +543,8 @@ DEV void warp_scan_blocks_snappy(const ScanArgs& a, int* csizes, const int ebsiz
   long long first = 0x7fffffffffffffffll;     /* serial: the first split short of its bound */
   long long pos0 = 0, total = 0;
   for (int pass = 0; pass < 2; pass++) {
-    long long sum = 0;
-    for (int b = b0; b < b1; b++) {
-      if (b < a.nfull) for (int s = 0; s < a.nsplits; s++) sum += 4 + (long long)ld_cg_i32(&csizes[(long long)b * a.nsplits + s]);
-      else sum += 4 + (long long)ld_cg_i32(&csizes[(long long)a.nfull * a.nsplits]);
-    }
-    long long incl = sum;
-#pragma unroll
-    for (int d = 1; d < 32; d <<= 1) {
-      const long long t = __shfl_up_sync(FULLMASK, incl, d);
-      if (lane >= d) incl += t;
-    }
+    const long long sum = scan_sum(a, csizes, b0, b1);
+    const long long incl = warp_prefix(sum);
     pos0 = 16 + 4ll * nblocks + (incl - sum);
     total = 16 + 4ll * nblocks + __shfl_sync(FULLMASK, incl, 31);
     if (!a.serial || pass == 1) break;
@@ -629,29 +602,12 @@ DEV void warp_scan_blocks_snappy(const ScanArgs& a, int* csizes, const int ebsiz
 /* One warp per stream: its snappy stream; whoever completes the stream count runs the snappy block scan */
 #define SN_WARPS 4
 DEV void senc_body(const FastArgs& a) {
-  const int lane = lane_id(), warp = (int)(threadIdx.x >> 5), nwarps = (int)(blockDim.x >> 5);
-  int mine = 0;
-  for (int idx = (int)blockIdx.x * nwarps + warp; idx < a.map.nstreams; idx += (int)gridDim.x * nwarps) {
-    int block, len, split;
-    long long off;
-    stream_locate(a.map, idx, &block, &off, &len, &split);
+  const int mine = fast_streams(a, [&](int idx, long long off, int len) {
     const long long gseg = (long long)idx * a.segs_full;
-    int c = sn_stream(a.in + off, len, a.recs + gseg * ZE_SEG_RECS, a.nrec + gseg, (u8*)(a.prev + off), a.slots + off);
-    if (c >= len) c = len;                         /* blosc.c:705-714: incompressible split is stored raw */
-    if (lane == 0) { a.csizes[idx] = c; a.needs[idx] = c; }
-    mine++;
-    __syncwarp();
-  }
-  if (mine == 0) return;
-  __threadfence();
-  int last = 0;
-  if (lane == 0) last = atomicAdd(a.done, mine) + mine == a.map.nstreams;
-  last = __shfl_sync(FULLMASK, last, 0);
-  if (!last) return;
-  __threadfence();
-  warp_scan_blocks_snappy(a.scan, a.csizes, a.ebsize);      /* (always folded: the host never launches scan_kernel for snappy) */
-  __syncwarp();
-  if (lane == 0) *a.done = 0;
+    return sn_stream(a.in + off, len, a.recs + gseg * ZE_SEG_RECS, a.nrec + gseg, (u8*)(a.prev + off), a.slots + off);
+  });
+  /* (always folded: the host never launches scan_kernel for snappy) */
+  streams_done(a.done, a.map.nstreams, mine, [&] { warp_scan_blocks_snappy(a.scan, a.csizes, a.ebsize); });
 }
 
 __global__ void __launch_bounds__(SN_WARPS * 32) senc_kernel(FastArgs a) { senc_body(a); }
@@ -663,12 +619,7 @@ __global__ void __launch_bounds__(SCAN_THREADS) scan_kernel(ScanArgs a) {
   const int nblocks = a.nfull + (a.has_leftover ? 1 : 0);
   const int per = (nblocks + SCAN_THREADS - 1) / SCAN_THREADS;
   const int b0 = tid * per, b1 = b0 + per < nblocks ? b0 + per : nblocks;
-  long long sum = 0;
-  for (int b = b0; b < b1; b++) {
-    if (b < a.nfull) for (int s = 0; s < a.nsplits; s++) sum += 4 + (long long)a.csizes[(long long)b * a.nsplits + s];
-    else sum += 4 + (long long)a.csizes[(long long)a.nfull * a.nsplits];
-  }
-  part[tid] = sum;
+  part[tid] = scan_sum(a, a.csizes, b0, b1);
   __syncthreads();
   /* Hillis-Steele inclusive scan over the 1024 partials */
   for (int d = 1; d < SCAN_THREADS; d <<= 1) {
@@ -677,32 +628,14 @@ __global__ void __launch_bounds__(SCAN_THREADS) scan_kernel(ScanArgs a) {
     part[tid] += v;
     __syncthreads();
   }
-  long long pos = 16 + 4ll * nblocks + (tid ? part[tid - 1] : 0);
-  int bad = 0;
-  for (int b = b0; b < b1; b++) {
-    a.bstarts[b] = (int)(pos > 0x7fffffffll ? 0x7fffffffll : pos);
-    const int ns = b < a.nfull ? a.nsplits : 1;
-    const int neblock = b < a.nfull ? a.blocksize / a.nsplits : a.leftover;
-    for (int s = 0; s < ns; s++) {
-      const long long idx = b < a.nfull ? (long long)b * a.nsplits + s : (long long)a.nfull * a.nsplits;
-      const int c = a.csizes[idx];
-      if (a.serial) {
-        /* serial_blosc hands each codec call maxout = min(neblock, room left in dest) (blosc.c:646-651):
-         * a clamped call only succeeds if the stream would have fitted that smaller budget, and a
-         * raw split needs the full neblock (blosc.c:705-711) */
-        const long long room = a.destsize - (pos + 4);
-        if (room < neblock && !(room > 0 && c < neblock && a.needs[idx] <= room)) bad = 1;
-      }
-      pos += 4 + (long long)c;
-    }
-  }
-  if (bad) atomicOr(&a.result[2], 1);
+  /* the status word, zero between calls, collects the threads' give-up verdicts */
+  if (scan_place(a, b0, b1, 16 + 4ll * nblocks + (tid ? part[tid - 1] : 0))) atomicOr(&a.result[B2_R_STATUS], 1);
   __syncthreads();
   if (tid == SCAN_THREADS - 1) {
     const long long total = 16 + 4ll * nblocks + part[SCAN_THREADS - 1];
-    a.result[0] = (int)(total > 0x7fffffffll ? 0x7fffffffll : total);
-    a.result[1] = (total <= a.destsize && a.result[2] == 0) ? 1 : 0;   /* blosc.c:1848 / :836-839 give up */
-    a.result[2] = 0;
+    a.result[B2_R_CBYTES] = (int)(total > 0x7fffffffll ? 0x7fffffffll : total);
+    a.result[B2_R_FITS] = (total <= a.destsize && a.result[B2_R_STATUS] == 0) ? 1 : 0;   /* blosc.c:1848 / :836-839 give up */
+    a.result[B2_R_STATUS] = 0;
   }
 }
 
@@ -791,14 +724,9 @@ DEV void decode_streams(const DecodeArgs& a, Codec codec) {
     mine++;
     __syncwarp();
   }
-  if (mine == 0) return;
-  __threadfence();
-  int last = 0;
-  if (lane_id() == 0) last = atomicAdd(a.done, mine) + mine == a.map.nstreams;
-  last = __shfl_sync(FULLMASK, last, 0);
-  if (!last) return;
-  __threadfence();
-  if (lane_id() == 0) { *a.status_out = ld_cg_i32(a.status); *a.status = 0; *a.done = 0; }
+  streams_done(a.done, a.map.nstreams, mine, [&] {
+    if (lane_id() == 0) { *a.status_out = ld_cg_i32(a.status); *a.status = 0; }
+  });
 }
 
 #define DECODE_WARPS 4

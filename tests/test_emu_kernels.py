@@ -148,6 +148,24 @@ def test_library_error_codes(emu):
     assert decompress(emu, "blosc_decompress_ctx", c, n)[0] == -1
 
 
+def test_block_scan_of_more_than_65536_blocks(emu, orc):
+    """A chunk of more than 65536 blocks (B2_FOLD_SCAN_MAX_BLOCKS) is scanned by its own scan_kernel launch instead of
+    the encoder's last warp: the same return codes and chunks as the oracle's under serial_blosc's per-split maxout rule
+    (nthreads 1) and t_blosc's total-fit rule (nthreads 2), with room to spare and with one byte too few."""
+    n = 128 * 65536 + 4100
+    src = gen("bench", n, seed=7)
+    for nt in (1, 2):
+        fit, _ = compress(orc, "orc_compress_ctx", 1, 1, 4, src, n + 16, "blosclz", 128, nt)
+        assert 0 < fit < n + 16
+        for destsize in (n + 16, fit - 1):
+            ra, a = compress(orc, "orc_compress_ctx", 1, 1, 4, src, destsize, "blosclz", 128, nt)
+            rb, b = compress(emu, "blosc_compress_ctx", 1, 1, 4, src, destsize, "blosclz", 128, nt)
+            assert ra == rb == (fit if destsize > fit else 0), (nt, destsize, ra, rb)
+            m = max(ra, 16)
+            assert (a[:m] == b[:m]).all() and (b[m:] == 0xAA).all(), (nt, destsize)
+            assert int.from_bytes(bytes(b[8:12]), "little") == 128
+
+
 def test_lz4_decoder_paths_are_all_exercised(emu, orc):
     """The batch-parallel, single-sequence and general decode paths must all run (and agree with
     the source) on shuffled bench.c data -- guards against a fast path silently never being taken."""

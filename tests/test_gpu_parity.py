@@ -139,6 +139,23 @@ def test_maxout_semantics(pkg, cuda):
     assert _gpu_compress(pkg, 5, 1, 4, big, len(big) + 16, "lz4", 0, 300)[0] == -1
 
 
+def test_block_scan_of_more_than_65536_blocks(pkg, orc, cuda):
+    """scan_kernel, launched for chunks of more than 65536 blocks: the oracle's return codes and chunks under the serial
+    (nthreads 1) and the pool (nthreads 2) fit rules, with room to spare and with one byte too few."""
+    n = 128 * 65536 + 4100
+    src = gen("bench", n, seed=7)
+    for comp, clevel in (("blosclz", 1), ("lz4", 5)):
+        for nt in (1, 2):
+            fit, _ = compress(orc, "orc_compress_ctx", clevel, 1, 4, src, n + 16, comp, 128, nt)
+            assert 0 < fit < n + 16
+            for destsize in (n + 16, fit - 1):
+                want_n, want = compress(orc, "orc_compress_ctx", clevel, 1, 4, src, destsize, comp, 128, nt)
+                got_n, got = _gpu_compress(pkg, clevel, 1, 4, src, destsize, comp, 128, nt)
+                assert got_n == want_n == (fit if destsize > fit else 0), (comp, nt, destsize, got_n, want_n)
+                m = max(got_n, 16)
+                assert (got[:m] == want[:m]).all() and (got[m:] == 0xAA).all(), (comp, nt, destsize)
+
+
 def test_compat_golden_chunks(pkg, cuda):
     """compat/*.cdata: every chunk written by blosc 1.3.0 ... 1.18.0 with blosclz / lz4 / lz4hc
     -- and zlib / zstd, through the decode-only GPU decoders -- decodes bit-exactly to int32
