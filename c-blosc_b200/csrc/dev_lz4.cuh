@@ -204,6 +204,20 @@ DEV int lz4_count_tail(const StreamBase& sb, const u8* __restrict__ s, int p, in
   return warp_count_match(s, p, q, limit);
 }
 
+/* catch-up (lz4.c:1107-1109) of the match at ip with candidate `match`, from `back` bytes on: the length of the
+ * run of equal bytes before them, 32 per round, bounded by the anchor and by the start of the stream */
+DEV int lz4_catch_up(const u8* __restrict__ s, int ip, int match, int anchor, int back) {
+  const int lane = lane_id();
+  for (;;) {
+    const int a = ip - 1 - back - lane, b = match - 1 - back - lane;
+    const bool ok = a >= anchor && b >= 0 && s[a] == s[b];
+    const unsigned m = __ballot_sync(FULLMASK, ok);
+    const int step = m == FULLMASK ? 32 : __ffs((int)~m) - 1;
+    back += step;
+    if (step < 32) return back;
+  }
+}
+
 /* ---- team mode: one CTA of four warps per stream ------------------------------------------------
  * A lone warp spends ~6 cycles per instruction on its dependent chain (ALU latency 4, one issue
  * per 2 cycles and pipe), so on a hard byte-plane the serial LZ4 loop is bound by the NUMBER of
@@ -232,6 +246,18 @@ DEV int lz4_count_tail(const StreamBase& sb, const u8* __restrict__ s, int p, in
 #ifdef SIMT_EMU
 /* x[]: 0 LZ4T_LONG, 1 match of 270+ bytes, 2 re-base, 3 chain start on prepared tiles, 4 chained miss, 5 walker waited for a tile */
 static long long g_dbg_lz4t_sessions = 0, g_dbg_lz4t_seqs = 0, g_dbg_lz4t_stale = 0, g_dbg_lz4t_x[6];
+/* the search after a chained miss, taken from the verdicts (LZ4T_S_*) */
+enum {
+  LZ4T_S_HIT0,                             /* + k: a hit at probe k (0..3) */
+  LZ4T_S_STALE = 4,                        /* a probe's verdict was computed from another candidate: the scalar probes take over */
+  LZ4T_S_MISS4,                            /* all four probes missed: on to the 32-wide rounds */
+  LZ4T_S_LIT,                              /* a hit with literals: general emission */
+  LZ4T_S_CAPPED,                           /* a hit whose catch-up length is 7+ and more than 7 bytes from the anchor: warp catch-up */
+  LZ4T_S_LONG,                             /* a hit whose length field is LZ4T_LONG */
+  LZ4T_S_HUGE,                             /* a hit of 270+ bytes with its catch-up: general emission */
+  LZ4T_S_N
+};
+static long long g_dbg_lz4t_s[LZ4T_S_N];
 #define LZ4T_DBG(x) do { if (lane_id() == 0) (x)++; } while (0)
 #else
 #define LZ4T_DBG(x) do {} while (0)
@@ -253,6 +279,8 @@ static long long g_dbg_lz4t_sessions = 0, g_dbg_lz4t_seqs = 0, g_dbg_lz4t_stale 
 #define LZ4T_END 0xffffffffu               /* snap of a position that was not compared (too close to the end of the
                                             * stream, or the table held no earlier position): no table entry equals it */
 #define LZ4T_LONG 13                       /* match-length field: 13 = "13 or more bytes after the first four" */
+#define LZ4T_HSHIFT 19                     /* the hash (at most 13 bits) is the top of a verdict's .x */
+#define LZ4T_BACKCAP 7                     /* catch-up length field: 7 = "7 or more" */
 static_assert(LZ4T_TILES % 3 == 0 && LZ4T_AHEAD >= 1 && LZ4T_AHEAD < LZ4T_TILES && LZ4T_RING > 15 + 255 + 4, "team ring layout");
 /* a preparer pulls the bytes this far past its tile into L1 (measured on an H100, power limit 400 and 700 W, on the bench.c planes, typesize 4:
  * encode 4.17 -> 4.08 ms; 4 and 16 KiB ahead into L2 instead: 4.10 and 4.15 ms) */
@@ -292,7 +320,8 @@ __device__ unsigned long long g_lz4_cycles[LZ4C_MAXSTREAMS][LZ4C_N];
 #endif
 
 struct Lz4Team {
-  uint2 vd[LZ4T_RING];                     /* .x: bit 0 hit, bits 2..5 length field, bits 8..20 hash; .y snap */
+  uint2 vd[LZ4T_RING];                     /* .x: bit 0 hit, bits 2..5 length field, bits 8..10 catch-up length (hits
+                                            * only), bits 19..31 hash (one shift takes it out); .y snap */
   int rdy[LZ4T_TILES];                     /* ready word of each slot: number + 1 of the tile whose verdicts it holds */
   const u8* s;                             /* current stream */
   int n;
@@ -326,7 +355,7 @@ DEV void lz4_team_prepare_tile(Lz4Team* tm, const void* tabmem, const u8* s, int
   /* racing with the walker's stores (and, at a stream's start, with its clearing of the table) is fine:
    * the walker takes the verdict only if the live entry still equals snap */
   const int snap = U16 ? (int)((const volatile u16*)tabmem)[h] : (int)((const volatile u32*)tabmem)[h];
-  u32 vx = h << 8, sn = LZ4T_END;
+  u32 vx = h << LZ4T_HSHIFT, sn = LZ4T_END;
   if ((unsigned)snap < (unsigned)p) {                  /* always true for entries the serial code could see here */
     LZ4C_T(c_t1);
     LZ4C_ADD(LZ4C_PREP_OWN, c_t1 - c_t0);
@@ -338,7 +367,21 @@ DEV void lz4_team_prepare_tile(Lz4Team* tm, const void* tabmem, const u8* s, int
     else if (x3) m = 8u + ((u32)(__ffs((int)x3) - 1) >> 3);
     else m = a4 != c4 ? 12u : (u32)LZ4T_LONG;
     const bool hit = (U16 || snap + 65535 >= p) && c0 == a0;
-    vx |= (hit ? 1u : 0u) | (m << 2);
+    /* catch-up length (lz4.c:1107-1109 without the anchor bound, which only the walker knows): equal bytes
+     * before p and before snap, at most 7 ("7 or more"), never reaching before the start of the stream */
+    u32 bk = 0;
+    if (hit) {
+      if (snap >= 8) {                                 /* p > snap: both windows lie inside the stream */
+        u32 p0, p1, q0, q1;
+        ldp_win8(sb, p - 8, p0, p1);
+        ldp_win8(sb, snap - 8, q0, q1);
+        const u32 y1 = p1 ^ q1, z0 = (u32)__clz((int)(p0 ^ q0)) >> 3;   /* equal bytes at the top of each word */
+        bk = y1 ? (u32)__clz((int)y1) >> 3 : 4u + (z0 < 3u ? z0 : 3u);
+      } else {
+        while (bk < (u32)snap && s[p - 1 - (int)bk] == s[snap - 1 - (int)bk]) bk++;
+      }
+    }
+    vx |= (hit ? 1u : 0u) | (m << 2) | (bk << 8);
     sn = (u32)snap;
     LZ4C_SPAN(LZ4C_PREP_GATHER, c_t1);
   }
@@ -392,6 +435,69 @@ DEV void lz4t_reach(Lz4Team* tm, int ip, int& wt, int& vt) {
     }
   }
   if (hi > vt) vt = hi;
+}
+
+/* walker, after a chained miss at `anchor`: the first LZ4_SCALAR_PROBES probes of the search (lz4.c:1043-1101), which
+ * starts at anchor + 1, taken from the verdicts.  A probe gets table[h(pos)], puts pos and tests the candidate exactly as
+ * the chained step does (without its store at ip-2), so a verdict whose snap equals the live entry is exact here too.
+ * Most breaks of a shuffled byte-plane end in one more literal-free 3- or 4-byte sequence a probe or two later; such a
+ * sequence is the chained hit at the anchor with candidate snap - back (same offset, length back + m), so it is handed
+ * back to the chain as that verdict.  Returns true then (pk, snap, ip = anchor).  Otherwise returns false with either
+ *   hit false: ip = anchor + 1 and lit = the first probe the scalar code still has to make (a stale verdict, the end
+ *              of the stream, or all four probes missed: LZ4_SCALAR_PROBES, on to the 32-wide rounds), or
+ *   hit true:  literals, a catch-up of more than 7 bytes or a match of 270+ bytes; ip, match, back, lit and the length
+ *              after the first four (have_mc, mc_carry) as the general emission takes them.
+ * Team mode has no PACK table. */
+template <bool U16>
+DEV bool lz4t_search(Lz4Team* tm, smem_addr_t vda, void* tabmem, const StreamBase& sb, int n, int anchor, int accel,
+                     int& twt, int& tvt, u32& pk, u32& snap, int& ip, bool& hit, int& match, int& back, int& lit,
+                     bool& have_mc, int& mc_carry) {
+  u16* tab16 = (u16*)tabmem;
+  u32* tab32 = (u32*)tabmem;
+  const int mfl1 = n - LZ4_MFLIMIT + 1;
+  ip = anchor + 1;
+  int it = 0, pos = ip;
+  for (;; it++) {
+    if (it == LZ4_SCALAR_PROBES) { LZ4T_DBG(g_dbg_lz4t_s[LZ4T_S_MISS4]); lit = it; return false; }
+    pos = ip + (it ? 1 + (it - 1) * accel : 0);                    /* lz4.c:1043-1053 */
+    if (ip + 1 + it * accel > mfl1) { lit = it; return false; }    /* the scalar loop ends the stream (lz4.c:1055) */
+    if ((pos >> 5) > tvt) lz4t_reach(tm, pos, twt, tvt);          /* publishes the tile of pos-2: nothing later reads below it */
+    u32 qk, qs;
+    smem_ld_u32x2(vda, ((u32)pos % (u32)LZ4T_RING) << 3, qk, qs);
+    const u32 h = qk >> LZ4T_HSHIFT;
+    const int cand = U16 ? (int)tab16[h] : (int)tab32[h];
+    __syncwarp();                                                  /* every lane has read the entry before any overwrites it */
+    if (cand != (int)qs) { LZ4T_DBG(g_dbg_lz4t_s[LZ4T_S_STALE]); lit = it; return false; }
+    if (U16) tab16[h] = (u16)pos; else tab32[h] = (u32)pos;
+    if (qk & 1u) { pk = qk; snap = qs; break; }
+  }
+  LZ4T_DBG(g_dbg_lz4t_s[LZ4T_S_HIT0 + it]);
+  const int vb = (int)((pk >> 8) & 7u), dist = pos - anchor;       /* catch-up length, cut at the anchor below */
+  const int bq = vb < dist ? vb : dist;
+  int m = (int)((pk >> 2) & 15u);
+  if (m == LZ4T_LONG) {
+    LZ4T_DBG(g_dbg_lz4t_s[LZ4T_S_LONG]);
+    m = LZ4T_LONG + lz4_count_tail(sb, sb.s, pos + 4 + LZ4T_LONG, (int)snap + 4 + LZ4T_LONG, n - LZ4_LASTLITERALS, n);
+  }
+  if (bq == dist && bq + m < 15 + 255) {                           /* no literals (a capped catch-up has bq = 7 < dist) */
+    const int mc = bq + m;
+    snap -= (u32)bq;
+    pk = 1u | ((u32)(mc < LZ4T_LONG ? mc : LZ4T_LONG) << 2);         /* from LZ4T_LONG on the chain counts again from the anchor */
+    ip = anchor;
+    LZ4C_ADD(LZ4C_SEQS, 1);
+    LZ4C_ADD(LZ4C_CHAIN_SEQS, ~0ull);                              /* the chain counts it as its own: moved to SEQS */
+    return true;
+  }
+  hit = true; ip = pos; match = (int)snap;                         /* imm stays false: the general path checks the limits */
+  have_mc = true; mc_carry = m;
+  back = bq;
+  if (vb == LZ4T_BACKCAP && dist > LZ4T_BACKCAP) {                 /* 7 or more: the rest of the catch-up (lz4.c:1107-1109) */
+    LZ4T_DBG(g_dbg_lz4t_s[LZ4T_S_CAPPED]);
+    back = lz4_catch_up(sb.s, pos, (int)snap, anchor, LZ4T_BACKCAP);
+  } else if (bq != dist) LZ4T_DBG(g_dbg_lz4t_s[LZ4T_S_LIT]);
+  else LZ4T_DBG(g_dbg_lz4t_s[LZ4T_S_HUGE]);
+  lit = pos - back - anchor;
+  return false;
 }
 
 /* Returns the compressed size, or 0 when the stream does not fit in `cap`
@@ -479,8 +585,8 @@ DEV int lz4_encode_stream(const u8* __restrict__ s, const int n, u8* __restrict_
         for (;;) {
           u32 pk, snap;
           smem_ld_u32x2(vda, e << 3, pk, snap);
-          const u32 h2 = smem_ld_u32(vda, (e >= 2u ? e - 2u : e - 2u + LZ4T_RING) << 3) >> 8;
-          const u32 h = pk >> 8;
+          const u32 h2 = smem_ld_u32(vda, (e >= 2u ? e - 2u : e - 2u + LZ4T_RING) << 3) >> LZ4T_HSHIFT;
+          const u32 h = pk >> LZ4T_HSHIFT;
           LZ4_TPUT(h2, ip - 2);                                            /* every lane the same word: no hand-off between lanes */
           const int cand = LZ4_TGET(h);
           __syncwarp();                                                    /* every lane has read the entry before any overwrites it */
@@ -489,7 +595,16 @@ DEV int lz4_encode_stream(const u8* __restrict__ s, const int n, u8* __restrict_
             scalar_post = true; break;                                     /* the plain probe below looks this one up itself */
           }
           LZ4_TPUT(h, ip);                                                 /* lz4.c:1291: ip goes into the table, hit or not */
-          if (!(pk & 1u)) { LZ4T_DBG(g_dbg_lz4t_x[4]); ip++; break; }                                 /* lz4.c:1298; on to the search below */
+          if (!(pk & 1u)) {                                                /* lz4.c:1298, then the search */
+            LZ4T_DBG(g_dbg_lz4t_x[4]);
+            if constexpr (TEAM) {                                          /* (not instantiated for encode_kernel, whose code stays as it was) */
+              if (!lz4t_search<U16>(tm, vda, tabmem, sb, n, anchor, accel, twt, tvt, pk, snap, ip, hit, match, back, lit, have_mc, mc_carry))
+                break;                                                     /* on to the search or the emission below */
+              /* its probes may have moved tvt past the tile of ip without the check below: with this one, at most
+               * 24 records are parked here and at most 8 more start in the rest of the tile before the next check */
+              if (nrec >= 24) LZ4_FLUSH_CHECKED();
+            } else { ip++; break; }
+          }
           const int off = ip - (int)snap;
           int mc = (int)((pk >> 2) & 15u);
           if (mc == LZ4T_LONG) {
@@ -632,7 +747,7 @@ DEV int lz4_encode_stream(const u8* __restrict__ s, const int n, u8* __restrict_
         /* ---- find a match (lz4.c:1043-1101): two scalar probes, then 32-wide rounds ---- */
         LZ4C_TW(c_f);
         bool ended = false;
-        for (int it = 0; it < LZ4_SCALAR_PROBES; it++) {
+        for (int it = TEAM ? lit : 0; it < LZ4_SCALAR_PROBES; it++) {   /* TEAM: lit = first probe lz4t_search left */
           const int pos = ip + (it ? 1 + (it - 1) * accel : 0);            /* probe offsets 0, 1, 1+accel, 1+2*accel (lz4.c:1043-1053) */
           if (ip + 1 + it * accel > mfl1) { ended = true; break; }         /* `goto _last_literals` (lz4.c:1055) */
           u32 b0, b1 = 0, b2 = 0;
@@ -693,16 +808,7 @@ DEV int lz4_encode_stream(const u8* __restrict__ s, const int n, u8* __restrict_
         if (!hit) { if (TEAM) LZ4C_SPAN(LZ4C_SEARCH, c_f); break; }  /* -> last literals */
 
         /* ---- catch up (lz4.c:1107-1109) ---- */
-        if (ip > anchor && match > 0 && s[ip - 1] == s[match - 1]) {
-          for (;;) {
-            const int a = ip - 1 - back - lane, b = match - 1 - back - lane;
-            const bool ok = a >= anchor && b >= 0 && s[a] == s[b];
-            const unsigned m = __ballot_sync(FULLMASK, ok);
-            const int step = m == FULLMASK ? 32 : __ffs((int)~m) - 1;
-            back += step;
-            if (step < 32) break;
-          }
-        }
+        if (ip > anchor && match > 0 && s[ip - 1] == s[match - 1]) back = lz4_catch_up(s, ip, match, anchor, 0);
         lit = ip - back - anchor;
         if (TEAM) LZ4C_SPAN(LZ4C_SEARCH, c_f);
       }
@@ -816,6 +922,7 @@ DEV void lz4t_begin(Lz4Team* tm, const u8* s, int n, bool u16) {
   bar_arrive(LZ4T_BAR_GO(0), 64); bar_arrive(LZ4T_BAR_GO(1), 64); bar_arrive(LZ4T_BAR_GO(2), 64);
 }
 DEV void lz4t_end(Lz4Team* tm) {
+  __syncwarp();                            /* every lane's last store of `wt` (lz4t_reach) lands before LZ4T_STOP */
   if (lane_id() == 0) lz4t_st_i32(&tm->wt, LZ4T_STOP);
   __syncwarp();
   bar_sync(LZ4T_BAR_IDLE(0), 64); bar_sync(LZ4T_BAR_IDLE(1), 64); bar_sync(LZ4T_BAR_IDLE(2), 64);

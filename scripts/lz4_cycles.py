@@ -9,10 +9,11 @@ given with --lib), compresses the buffer in team mode (one warm-up call, then th
 prints, per split of a block, the streams' sequence counts and clock64() cycles, then the phase
 breakdown of the hard streams (more than 1000 sequences) per sequence.  Phases (dev_lz4.cuh, LZ4C_*):
   start    chain start: publishing the walker's tile until the chain's first tiles are ready
-  chain    the walker's own work in a chain (chain time minus its tile waits)
+  chain    the walker's own work in a chain (chain time minus its tile waits), including the first four probes
+           of the search after a chained miss, which the walker takes from the verdicts
   fullwait the walker waiting for the ready word of a tile inside a chain
   reprobe  stale verdicts and post-match probes done by the scalar code
-  search   the search after a chain break (scalar probes, 32-wide rounds, catch-up)
+  search   the rest of a search the chain left (scalar probes, 32-wide rounds, catch-up)
   other    the rest of the call (emission of searched sequences, table init, last literals)
 and, for the preparers, the cycles per tile from being allowed to prepare it to posting its ready word,
 split into the load of the tile's own bytes (with hash and table read) and the candidate gather (with
