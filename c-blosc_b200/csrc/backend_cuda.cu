@@ -217,11 +217,11 @@ static int team_wanted(const EncodeArgs* a) {
 }
 
 #ifdef B2_LZ4_CYCLES
-/* the team encoder's per-stream cycle counters (dev_lz4.cuh, LZ4C_*): LZ4C_MAXSTREAMS x LZ4C_N u64 */
+/* the team encoder's per-stream cycle counters (dev_lz4.cuh, LZ4C_*): LZ4C_MAXSTREAMS x LZ4C_NREC u64 */
 extern "C" int b2_lz4_cycles_read(unsigned long long* dst, int nstreams) {
   if (nstreams > LZ4C_MAXSTREAMS) nstreams = LZ4C_MAXSTREAMS;
   CK(cudaDeviceSynchronize());
-  CK(cudaMemcpyFromSymbol(dst, g_lz4_cycles, (size_t)nstreams * LZ4C_N * sizeof(unsigned long long)));
+  CK(cudaMemcpyFromSymbol(dst, g_lz4_cycles, (size_t)nstreams * LZ4C_NREC * sizeof(unsigned long long)));
   return nstreams;
 }
 #endif

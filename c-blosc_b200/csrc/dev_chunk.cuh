@@ -240,7 +240,7 @@ __global__ void __launch_bounds__(TEAM_WARPS * 32, TEAM_CTAS_PER_SM) encode_team
 #endif
   if (threadIdx.x == 0) { tm->cmd = 0; tm->gen = 0; }
 #ifdef B2_LZ4_CYCLES
-  if (threadIdx.x < LZ4C_N) tm->cyc[threadIdx.x] = 0;
+  if (threadIdx.x < LZ4C_NREC) tm->cyc[threadIdx.x] = 0;
 #endif
   __syncthreads();
 #ifndef SIMT_EMU
@@ -259,10 +259,10 @@ __global__ void __launch_bounds__(TEAM_WARPS * 32, TEAM_CTAS_PER_SM) encode_team
       asm volatile("mov.u32 %0, %%warpid;" : "=r"(wid));
       __syncwarp();
       const int k = lane_id();
-      if (idx < LZ4C_MAXSTREAMS && k < LZ4C_N)
+      if (idx < LZ4C_MAXSTREAMS && k < LZ4C_NREC)
         g_lz4_cycles[idx][k] = k == LZ4C_TOTAL ? total : k == LZ4C_SMID ? smid : k == LZ4C_SUBP ? (wid & 3u) : tm->cyc[k];
       __syncwarp();
-      if (k < LZ4C_N) tm->cyc[k] = 0;
+      if (k < LZ4C_NREC) tm->cyc[k] = 0;
     }
 #endif
     return c;

@@ -258,9 +258,26 @@ enum {
   LZ4T_S_N
 };
 static long long g_dbg_lz4t_s[LZ4T_S_N];
+/* the chained windows (LZ4T_W_*): how many, how many elements they committed, and what ended them */
+enum {
+  LZ4T_W_WINDOWS,
+  LZ4T_W_ELEMS,                            /* elements committed (valid, stores made), summed over the windows */
+  LZ4T_W_STALE0, LZ4T_W_STALEJ,            /* the first invalid element was element 0 / a later one */
+  LZ4T_W_FWD,                              /* an element's lookup was answered by an earlier store of the same window */
+  LZ4T_W_CROSS,                            /* h(q_j - 2) == h(q_k) for two different elements j, k of a window */
+  LZ4T_W_MISS0, LZ4T_W_MISSJ,              /* a valid miss ended the window at element 0 / a later one */
+  LZ4T_W_LONG0, LZ4T_W_LONGJ,              /* a valid LZ4T_LONG ended the window at element 0 / a later one */
+  LZ4T_W_HUGE,                             /* ... and its match was 270+ bytes: general emission */
+  LZ4T_W_END, LZ4T_W_CAP, LZ4T_W_TILE,     /* the next position is too close to the end / the window is full / past vt */
+  LZ4T_W_FULL,                             /* the flush before a window found the output too small */
+  LZ4T_W_N
+};
+static long long g_dbg_lz4t_w[LZ4T_W_N];
 #define LZ4T_DBG(x) do { if (lane_id() == 0) (x)++; } while (0)
+#define LZ4T_DBGN(x, v) do { if (lane_id() == 0) (x) += (v); } while (0)
 #else
 #define LZ4T_DBG(x) do {} while (0)
+#define LZ4T_DBGN(x, v) do {} while (0)
 #endif
 #ifndef LZ4T_TILES
 #define LZ4T_TILES 12                      /* ring slots of 32 positions; a multiple of 3 (one owner per slot) */
@@ -281,7 +298,9 @@ static long long g_dbg_lz4t_s[LZ4T_S_N];
 #define LZ4T_LONG 13                       /* match-length field: 13 = "13 or more bytes after the first four" */
 #define LZ4T_HSHIFT 19                     /* the hash (at most 13 bits) is the top of a verdict's .x */
 #define LZ4T_BACKCAP 7                     /* catch-up length field: 7 = "7 or more" */
+#define LZ4T_W 16                          /* chained sequences the walker takes per window: two table stores each, one per lane */
 static_assert(LZ4T_TILES % 3 == 0 && LZ4T_AHEAD >= 1 && LZ4T_AHEAD < LZ4T_TILES && LZ4T_RING > 15 + 255 + 4, "team ring layout");
+static_assert(2 * LZ4T_W <= 32, "window layout");
 /* a preparer pulls the bytes this far past its tile into L1 (measured on an H100, power limit 400 and 700 W, on the bench.c planes, typesize 4:
  * encode 4.17 -> 4.08 ms; 4 and 16 KiB ahead into L2 instead: 4.10 and 4.15 ms) */
 #define LZ4T_PREFETCH 512
@@ -305,9 +324,15 @@ enum {
   LZ4C_STALE,        /* chained positions whose verdict's snap differed from the live table */
   LZ4C_N = 16
 };
+/* the chained windows and what ended each: a stale element, a valid miss or LZ4T_LONG, the end of the stream,
+ * LZ4T_W elements, the next position past the checked tiles */
+enum {
+  LZ4C_WINDOWS = LZ4C_N, LZ4C_W_STALE, LZ4C_W_MISS, LZ4C_W_LONG, LZ4C_W_END, LZ4C_W_CAP, LZ4C_W_TILE,
+  LZ4C_NREC                                /* columns of a stream's record */
+};
 #ifdef B2_LZ4_CYCLES
 #define LZ4C_MAXSTREAMS 16384
-__device__ unsigned long long g_lz4_cycles[LZ4C_MAXSTREAMS][LZ4C_N];
+__device__ unsigned long long g_lz4_cycles[LZ4C_MAXSTREAMS][LZ4C_NREC];
 #define LZ4C_T(t) const long long t = clock64()
 #define LZ4C_TW(t) const long long t = TEAM ? clock64() : 0ll     /* in code that encode_kernel shares */
 #define LZ4C_ADD(k, v) do { if (lane_id() == 0) atomicAdd(&tm->cyc[k], (unsigned long long)(v)); } while (0)
@@ -331,8 +356,9 @@ struct Lz4Team {
   int cmd;                                 /* LZ4T_QUIT ends the preparers */
   int sub[4];                              /* SM sub-partition of each warp of the CTA */
   int slot;                                /* sub-partition this CTA's walker should run on */
+  u32 seen[8192 / 32];                     /* walker: hashes of the stores of the window being checked, one bit each (zero between windows) */
 #ifdef B2_LZ4_CYCLES
-  unsigned long long cyc[LZ4C_N];
+  unsigned long long cyc[LZ4C_NREC];
 #endif
 };
 #define LZ4T_SMEM_BYTES ((int)sizeof(Lz4Team))
@@ -435,6 +461,14 @@ DEV void lz4t_reach(Lz4Team* tm, int ip, int& wt, int& vt) {
     }
   }
   if (hi > vt) vt = hi;
+}
+
+/* walker: moves vt over the tiles after it whose ready words are posted already, without waiting, up to
+ * wt + LZ4T_AHEAD (a preparer only reuses the slot of a tile below wt) */
+DEV void lz4t_extend(Lz4Team* tm, int wt, int& vt) {
+  const int t = vt + 1 + lane_id();
+  const bool ready = t <= wt + LZ4T_AHEAD && lz4t_ld_i32(&tm->rdy[t % LZ4T_TILES]) == t + 1;
+  vt += __ffs((int)~__ballot_sync(FULLMASK, ready)) - 1;
 }
 
 /* walker, after a chained miss at `anchor`: the first LZ4_SCALAR_PROBES probes of the search (lz4.c:1043-1101), which
@@ -566,12 +600,21 @@ DEV int lz4_encode_stream(const u8* __restrict__ s, const int n, u8* __restrict_
       int mc_carry = 0;
 
       bool scalar_post = post;
-      if (TEAM && post && ip + 64 <= n) {
+      if constexpr (TEAM) if (post && ip + 64 <= n) {   /* (not instantiated for encode_kernel) */
         /* ---- chained "test next position" (lz4.c:1236-1294) with the verdicts prepared by the helper
-         * warps (see "team mode" above) ---- */
+         * warps (see "team mode" above), a window of up to LZ4T_W sequences per step:
+         * 1. path: hop from q_0 = ip along the verdicts, q_{j+1} = q_j + 4 + length field; a miss or an LZ4T_LONG is
+         *    the window's last element, and the hop stops before a position whose tile is past tvt, that is too close
+         *    to the end of the stream, or when the window is full.
+         * 2. check: the serial code would store S_2j = (h(q_j - 2), q_j - 2) and S_2j+1 = (h(q_j), q_j), and element
+         *    j reads table[h(q_j)] after S_2j.  Lane m takes S_m; that read is the position of the highest lower lane
+         *    with the same hash, or else the live entry (read before any store of the window).  Element j is exact
+         *    when it equals the verdict's snap, so the elements before the first one that is not are exactly what as
+         *    many serial iterations would have done.
+         * 3. commit: their stores (per hash the last one in serial order) and their 3-byte records.
+         * The element that ends the window goes to the code that handled it one sequence at a time. ---- */
         scalar_post = false;
         bool finished = false;
-        if (nrec >= 24) LZ4_FLUSH_CHECKED();
         LZ4T_DBG(g_dbg_lz4t_sessions);
         LZ4C_T(c_s0);
         LZ4C_ADD(LZ4C_SESSIONS, 1);
@@ -582,66 +625,146 @@ DEV int lz4_encode_stream(const u8* __restrict__ s, const int n, u8* __restrict_
         LZ4C_T(c_s1);
         const smem_addr_t vda = smem_addr(tm->vd);
         u32 e = (u32)ip % (u32)LZ4T_RING;     /* ring entry of ip: slot (ip >> 5) mod LZ4T_TILES, lane ip & 31 */
+        bool given = false;                   /* element 0 is lz4t_search's hit at ip: checked and stored already */
+        u32 gpk = 0, gsnap = 0;
         for (;;) {
-          u32 pk, snap;
-          smem_ld_u32x2(vda, e << 3, pk, snap);
-          const u32 h2 = smem_ld_u32(vda, (e >= 2u ? e - 2u : e - 2u + LZ4T_RING) << 3) >> LZ4T_HSHIFT;
-          const u32 h = pk >> LZ4T_HSHIFT;
-          LZ4_TPUT(h2, ip - 2);                                            /* every lane the same word: no hand-off between lanes */
-          const int cand = LZ4_TGET(h);
-          __syncwarp();                                                    /* every lane has read the entry before any overwrites it */
-          if (cand != (int)snap) {                                         /* the verdict was computed from another candidate */
-            LZ4T_DBG(g_dbg_lz4t_stale); LZ4C_ADD(LZ4C_STALE, 1);
+          /* a window parks at most LZ4T_W records; op only grows inside a chain, so one limitedOutput check per
+           * parked batch, before anything is written, is exact (LZ4_FLUSH_CHECKED) */
+          if (nrec > 32 - LZ4T_W) {
+#ifdef SIMT_EMU
+            if (limited && op + 1 + LZ4_LASTLITERALS > olimit) LZ4T_DBG(g_dbg_lz4t_w[LZ4T_W_FULL]);
+#endif
+            LZ4_FLUSH_CHECKED();
+          }
+          lz4t_extend(tm, twt, tvt);
+          /* 1. path; lane j keeps element j (position, ring entry, verdict) */
+          int cnt = 0, q = ip, why;
+          u32 ee = e, pk, snap;
+          if (given) { pk = gpk; snap = gsnap; } else smem_ld_u32x2(vda, ee << 3, pk, snap);
+          int jq = 0;
+          u32 je = 0, jpk = 0, jsnap = 0;
+          for (;;) {
+            if (lane == cnt) { jq = q; je = ee; jpk = pk; jsnap = snap; }
+            cnt++;
+            const u32 step = ((pk >> 2) & 15u) + 4u;
+            u32 en = ee + step;
+            if (en >= (u32)LZ4T_RING) en -= (u32)LZ4T_RING;
+            u32 npk, nsnap;
+            smem_ld_u32x2(vda, en << 3, npk, nsnap);                       /* ahead of the tests: en is inside the ring */
+            if (!(pk & 1u)) { why = LZ4C_W_MISS; break; }
+            if (step == LZ4T_LONG + 4u) { why = LZ4C_W_LONG; break; }
+            q += (int)step; ee = en;
+            if (cnt == LZ4T_W) { why = LZ4C_W_CAP; break; }
+            if (q + 64 > n) { why = LZ4C_W_END; break; }
+            if ((q >> 5) > tvt) { why = LZ4C_W_TILE; break; }
+            pk = npk; snap = nsnap;
+          }
+          /* 2. check: lane m holds S_m */
+          u32 jh2 = 0;
+          if (lane < cnt) jh2 = smem_ld_u32(vda, (je >= 2u ? je - 2u : je - 2u + LZ4T_RING) << 3) >> LZ4T_HSHIFT;
+          const int el = lane >> 1;
+          const bool odd = (lane & 1) != 0;
+          const u32 sh2 = __shfl_sync(FULLMASK, jh2, el), sh = __shfl_sync(FULLMASK, jpk >> LZ4T_HSHIFT, el);
+          const int sq = __shfl_sync(FULLMASK, jq, el);
+          const u32 ssnap = __shfl_sync(FULLMASK, jsnap, el);
+          const bool act = lane < 2 * cnt && !(given && lane < 2);
+          const u32 skey = odd ? sh : sh2;
+          const int spos = odd ? sq : sq - 2;
+          /* the live entries, and whether two stores of the window share a hash: one bit per hash, set with an atomic */
+          int look = 0;
+          bool dup = false;
+          if (act) {
+            if (odd) look = LZ4_TGET(skey);
+            const u32 bit = 1u << (skey & 31u);
+            dup = (atomicOr(&tm->seen[skey >> 5], bit) & bit) != 0;
+          }
+          unsigned peers = 1u << lane;                                     /* lanes with my hash: mine alone, unless ... */
+          if (__ballot_sync(FULLMASK, dup)) {                              /* (rare) a hash is shared: the nearest lower lane forwards its position */
+            peers = __match_any_sync(FULLMASK, act ? skey : 0x80000000u | (u32)lane);   /* hashes have 13 bits */
+            const unsigned lower = peers & ((1u << lane) - 1u);
+            const int fpos = __shfl_sync(FULLMASK, spos, lower ? 31 - __clz((int)lower) : lane);
+            if (act && odd && lower) look = fpos;
+#ifdef SIMT_EMU
+            const unsigned fwd = __ballot_sync(FULLMASK, act && odd && lower != 0);
+            const unsigned cross = __ballot_sync(FULLMASK, act && !odd && ((peers & 0xaaaaaaaau) & ~(2u << lane)) != 0);
+            if (fwd) LZ4T_DBG(g_dbg_lz4t_w[LZ4T_W_FWD]);
+            if (cross) LZ4T_DBG(g_dbg_lz4t_w[LZ4T_W_CROSS]);
+#endif
+          }
+          const unsigned bad = __ballot_sync(FULLMASK, act && odd && look != (int)ssnap);
+          const int nv = bad ? (__ffs((int)bad) - 1) >> 1 : cnt;           /* valid elements: a prefix */
+          LZ4T_DBG(g_dbg_lz4t_w[LZ4T_W_WINDOWS]);
+          LZ4T_DBGN(g_dbg_lz4t_w[LZ4T_W_ELEMS], nv);
+          __syncwarp();                                                    /* every lane has read the table before any store */
+          /* 3. commit */
+          const unsigned le = nv >= 16 ? FULLMASK : (1u << (2 * nv)) - 1u;
+          if (act && lane < 2 * nv && (((peers & le) >> lane) >> 1) == 0) LZ4_TPUT(skey, spos);
+          if (act) tm->seen[skey >> 5] = 0u;
+          __syncwarp();
+          const int nb = nv < cnt || why == LZ4C_W_MISS || why == LZ4C_W_LONG ? (nv < cnt ? nv : cnt - 1) : cnt;
+          const u32 rv = (u32)((jpk >> 2) & 15u) | ((u32)(jq - (int)jsnap) << 8);   /* lz4.c:1187-1226 with 0 literals, 4..16 bytes */
+          const u32 rmine = __shfl_sync(FULLMASK, rv, (lane - nrec) & 31);
+          if (lane >= nrec && lane < nrec + nb) { rec = rmine; recop = op + 3 * (lane - nrec); }
+          nrec += nb;
+          op += 3 * nb;
+          LZ4T_DBGN(g_dbg_lz4t_seqs, nb);
+          LZ4C_ADD(LZ4C_CHAIN_SEQS, nb);
+          LZ4C_ADD(LZ4C_WINDOWS, 1);
+          if (nb < cnt) {                                                  /* the element that ends the window */
+            ip = __shfl_sync(FULLMASK, jq, nb);
+            e = __shfl_sync(FULLMASK, je, nb);
+            snap = __shfl_sync(FULLMASK, jsnap, nb);
+          } else { ip = q; e = ee; }
+          anchor = ip;
+          given = false;
+          if (nv < cnt) {                                                  /* its verdict was computed from another candidate */
+            LZ4T_DBG(g_dbg_lz4t_stale); LZ4C_ADD(LZ4C_STALE, 1); LZ4C_ADD(LZ4C_W_STALE, 1);
+            LZ4T_DBG(g_dbg_lz4t_w[nv ? LZ4T_W_STALEJ : LZ4T_W_STALE0]);
             scalar_post = true; break;                                     /* the plain probe below looks this one up itself */
           }
-          LZ4_TPUT(h, ip);                                                 /* lz4.c:1291: ip goes into the table, hit or not */
-          if (!(pk & 1u)) {                                                /* lz4.c:1298, then the search */
+          LZ4C_ADD(why, 1);
+          if (why == LZ4C_W_MISS) {                                        /* lz4.c:1298, then the search */
             LZ4T_DBG(g_dbg_lz4t_x[4]);
-            if constexpr (TEAM) {                                          /* (not instantiated for encode_kernel, whose code stays as it was) */
-              if (!lz4t_search<U16>(tm, vda, tabmem, sb, n, anchor, accel, twt, tvt, pk, snap, ip, hit, match, back, lit, have_mc, mc_carry))
-                break;                                                     /* on to the search or the emission below */
-              /* its probes may have moved tvt past the tile of ip without the check below: with this one, at most
-               * 24 records are parked here and at most 8 more start in the rest of the tile before the next check */
-              if (nrec >= 24) LZ4_FLUSH_CHECKED();
-            } else { ip++; break; }
+            LZ4T_DBG(g_dbg_lz4t_w[nb ? LZ4T_W_MISSJ : LZ4T_W_MISS0]);
+            if (!lz4t_search<U16>(tm, vda, tabmem, sb, n, anchor, accel, twt, tvt, gpk, gsnap, ip, hit, match, back, lit, have_mc, mc_carry))
+              break;                                                       /* on to the search or the emission below */
+            given = true;                                                  /* a literal-free hit at ip = anchor: element 0 of the next window */
+            continue;
           }
-          const int off = ip - (int)snap;
-          int mc = (int)((pk >> 2) & 15u);
-          if (mc == LZ4T_LONG) {
+          if (why == LZ4C_W_LONG) {
             LZ4T_DBG(g_dbg_lz4t_x[0]);
-            mc = LZ4T_LONG + lz4_count_tail(sb, s, ip + 4 + LZ4T_LONG, ip - off + 4 + LZ4T_LONG, matchlimit, n);   /* ip+64 <= n: far from matchlimit */
+            LZ4T_DBG(g_dbg_lz4t_w[nb ? LZ4T_W_LONGJ : LZ4T_W_LONG0]);
+            const int off = ip - (int)snap;
+            const int mc = LZ4T_LONG + lz4_count_tail(sb, s, ip + 4 + LZ4T_LONG, ip - off + 4 + LZ4T_LONG, matchlimit, n);   /* ip+64 <= n: far from matchlimit */
             if (mc >= 15 + 255) {                                          /* very long match: general emission below */
               hit = true; imm = true; match = ip - off;
               have_mc = true; mc_carry = mc;
               LZ4T_DBG(g_dbg_lz4t_x[1]);
+              LZ4T_DBG(g_dbg_lz4t_w[LZ4T_W_HUGE]);
               break;
             }
-          }
-          /* lz4.c:1187-1226 with 0 literals: token, offset and -- from 19 bytes on -- one length byte.
-           * Both limitedOutput checks of such a sequence ask for (op after it) + 6 <= olimit; op only
-           * grows inside a chain, so the check is made once per parked batch, before anything is
-           * written (LZ4_FLUSH_CHECKED) */
-          const bool ext = mc >= 15;
-          LZ4T_DBG(g_dbg_lz4t_seqs);
-          LZ4C_ADD(LZ4C_CHAIN_SEQS, 1);
-          if (lane == nrec) { rec = (ext ? 15u | ((u32)(mc - 15) << 24) : (u32)mc) | ((u32)off << 8); recop = op; }
-          nrec++;
-          op += ext ? 4 : 3;
-          ip += mc + 4;
-          e += (u32)(mc + 4);                                              /* mc + 4 < 15 + 255 + 4 < LZ4T_RING */
-          if (e >= (u32)LZ4T_RING) e -= (u32)LZ4T_RING;
-          anchor = ip;
+            /* token, offset and -- from 19 bytes on -- one length byte (at most 31 records are parked here) */
+            const bool ext = mc >= 15;
+            LZ4T_DBG(g_dbg_lz4t_seqs);
+            LZ4C_ADD(LZ4C_CHAIN_SEQS, 1);
+            if (lane == nrec) { rec = (ext ? 15u | ((u32)(mc - 15) << 24) : (u32)mc) | ((u32)off << 8); recop = op; }
+            nrec++;
+            op += ext ? 4 : 3;
+            ip += mc + 4;
+            e += (u32)(mc + 4);                                            /* mc + 4 < 15 + 255 + 4 < LZ4T_RING */
+            if (e >= (u32)LZ4T_RING) e -= (u32)LZ4T_RING;
+            anchor = ip;
+          } else if (why == LZ4C_W_CAP) LZ4T_DBG(g_dbg_lz4t_w[LZ4T_W_CAP]);
+          else if (why == LZ4C_W_TILE) LZ4T_DBG(g_dbg_lz4t_w[LZ4T_W_TILE]);
           if (ip + 64 > n) {                                               /* a match ended close to the end of the stream */
+            if (why == LZ4C_W_END) LZ4T_DBG(g_dbg_lz4t_w[LZ4T_W_END]);
             if (ip >= mfl1) finished = true;                               /* lz4.c:1230-1233 */
             else scalar_post = true;                                       /* the plain probe below takes over */
             break;
           }
-          if ((ip >> 5) > tvt) {                                           /* on to a tile not checked yet */
-            LZ4C_T(c_w);
-            lz4t_reach(tm, ip, twt, tvt);
-            LZ4C_SPAN(LZ4C_FULLWAIT, c_w);
-            if (nrec >= 24) LZ4_FLUSH_CHECKED();                           /* at most 8 sequences start inside one tile */
-          }
+          LZ4C_T(c_w);
+          lz4t_reach(tm, ip, twt, tvt);                                    /* publishes the tile of ip - 2, waits for that of ip */
+          LZ4C_SPAN(LZ4C_FULLWAIT, c_w);
         }
         LZ4C_SPAN(LZ4C_SESSION, c_s1);
         if (finished) break;
@@ -916,6 +1039,7 @@ DEV int lz4_encode_stream(const u8* __restrict__ s, const int n, u8* __restrict_
 DEV void lz4t_begin(Lz4Team* tm, const u8* s, int n, bool u16) {
   const int lane = lane_id();
   for (int i = lane; i < LZ4T_TILES; i += 32) tm->rdy[i] = 0;
+  for (int i = lane; i < 8192 / 32; i += 32) tm->seen[i] = 0;
   if (lane == 0) { tm->s = s; tm->n = n; tm->u16 = u16 ? 1 : 0; tm->wt = 0; tm->gen = tm->gen + 1; }
   __syncwarp();
   __threadfence_block();

@@ -18,7 +18,9 @@ breakdown of the hard streams (more than 1000 sequences) per sequence.  Phases (
 and, for the preparers, the cycles per tile from being allowed to prepare it to posting its ready word,
 split into the load of the tile's own bytes (with hash and table read) and the candidate gather (with
 compare); and the share of chained positions whose verdict was stale (its snap differed from the live
-table), which the scalar code probes again."""
+table), which the scalar code probes again; and the chained windows: sequences per window and what ended them
+(a stale element, a valid miss, a valid LZ4T_LONG, the end of the stream, a full window, the next position
+past the checked tiles)."""
 import argparse
 import ctypes as C
 import os
@@ -33,6 +35,9 @@ sys.path.insert(0, ROOT)
 TOTAL, START, SESSION, FULLWAIT, REPROBE, SEARCH, SESSIONS, SEQS, CHAIN_SEQS, PREP_BUSY, PREP_OWN, PREP_GATHER, \
     PREP_TILES, SMID, SUBP, STALE = range(16)
 NCOL = 16
+# the second enum: chained windows and what ended each
+WINDOWS, W_STALE, W_MISS, W_LONG, W_END, W_CAP, W_TILE = range(NCOL, NCOL + 7)
+NREC = NCOL + 7                                 # LZ4C_NREC: columns of a stream's record
 MAXSTREAMS = 16384
 
 
@@ -70,7 +75,7 @@ def main():
     pkg.set_profiling(True); pkg.prof_reset()
     cb = pkg.compress_ctx(clevel, shuf, ts, nbytes, d_src, d_chunk, nbytes + 16, comp)
     prof = pkg.prof_get(); pkg.set_profiling(False)
-    rec = np.zeros((MAXSTREAMS, NCOL), np.uint64)
+    rec = np.zeros((MAXSTREAMS, NREC), np.uint64)
     ns = pkg.lib.b2_lz4_cycles_read(rec.ctypes.data_as(C.c_void_p), MAXSTREAMS)
     props = torch.cuda.get_device_properties(0)
     print(f"{props.name}, {props.multi_processor_count} SMs; {CFG2}: cbytes {cb}; kernels (ms) "
@@ -119,6 +124,11 @@ def main():
     print(f"stale verdicts re-probed: {h[:, STALE].sum() / hard.sum():.0f} per stream, "
           f"{h[:, STALE].sum() / seqs:.2%} of all sequences, {h[:, STALE].sum() / max(looked, 1):.2%} of chained lookups; "
           f"chain cycles per chained sequence {chain.sum() / max(h[:, CHAIN_SEQS].sum(), 1):.1f}")
+    win = h[:, WINDOWS].sum()
+    ends = ", ".join(f"{name} {h[:, k].sum() / max(win, 1):.1%}" for name, k in
+                     (("stale", W_STALE), ("miss", W_MISS), ("long", W_LONG), ("end", W_END), ("full", W_CAP), ("tile", W_TILE)))
+    print(f"windows: {win / hard.sum():.0f} per stream, {h[:, CHAIN_SEQS].sum() / max(win, 1):.2f} chained sequences per window; "
+          f"ended by {ends}")
 
 
 if __name__ == "__main__":
