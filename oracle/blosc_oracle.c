@@ -742,10 +742,9 @@ int orc_compress_ctx(int clevel, int doshuffle, size_t typesize, size_t nbytes, 
   orc_ctx c;
   uint8_t* d = (uint8_t*)dest;
   const uint8_t* s = (const uint8_t*)src;
-  uint8_t* tmp;
-  int32_t ntbytes, j, pass;
-  int compformat;
-  (void)numinternalthreads;
+  uint8_t *tmp, *blk;
+  int32_t ntbytes, j, pass, ebsize;
+  int compformat, pool;
   /* initialize_context_compression, blosc.c:1062-1145 */
   if (nbytes > (size_t)(INT_MAX - ORC_MAX_OVERHEAD)) return 0;
   if (destsize < ORC_MAX_OVERHEAD) return 0;
@@ -778,10 +777,17 @@ int orc_compress_ctx(int clevel, int doshuffle, size_t typesize, size_t nbytes, 
   d[2] = (uint8_t)c.flags;
   /* blosc_compress_context, blosc.c:1250-1279 */
   if ((c.flags & 2) && c.nbytes + ORC_MAX_OVERHEAD > c.destsize) return 0;
-  tmp = (uint8_t*)malloc((size_t)c.blocksize + 16);
+  /* do_job (blosc.c:908-913): serial_blosc when nthreads is 1 or there is at most one block, else the pool
+   * (t_blosc), which first validates nthreads (:1975-1986) */
+  pool = numinternalthreads != 1 && c.nbytes / c.blocksize > 1;
+  if (pool && (numinternalthreads < 1 || numinternalthreads > 256)) return -1;
+  /* the pool compresses each block on its own into a scratch of ebsize bytes (:1745,1810) */
+  ebsize = c.blocksize + c.typesize * 4;
+  tmp = (uint8_t*)malloc((size_t)c.blocksize + 16 + (size_t)ebsize);
   if (!tmp) return -1;
+  blk = tmp + c.blocksize + 16;
   for (pass = 0; pass < 2; pass++) {                            /* second pass = memcpy fallback :1264-1272 */
-    for (j = 0; j < c.nblocks; j++) {                           /* serial_blosc :814-861 */
+    for (j = 0; j < c.nblocks; j++) {                           /* serial_blosc :814-861, t_blosc :1792-1856 */
       int32_t bsize = c.blocksize, cb;
       int leftoverblock = 0;
       if (!(c.flags & 2)) sti32(d + 16 + 4 * j, ntbytes);
@@ -789,6 +795,13 @@ int orc_compress_ctx(int clevel, int doshuffle, size_t typesize, size_t nbytes, 
       if (c.flags & 2) {
         memcpy(d + 16 + (size_t)j * c.blocksize, s + (size_t)j * c.blocksize, (size_t)bsize);
         cb = bsize;
+      } else if (pool) {
+        /* no per-split clamp: the pool gives up only when the running total passes destsize (:1845-1850).
+         * It copies the blocks out in whatever order they finish; this takes them in order, as the
+         * serial path does. */
+        cb = orc_block_c(&c, bsize, leftoverblock, 0, ebsize, s + (size_t)j * c.blocksize, blk, tmp);
+        if (cb == 0 || (cb > 0 && ntbytes + cb > c.destsize)) { ntbytes = 0; break; }
+        if (cb > 0) memcpy(d + ntbytes, blk, (size_t)cb);
       } else {
         cb = orc_block_c(&c, bsize, leftoverblock, ntbytes, c.destsize, s + (size_t)j * c.blocksize,
                          d + ntbytes, tmp);
