@@ -476,6 +476,16 @@ static int copy_any(void* dst, int dst_dev, const void* src, int src_dev, size_t
   return rc;
 }
 
+/* copy_any outside a call's workspace: one is taken for the copy only when either side is device memory */
+static int copy_some(void* dst, int dst_dev, const void* src, int src_dev, size_t n) {
+  b2_ws* w = NULL;
+  int rc;
+  if ((dst_dev || src_dev) && !(w = ws_acquire())) return -1;
+  rc = copy_any(dst, dst_dev, src, src_dev, n, w ? w->stream : NULL);
+  if (w) ws_release(w);
+  return rc;
+}
+
 static int stage_ready(b2_ws* w) {
   int k;
   if (w->stage_ok) return 0;
@@ -576,13 +586,9 @@ static int lz4_fast_wanted(void) {
 
 /* header + raw payload (blosc.c:825-830) */
 static int emit_memcpyed(const uint8_t* hdr, const void* src, int src_dev, void* dest, int dest_dev, int32_t nbytes) {
-  b2_ws* w = NULL;
-  int rc = 0;
-  if (src_dev || dest_dev) { w = ws_acquire(); if (!w) return -1; }
-  rc = copy_any(dest, dest_dev, hdr, 0, 16, w ? w->stream : NULL);
-  if (!rc) rc = copy_any((uint8_t*)dest + 16, dest_dev, src, src_dev, (size_t)nbytes, w ? w->stream : NULL);
-  if (w) ws_release(w);
-  return rc ? -1 : nbytes + 16;
+  if (copy_some(dest, dest_dev, hdr, 0, 16) || copy_some((uint8_t*)dest + 16, dest_dev, src, src_dev, (size_t)nbytes))
+    return -1;
+  return nbytes + 16;
 }
 
 /* ------------------------------------------------------------------------- */
@@ -865,7 +871,7 @@ static int launch_decode_blocks(b2_ws* w, const b2_hdr* h, int codec, const uint
 }
 
 /* Decode blocks [first, first+count) of a chunk that is already on the device into `d_out`
- * (device), which represents buffer offsets [first*blocksize, ...).  Shared by decompress and getitem. */
+ * (device), which represents buffer offsets [first*blocksize, ...).  Shared by decompress and a one-range read. */
 static int decode_blocks(b2_ws* w, const b2_hdr* h, int codec, const uint8_t* d_chunk, int first, int count,
                          uint8_t* d_out) {
   const int has_left = h->leftover > 0 && first + count == h->nblocks;
@@ -887,13 +893,7 @@ static int decompress_impl(const void* src, void* dest, size_t destsize, int num
   b2_ws* w;
 
   src_dev = b2_ptr_is_device(src);
-  if (src_dev) {
-    w = ws_acquire();
-    if (!w) return -1;
-    rc = copy_any(hb, 0, src, 1, 16, w->stream);
-    ws_release(w);
-    if (rc) return -1;
-  } else memcpy(hb, src, 16);
+  if (copy_some(hb, 0, src, src_dev, 16)) return -1;
   parse_header(hb, &h);
   if (max_cbytes >= 0 && (h.cbytes < BLOSC_MAX_OVERHEAD || h.cbytes > max_cbytes || h.nbytes != expect_nbytes)) return -1;
 
@@ -919,13 +919,8 @@ static int decompress_impl(const void* src, void* dest, size_t destsize, int num
   if (h.nblocks <= 0) return 0;
   if (check_threads(numinternalthreads, h.nbytes, h.blocksize) < 0) return -1;
 
-  if (h.flags & BLOSC_MEMCPYED) {                                          /* blosc.c:843-848 */
-    w = NULL;
-    if (src_dev || dest_dev) { w = ws_acquire(); if (!w) return -1; }
-    rc = copy_any(dest, dest_dev, (const uint8_t*)src + 16, src_dev, (size_t)h.nbytes, w ? w->stream : NULL);
-    if (w) ws_release(w);
-    return rc ? -1 : h.nbytes;
-  }
+  if (h.flags & BLOSC_MEMCPYED)                                            /* blosc.c:843-848 */
+    return copy_some(dest, dest_dev, (const uint8_t*)src + 16, src_dev, (size_t)h.nbytes) ? -1 : h.nbytes;
 
   w = ws_acquire();
   if (!w) return -1;
@@ -959,13 +954,7 @@ int blosc_decompress_ctx(const void* src, void* dest, size_t destsize, int numin
 static int getitem_header(const void* src, int src_dev, long long max_cbytes, b2_hdr* h, int* codec) {
   uint8_t hb[16];
   int rc;
-  if (src_dev) {
-    b2_ws* w = ws_acquire();
-    if (!w) return -1;
-    rc = copy_any(hb, 0, src, 1, 16, w->stream);
-    ws_release(w);
-    if (rc) return -1;
-  } else memcpy(hb, src, 16);
+  if (copy_some(hb, 0, src, src_dev, 16)) return -1;
   parse_header(hb, h);
   if (max_cbytes >= 0 && (h->cbytes < BLOSC_MAX_OVERHEAD || h->cbytes > max_cbytes)) return -1;
   if (h->version != BLOSC_VERSION_FORMAT) return -9;
@@ -991,78 +980,14 @@ static int getitem_range(const b2_hdr* h, int start, int nitems, long long* b_lo
   return 0;
 }
 
-static int getitem_impl(const void* src, int start, int nitems, void* dest, long long max_cbytes) {    /* blosc.c:1574-1703 */
-  b2_hdr h;
-  int src_dev, dest_dev, codec = 0, rc, result = -1;
-  b2_ws* w;
-  long long b_lo, b_hi, first, last;
-
-  src_dev = b2_ptr_is_device(src);
-  rc = getitem_header(src, src_dev, max_cbytes, &h, &codec);
-  if (rc) return rc;
-  if (getitem_range(&h, start, nitems, &b_lo, &b_hi)) return -1;
-  if (b_hi <= b_lo) return 0;                                              /* no block overlaps: loop copies nothing */
-  dest_dev = b2_ptr_is_device(dest);
-
-  if (h.flags & BLOSC_MEMCPYED) {                                          /* :1678-1683 */
-    w = NULL;
-    if (src_dev || dest_dev) { w = ws_acquire(); if (!w) return -1; }
-    rc = copy_any(dest, dest_dev, (const uint8_t*)src + 16 + b_lo, src_dev, (size_t)(b_hi - b_lo), w ? w->stream : NULL);
-    if (w) ws_release(w);
-    return rc ? -1 : (int)(b_hi - b_lo);
-  }
-
-  first = b_lo / h.blocksize; last = (b_hi - 1) / h.blocksize;             /* only overlapping blocks are decoded, :1666 */
-  w = ws_acquire();
-  if (!w) return -1;
-  do {
-    const uint8_t* d_chunk;
-    const int count = (int)(last - first + 1);
-    if (src_dev) d_chunk = (const uint8_t*)src;
-    else {
-      /* only what the decoder will read crosses PCIe: the header with bstarts[], and the bytes of the blocks that
-       * overlap the request -- from the lowest of their bstarts to the next bstart above the highest (blosc.c:1655-1668
-       * decodes just those blocks; the kernel bounds-checks every offset against cbytes as blosc_d does) */
-      const uint8_t* hs = (const uint8_t*)src;
-      const size_t index_end = 16 + 4 * (size_t)h.nblocks;
-      size_t lo = (size_t)h.cbytes, hi = 0, cut = (size_t)h.cbytes;
-      long long b;
-      int bad = 0;
-      if (buf_ensure(&w->in, (size_t)h.cbytes + 64)) break;
-      for (b = first; b <= last; b++) {
-        const int32_t bs_b = rd_i32(hs + 16 + 4 * b);
-        if (bs_b < (int32_t)index_end || bs_b > h.cbytes) { bad = 1; break; }
-        if ((size_t)bs_b < lo) lo = (size_t)bs_b;
-        if ((size_t)bs_b > hi) hi = (size_t)bs_b;
-      }
-      if (bad) { result = -1; break; }                                     /* blosc_d would refuse this offset (blosc.c:761) */
-      for (b = 0; b < h.nblocks; b++) {                                    /* where the last needed block ends */
-        const int32_t bs_b = rd_i32(hs + 16 + 4 * b);
-        if ((size_t)bs_b > hi && (size_t)bs_b < cut) cut = (size_t)bs_b;
-      }
-      if (h2d_any(w, w->in.p, hs, index_end)) break;
-      if (h2d_any(w, (uint8_t*)w->in.p + lo, hs + lo, cut - lo)) break;
-      d_chunk = (const uint8_t*)w->in.p;
-    }
-    if (buf_ensure(&w->out, (size_t)count * (size_t)h.blocksize + 64)) break;
-    rc = decode_blocks(w, &h, codec, d_chunk, (int)first, count, (uint8_t*)w->out.p);
-    if (rc < 0) { result = rc; break; }                                    /* :1689-1692 returns blosc_d's code */
-    if (copy_any(dest, dest_dev, (const uint8_t*)w->out.p + (b_lo - first * h.blocksize), 1, (size_t)(b_hi - b_lo), w->stream)) break;
-    result = (int)(b_hi - b_lo);
-  } while (0);
-  ws_release(w);
-  return result;
-}
-
-int blosc_getitem(const void* src, int start, int nitems, void* dest) { return getitem_impl(src, start, nitems, dest, -1); }
-
 /* ------------------------------------------------------------------------- */
-/* many item ranges of one chunk in one pass (blosc_b200_getitems)             */
+/* item ranges of one chunk in one pass (blosc_getitem, blosc_b200_getitems)  */
 /* ------------------------------------------------------------------------- */
 /* Every block that some range overlaps is decoded exactly once, by one decode launch over the sorted list of those
  * blocks: the j-th listed block decodes to j * blocksize of a compact scratch (StreamMap.blocks).  A range covers a
  * run of consecutive blocks, which stay adjacent in the list, so it is one contiguous span of the scratch.  One
- * unfilter launch and one gather launch (gather_kernel) then copy every range to its place in dest. */
+ * unfilter launch and one gather launch (gather_kernel) then copy every range to its place in dest.  A single range
+ * needs neither the list nor the gather: its blocks decode as one run and one copy moves it to dest. */
 typedef struct { long long lo, hi; } b2_iv;
 
 static int cmp_iv(const void* a, const void* b) {
@@ -1086,29 +1011,48 @@ static int merge_ivs(b2_iv* iv, int n) {
   return k + 1;
 }
 
-/* Stage what the decoder reads of a host-resident chunk: the header with bstarts[] and, for every listed block, its
- * bytes from its bstart to the next bstart above it (as getitem_impl does for one span); adjacent spans are copied as
- * one.  -1 when a listed block's bstart is out of bounds (blosc_d would refuse it, blosc.c:761). */
+/* Stage what the decoder reads of a host-resident chunk: the header with bstarts[] and, for every listed block (the
+ * list is ascending), its bytes from its bstart to the next bstart above it; adjacent spans are copied as one.  -1 when
+ * a listed block's bstart is out of bounds (blosc_d would refuse it, blosc.c:761). */
 static int stage_blocks(b2_ws* w, const b2_hdr* h, const uint8_t* hs, const int* blocks, int count) {
   const size_t index_end = 16 + 4 * (size_t)h->nblocks;
-  int32_t* sorted = (int32_t*)malloc(4 * (size_t)h->nblocks + 4);
+  const int run = blocks[count - 1] - blocks[0] == count - 1;              /* consecutive block numbers */
+  int32_t* sorted = run ? NULL : (int32_t*)malloc(4 * (size_t)h->nblocks + 4);
   b2_iv* iv = (b2_iv*)malloc(sizeof(b2_iv) * (size_t)count + sizeof(b2_iv));
   int i, n = 0, rc = -1;
   do {
-    if (!sorted || !iv) break;
-    for (i = 0; i < h->nblocks; i++) sorted[i] = rd_i32(hs + 16 + 4 * (size_t)i);
-    qsort(sorted, (size_t)h->nblocks, 4, cmp_i32);
-    for (i = 0; i < count; i++) {
-      const int32_t bs_b = rd_i32(hs + 16 + 4 * (size_t)blocks[i]);
-      int lo = 0, hi = h->nblocks;
-      if (bs_b < (int32_t)index_end || bs_b > h->cbytes) break;
-      while (lo < hi) { const int m = (lo + hi) / 2; if (sorted[m] <= bs_b) lo = m + 1; else hi = m; }   /* first above */
-      iv[n].lo = bs_b;
-      iv[n].hi = (lo < h->nblocks && sorted[lo] < h->cbytes) ? sorted[lo] : h->cbytes;
-      n++;
+    if ((!run && !sorted) || !iv) break;
+    if (run) {
+      /* one span, from the lowest of their bstarts to the next bstart above the highest: two linear passes over
+       * bstarts[], no sort, whatever the chunk's number of blocks */
+      int32_t lo = h->cbytes, hi = 0, cut = h->cbytes;
+      for (i = 0; i < count; i++) {
+        const int32_t bs_b = rd_i32(hs + 16 + 4 * (size_t)(blocks[0] + i));
+        if (bs_b < (int32_t)index_end || bs_b > h->cbytes) break;
+        if (bs_b < lo) lo = bs_b;
+        if (bs_b > hi) hi = bs_b;
+      }
+      if (i < count) break;
+      for (i = 0; i < h->nblocks; i++) {
+        const int32_t bs_b = rd_i32(hs + 16 + 4 * (size_t)i);
+        if (bs_b > hi && bs_b < cut) cut = bs_b;
+      }
+      iv[0].lo = lo; iv[0].hi = cut; n = 1;
+    } else {
+      for (i = 0; i < h->nblocks; i++) sorted[i] = rd_i32(hs + 16 + 4 * (size_t)i);
+      qsort(sorted, (size_t)h->nblocks, 4, cmp_i32);
+      for (i = 0; i < count; i++) {
+        const int32_t bs_b = rd_i32(hs + 16 + 4 * (size_t)blocks[i]);
+        int lo = 0, hi = h->nblocks;
+        if (bs_b < (int32_t)index_end || bs_b > h->cbytes) break;
+        while (lo < hi) { const int m = (lo + hi) / 2; if (sorted[m] <= bs_b) lo = m + 1; else hi = m; }   /* first above */
+        iv[n].lo = bs_b;
+        iv[n].hi = (lo < h->nblocks && sorted[lo] < h->cbytes) ? sorted[lo] : h->cbytes;
+        n++;
+      }
+      if (i < count) break;
+      n = merge_ivs(iv, n);
     }
-    if (i < count) break;
-    n = merge_ivs(iv, n);
     if (buf_ensure(&w->in, (size_t)h->cbytes + 64)) break;
     if (h2d_any(w, w->in.p, hs, index_end)) break;
     for (i = 0; i < n; i++)
@@ -1179,7 +1123,7 @@ static long long getitems_run(b2_ws* w, const b2_hdr* h, int codec, const uint8_
 
 /* The host plan: `n` ranges of one chunk, in host memory; range r goes to dest + dsts[r] (back to back in request order
  * when dsts is NULL).  The header and every range are validated before anything is launched or written.  Returns the
- * bytes written. */
+ * bytes written, or blosc_getitem's code. */
 static long long getitems_chunk(const void* src, long long max_cbytes, int n, const int* starts, const int* nitems,
                                 const long long* dsts, void* dest) {
   b2_hdr h;
@@ -1216,11 +1160,12 @@ static long long getitems_chunk(const void* src, long long max_cbytes, int n, co
   if (nr == 0) { free(tab); free(lo_b); return 0; }
   dest_dev = b2_ptr_is_device(dest);
 
-  if ((h.flags & BLOSC_MEMCPYED) && !src_dev && !dest_dev) {               /* :1678-1683, host to host */
-    for (r = 0; r < nr; r++)
-      memcpy((uint8_t*)dest + tab[r].dst, (const uint8_t*)src + 16 + tab[r].src, (size_t)(tab[r + 1].pos - tab[r].pos));
+  if ((h.flags & BLOSC_MEMCPYED) && (nr == 1 || (!src_dev && !dest_dev))) {  /* :1678-1683, one copy per range */
+    for (r = 0, rc = 0; r < nr && !rc; r++)
+      rc = copy_some((uint8_t*)dest + tab[r].dst, dest_dev, (const uint8_t*)src + 16 + tab[r].src, src_dev,
+                     (size_t)(tab[r + 1].pos - tab[r].pos));
     free(tab); free(lo_b);
-    return total;
+    return rc ? -1 : total;
   }
 
   w = ws_acquire();
@@ -1257,16 +1202,25 @@ static long long getitems_chunk(const void* src, long long max_cbytes, int n, co
         long long b;
         for (b = iv[k].lo; b < iv[k].hi; b++) blocks[count++] = (int)b;
       }
+      if (src_dev) d_chunk = (const uint8_t*)src;
+      else {
+        if (stage_blocks(w, &h, (const uint8_t*)src, blocks, count)) break;
+        d_chunk = (const uint8_t*)w->in.p;
+      }
+      if (nr == 1) {                               /* one range: its run of blocks decodes with no list and no gather */
+        if (buf_ensure(&w->out, (size_t)count * (size_t)bs + 64)) break;
+        rc = decode_blocks(w, &h, codec, d_chunk, blocks[0], count, (uint8_t*)w->out.p);
+        if (rc < 0) { result = rc; break; }                                /* :1689-1692 returns blosc_d's code */
+        if (copy_any((uint8_t*)dest + tab[0].dst, dest_dev, (const uint8_t*)w->out.p + (lo_b[0] - (long long)blocks[0] * bs),
+                     1, (size_t)total, w->stream)) break;
+        result = total;
+        break;
+      }
       for (r = 0; r < nr; r++) {                                           /* range r -> its span of the scratch */
         const long long first = lo_b[r] / bs;
         int lo = 0, hi = count - 1;
         while (lo < hi) { const int m = (lo + hi + 1) / 2; if (blocks[m] <= first) lo = m; else hi = m - 1; }
         tab[r].src = (long long)lo * bs + (lo_b[r] - first * bs);
-      }
-      if (src_dev) d_chunk = (const uint8_t*)src;
-      else {
-        if (stage_blocks(w, &h, (const uint8_t*)src, blocks, count)) break;
-        d_chunk = (const uint8_t*)w->in.p;
       }
       if (buf_ensure(&w->bstarts, sizeof(int) * (size_t)count + 64)) break;
       if (b2_copy_h2d(w->bstarts.p, blocks, sizeof(int) * (size_t)count, w->stream)) break;
@@ -1278,6 +1232,10 @@ static long long getitems_chunk(const void* src, long long max_cbytes, int n, co
   ws_release(w);
   free(tab); free(lo_b); free(iv); free(blocks); free(tmp);
   return result;
+}
+
+int blosc_getitem(const void* src, int start, int nitems, void* dest) {                 /* blosc.c:1574-1703 */
+  return (int)getitems_chunk(src, -1, 1, &start, &nitems, NULL, dest);
 }
 
 /* Stage the payload of a memcpyed host chunk that the listed blocks cover, block j of the list at j * blocksize of
@@ -1590,11 +1548,7 @@ long long blosc_b200_frame_compress(int clevel, int doshuffle, size_t typesize, 
     wr_u64(index + 8, (uint64_t)nbytes); wr_u64(index + 16, (uint64_t)j.cursor);
     wr_u32(index + 24, (uint32_t)chunksize); wr_u32(index + 28, (uint32_t)nchunks);
     for (i = 0; i < (int)nchunks; i++) wr_u64(index + B2_FRAME_HDR + 8 * (size_t)i, j.offsets[i]);
-    if (dest_dev) {
-      b2_ws* w = ws_acquire();
-      rc = w ? copy_any(dest, 1, index, 0, index_bytes, w->stream) : -1;
-      if (w) ws_release(w);
-    } else memcpy(dest, index, index_bytes);
+    rc = copy_some(dest, dest_dev, index, 0, index_bytes);
   }
   free(j.offsets); free(index);
   if (rc) return j.err ? j.err : (j.failed ? 0 : -1);            /* 0: does not fit in destsize, as blosc_compress */
@@ -1610,16 +1564,8 @@ static int frame_open(const void* frame, size_t framesize, size_t* nbytes, size_
   uint64_t cbytes;
   size_t n, k;
   const int dev = b2_ptr_is_device(frame);
-  b2_ws* w = NULL;
-  int rc = 0;
-  if (framesize < B2_FRAME_HDR) return -1;
-  if (dev) {
-    w = ws_acquire();
-    if (!w) return -1;
-    rc = copy_any(hb, 0, frame, 1, B2_FRAME_HDR, w->stream);
-    if (rc) { ws_release(w); return -1; }
-  } else memcpy(hb, frame, B2_FRAME_HDR);
-  rc = -1;
+  int rc = -1;
+  if (framesize < B2_FRAME_HDR || copy_some(hb, 0, frame, dev, B2_FRAME_HDR)) return -1;
   do {
     if (memcmp(hb, "B2FR", 4) != 0 || hb[4] != 1) break;
     *nbytes = (size_t)rd_u64(hb + 8); cbytes = rd_u64(hb + 16);
@@ -1630,8 +1576,7 @@ static int frame_open(const void* frame, size_t framesize, size_t* nbytes, size_
     raw = (uint8_t*)malloc(8 * n + 8);
     off = (uint64_t*)malloc(8 * (n + 1));
     if (!raw || !off) { free(raw); free(off); break; }
-    if (dev) { if (copy_any(raw, 0, (const uint8_t*)frame + B2_FRAME_HDR, 1, 8 * n, w->stream)) { free(raw); free(off); break; } }
-    else memcpy(raw, (const uint8_t*)frame + B2_FRAME_HDR, 8 * n);
+    if (copy_some(raw, 0, (const uint8_t*)frame + B2_FRAME_HDR, dev, 8 * n)) { free(raw); free(off); break; }
     for (k = 0; k < n; k++) off[k] = rd_u64(raw + 8 * k);
     off[n] = cbytes;
     free(raw);
@@ -1641,7 +1586,6 @@ static int frame_open(const void* frame, size_t framesize, size_t* nbytes, size_
     if (rc) { free(off); break; }
     *nchunks = n; *offsets = off;
   } while (0);
-  if (w) ws_release(w);
   return rc;
 }
 
@@ -1689,40 +1633,6 @@ long long blosc_b200_frame_decompress(const void* frame, size_t framesize, void*
   return rc ? -1 : (long long)nb;
 }
 
-long long blosc_b200_frame_getitem(const void* frame, size_t framesize, size_t start, size_t nitems, void* dest) {
-  size_t nb = 0, cs = 0, nc = 0, ts = 0, ipc, done = 0;
-  uint64_t* off = NULL;
-  uint8_t hb[16];
-  long long result = -1;
-  if (!backend_ready()) return -1;
-  if (frame_open(frame, framesize, &nb, &cs, &nc, &off)) return -1;
-  do {
-    if (nc == 0) { result = nitems == 0 ? 0 : -1; break; }
-    if (b2_ptr_is_device(frame)) {
-      b2_ws* w = ws_acquire();
-      int rc = w ? copy_any(hb, 0, (const uint8_t*)frame + off[0], 1, 16, w->stream) : -1;
-      if (w) ws_release(w);
-      if (rc) break;
-    } else memcpy(hb, (const uint8_t*)frame + off[0], 16);
-    ts = hb[3];
-    if (ts == 0 || cs % ts) break;
-    ipc = cs / ts;                                     /* items per chunk */
-    if (start > nb / ts || nitems > nb / ts - start) { fprintf(stderr, "`start`+`nitems` out of bounds"); break; }
-    result = 0;
-    while (done < nitems) {
-      const size_t c = (start + done) / ipc, first = (start + done) % ipc;
-      const size_t take = nitems - done < ipc - first ? nitems - done : ipc - first;
-      const int rc = getitem_impl((const uint8_t*)frame + off[c], (int)first, (int)take, (uint8_t*)dest + done * ts,
-                                  (long long)(off[c + 1] - off[c]));
-      if (rc != (int)(take * ts)) { result = rc < 0 ? rc : -1; break; }
-      done += take;
-      result += rc;
-    }
-  } while (0);
-  free(off);
-  return result;
-}
-
 /* One piece of a frame range: the part that falls in one chunk */
 typedef struct { size_t chunk, order; int start, nitems; long long dst; } b2_piece;
 
@@ -1732,34 +1642,9 @@ static int cmp_piece(const void* a, const void* b) {
   return x->order < y->order ? -1 : x->order > y->order;
 }
 
-static long long frame_getitems_host(const void* frame, size_t framesize, size_t nranges, const size_t* starts,
-                                     const size_t* nitems, void* dest);
-
-/* Range lists in device memory are copied to the host (one copy each), and the frame is planned there */
-long long blosc_b200_frame_getitems(const void* frame, size_t framesize, size_t nranges, const size_t* starts,
-                                    const size_t* nitems, void* dest) {
-  size_t* h = NULL;
-  b2_ws* w;
-  long long result = -1;
-  int starts_dev, nitems_dev;
-  if (nranges == 0) return 0;
-  if (!backend_ready()) return -1;
-  starts_dev = b2_ptr_is_device(starts); nitems_dev = b2_ptr_is_device(nitems);
-  if (!starts_dev && !nitems_dev) return frame_getitems_host(frame, framesize, nranges, starts, nitems, dest);
-  if (nranges > ((size_t)-1) / (2 * sizeof(size_t)) || !(h = (size_t*)malloc(2 * sizeof(size_t) * nranges))) return -1;
-  if ((w = ws_acquire()) != NULL) {
-    if (!copy_any(h, 0, starts, starts_dev, sizeof(size_t) * nranges, w->stream) &&
-        !copy_any(h + nranges, 0, nitems, nitems_dev, sizeof(size_t) * nranges, w->stream))
-      result = 0;
-    ws_release(w);
-  }
-  if (result == 0) result = frame_getitems_host(frame, framesize, nranges, h, h + nranges, dest);
-  free(h);
-  return result;
-}
-
-/* Every range is checked as blosc_b200_frame_getitem checks one before anything is read; then the ranges are cut at
- * chunk boundaries and each touched chunk runs the chunk plan once, each piece landing at its own dest offset. */
+/* Every range is checked against the frame's items before anything is read; then the ranges are cut at chunk
+ * boundaries and each touched chunk, in ascending order, runs the chunk plan once, each piece landing at its own dest
+ * offset. */
 static long long frame_getitems_host(const void* frame, size_t framesize, size_t nranges, const size_t* starts,
                                      const size_t* nitems, void* dest) {
   size_t nb = 0, cs = 0, nc = 0, ts = 0, ipc, r, npieces = 0, i, j;
@@ -1774,12 +1659,7 @@ static long long frame_getitems_host(const void* frame, size_t framesize, size_t
       result = r == nranges ? 0 : -1;
       break;
     }
-    if (b2_ptr_is_device(frame)) {
-      b2_ws* w = ws_acquire();
-      int rc = w ? copy_any(hb, 0, (const uint8_t*)frame + off[0], 1, 16, w->stream) : -1;
-      if (w) ws_release(w);
-      if (rc) break;
-    } else memcpy(hb, (const uint8_t*)frame + off[0], 16);
+    if (copy_some(hb, 0, (const uint8_t*)frame + off[0], b2_ptr_is_device(frame), 16)) break;
     ts = hb[3];
     if (ts == 0 || cs % ts) break;
     ipc = cs / ts;                                     /* items per chunk */
@@ -1823,6 +1703,29 @@ static long long frame_getitems_host(const void* frame, size_t framesize, size_t
     }
   } while (0);
   free(pieces); free(off);
+  return result;
+}
+
+long long blosc_b200_frame_getitem(const void* frame, size_t framesize, size_t start, size_t nitems, void* dest) {
+  if (!backend_ready()) return -1;
+  return frame_getitems_host(frame, framesize, 1, &start, &nitems, dest);
+}
+
+/* Range lists in device memory are copied to the host (one copy each), and the frame is planned there */
+long long blosc_b200_frame_getitems(const void* frame, size_t framesize, size_t nranges, const size_t* starts,
+                                    const size_t* nitems, void* dest) {
+  size_t* h = NULL;
+  long long result = -1;
+  int starts_dev, nitems_dev;
+  if (nranges == 0) return 0;
+  if (!backend_ready()) return -1;
+  starts_dev = b2_ptr_is_device(starts); nitems_dev = b2_ptr_is_device(nitems);
+  if (!starts_dev && !nitems_dev) return frame_getitems_host(frame, framesize, nranges, starts, nitems, dest);
+  if (nranges > ((size_t)-1) / (2 * sizeof(size_t)) || !(h = (size_t*)malloc(2 * sizeof(size_t) * nranges))) return -1;
+  if (!copy_some(h, 0, starts, starts_dev, sizeof(size_t) * nranges) &&
+      !copy_some(h + nranges, 0, nitems, nitems_dev, sizeof(size_t) * nranges))
+    result = frame_getitems_host(frame, framesize, nranges, h, h + nranges, dest);
+  free(h);
   return result;
 }
 

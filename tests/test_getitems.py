@@ -1,9 +1,10 @@
 """blosc_b200_getitems / blosc_b200_frame_getitems: many item ranges in one call, each touched block decoded once.
 
-Every result is checked against the concatenation of per-range blosc_getitem (frame_getitem) calls on the same library,
-and, where oracle/_ref was built, against the reference's blosc_getitem on a chunk the reference wrote.  CPU: the
-product's host code and kernels inside the SIMT emulator (tests/emu).  GPU: the same matrix through the CUDA library,
-plus host / device pointer combinations, launch counts and the profiler's decode count."""
+Every result is checked against the slices of the source array it was compressed from, against the concatenation of
+per-range blosc_getitem (frame_getitem) calls on the same library, and, where oracle/_ref was built, against the
+reference's blosc_getitem on a chunk the reference wrote.  CPU: the product's host code and kernels inside the SIMT
+emulator (tests/emu).  GPU: the same matrix through the CUDA library, plus host / device pointer combinations, launch
+counts and the profiler's decode count."""
 import ctypes as C
 import glob
 import os
@@ -59,6 +60,7 @@ def elib(tmp_path_factory):
     lib.emu_last_decode_streams.restype = ci
     lib.emu_last_decode_blocks.restype = ci
     lib.emu_launches_with_gather.restype = ll
+    lib.emu_set_device_ptrs.argtypes = [C.c_void_p, C.c_void_p]
     return lib
 
 
@@ -97,10 +99,15 @@ def _getitems(lib, src, ranges, dest_len):
     return r, out
 
 
-def _check_chunk(lib, chunk, ts, nbytes, bs_items, seed, ref=None, refchunk=None, k=14):
+def _slices(src, ranges, ts):
+    return np.concatenate([src[ts * s:ts * (s + n)] for s, n in ranges])
+
+
+def _check_chunk(lib, chunk, src, ts, nbytes, bs_items, seed, ref=None, refchunk=None, k=14):
     rng = np.random.default_rng(seed)
     ranges = _ranges(nbytes // ts, bs_items, ts, rng, k)
     want = _per_range(lib, chunk, ranges, ts)
+    assert (want == _slices(src, ranges, ts)).all()
     r, out = _getitems(lib, chunk, ranges, len(want))
     assert r == len(want), (r, len(want))
     assert (out[:r] == want).all() and (out[r:] == 0xAA).all()
@@ -137,8 +144,8 @@ def test_getitems_equals_getitem_emu(elib, ref_if_built, monkeypatch, comp, swit
             if ref_if_built is not None and comp in ("blosclz", "lz4", "lz4hc") and split == FORWARD_COMPAT_SPLIT:
                 r, rc = compress(ref_if_built, "blosc_compress_ctx", 5, shuf, ts, src, len(src) + 16, comp, 8192)
                 refchunk = rc[:r].copy()
-            _check_chunk(elib, chunk, ts, len(src), bs // ts, seed=ts * 7 + shuf, ref=ref_if_built if refchunk is not None
-                         else None, refchunk=refchunk, k=6)
+            _check_chunk(elib, chunk, src, ts, len(src), bs // ts, seed=ts * 7 + shuf,
+                         ref=ref_if_built if refchunk is not None else None, refchunk=refchunk, k=6)
 
 
 def test_getitems_memcpyed_emu(elib):
@@ -149,7 +156,7 @@ def test_getitems_memcpyed_emu(elib):
         for dev in (0, 1):
             elib.emu_set_all_device(dev)
             try:
-                _check_chunk(elib, c[:r].copy(), ts, n, max(n // ts // 3, 1), seed=n + dev)
+                _check_chunk(elib, c[:r].copy(), src, ts, n, max(n // ts // 3, 1), seed=n + dev)
             finally:
                 elib.emu_set_all_device(0)
 
@@ -161,31 +168,64 @@ def test_getitems_device_pointers_emu(elib, dev):
     c = compress(elib, "blosc_compress_ctx", 5, 1, 4, src, len(src) + 16, "lz4", 16384)[1]
     elib.emu_set_all_device(dev)
     try:
-        _check_chunk(elib, c, 4, len(src), 4096, seed=11)
+        _check_chunk(elib, c, src, 4, len(src), 4096, seed=11)
     finally:
         elib.emu_set_all_device(0)
 
 
-def test_getitems_one_pass_emu(elib):
+def test_getitems_launches_emu(elib):
     """One decode, one unfilter and one gather launch per call whatever the number of ranges, and the decode covers
-    the touched blocks times their splits, not the ranges"""
+    the touched blocks times their splits, not the ranges.  One range decodes its blocks with no list and no gather,
+    as blosc_getitem does."""
     src = bench_words(8 * 65536 + 1000)
     r, c = compress(elib, "blosc_compress_ctx", 5, 1, 4, src, len(src) + 16, "lz4", 16384)
     assert r > 0 and not c[2] & 0x10 and int(c[8:12].view(np.int32)[0]) == 65536   # 4 streams per full block
     nit = len(src) // 4
     counts = []
-    for ranges, blocks in (([(20000, 64)], 1),
-                           ([(16384 * b + 7, 64) for b in (1, 3, 3, 1, 5)] * 3, 3),
-                           ([(int(s), 64) for s in np.random.default_rng(1).integers(0, nit - 64, 4096)], 9)):
+    # (ranges, blocks listed in the decode launch, its streams); the short last block has 1 stream
+    spread = [(int(s), 64) for s in np.random.default_rng(1).integers(0, nit - 64, 4096)]
+    for ranges, listed, streams in (([(20000, 64)], 0, 4),
+                                    ([(16384 * b + 7, 64) for b in (1, 3, 3, 1, 5)] * 3, 3, 12),
+                                    (spread, 9, 33)):
         before = elib.emu_launches_with_gather()
         got, out = _getitems(elib, c, ranges, 64 * 4 * len(ranges))
         counts.append(elib.emu_launches_with_gather() - before)
         assert got == 64 * 4 * len(ranges)
         want = np.concatenate([src[4 * s:4 * (s + n)] for s, n in ranges])
         assert (out[:got] == want).all()
-        assert elib.emu_last_decode_blocks() == blocks
-        assert elib.emu_last_decode_streams() == 4 * blocks - (1 if blocks == 9 else 0) * 3   # the short block: 1 stream
-    assert counts == [3, 3, 3]
+        assert elib.emu_last_decode_blocks() == listed
+        assert elib.emu_last_decode_streams() == streams
+    assert counts == [2, 3, 3]
+    before = elib.emu_launches_with_gather()
+    one = np.zeros(64 * 4, np.uint8)
+    assert elib.blosc_getitem(ptr(c), ci(20000), ci(64), ptr(one)) == 64 * 4
+    assert elib.emu_launches_with_gather() - before == counts[0]
+    assert (one == src[4 * 20000:4 * 20064]).all()
+
+
+@pytest.mark.parametrize("src_dev,dest_dev", [(0, 0), (0, 1), (1, 0), (1, 1)])
+def test_getitem_one_range_memcpyed_emu(elib, src_dev, dest_dev):
+    """One range of a memcpyed chunk is one copy from the payload to dest, with no launch, wherever src and dest are"""
+    src = gen("rand", 40000, seed=3)
+    r, c = compress(elib, "blosc_compress_ctx", 0, 1, 4, src, len(src) + 16, "lz4")
+    assert r == len(src) + 16 and c[2] & 0x2                    # BLOSC_MEMCPYED
+    chunk = c[:r].copy()
+    out = np.full(len(src) + 8, 0xAA, np.uint8)
+    elib.emu_set_device_ptrs(chunk.ctypes.data if src_dev else None, out.ctypes.data if dest_dev else None)
+    try:
+        for s, n in ((0, 10000), (1234, 1), (5000, 777), (9999, 1), (3, 0)):
+            st, nn = np.array([s], np.int32), np.array([n], np.int32)
+            for many in (False, True):
+                out[:] = 0xAA
+                before = elib.emu_launches_with_gather()
+                if many:
+                    got = elib.blosc_b200_getitems(ptr(chunk), 1, st.ctypes.data, nn.ctypes.data, ptr(out))
+                else:
+                    got = elib.blosc_getitem(ptr(chunk), ci(s), ci(n), ptr(out))
+                assert elib.emu_launches_with_gather() == before
+                assert got == 4 * n and (out[:got] == src[4 * s:4 * (s + n)]).all() and (out[got:] == 0xAA).all()
+    finally:
+        elib.emu_set_device_ptrs(None, None)
 
 
 def test_getitems_rejects_emu(elib):
@@ -221,7 +261,7 @@ def test_getitems_rejects_emu(elib):
             r, out = _getitems(elib, h, good + [(2 * 2048 + 5, 3)], 256)
             assert r == elib.blosc_getitem(ptr(h), ci(2 * 2048 + 5), ci(3), ptr(np.zeros(64, np.uint8))) < 0
             assert (out == 0xAA).all()
-            assert _check_chunk(elib, h, 4, 2 * 8192, 2048, seed=5) is not None        # blocks 0 and 1 only
+            assert _check_chunk(elib, h, src, 4, 2 * 8192, 2048, seed=5) is not None   # blocks 0 and 1 only
         finally:
             elib.emu_set_all_device(0)
 
@@ -242,7 +282,7 @@ def _frame_ranges(nit, per_chunk, rng):
     return [out[i] for i in rng.permutation(len(out))]
 
 
-def _check_frame(lib, frame, fb, ts, nit, per_chunk, seed):
+def _check_frame(lib, frame, fb, src, ts, nit, per_chunk, seed):
     ranges = _frame_ranges(nit, per_chunk, np.random.default_rng(seed))
     parts = []
     for s, n in ranges:
@@ -250,6 +290,7 @@ def _check_frame(lib, frame, fb, ts, nit, per_chunk, seed):
         assert lib.blosc_b200_frame_getitem(ptr(frame), fb, s, n, ptr(buf)) == n * ts
         parts.append(buf[:n * ts])
     want = np.concatenate(parts)
+    assert (want == _slices(src, ranges, ts)).all()
     st = np.array([s for s, _ in ranges], np.uint64)
     nn = np.array([n for _, n in ranges], np.uint64)
     out = np.full(len(want) + 8, 0xAA, np.uint8)
@@ -268,7 +309,7 @@ def test_frame_getitems_emu(elib, dev):
     frame, fb = _frame(elib, src, 4, 24000)
     elib.emu_set_all_device(dev)
     try:
-        _check_frame(elib, frame, fb, 4, len(src) // 4, 6000, seed=dev)
+        _check_frame(elib, frame, fb, src, 4, len(src) // 4, 6000, seed=dev)
     finally:
         elib.emu_set_all_device(0)
 
@@ -300,7 +341,7 @@ def test_getitems_equals_getitem_gpu(glib, cuda, ref_if_built, monkeypatch, comp
                 if ref_if_built is not None and comp in ("blosclz", "lz4", "lz4hc") and split == FORWARD_COMPAT_SPLIT:
                     r, rc = compress(ref_if_built, "blosc_compress_ctx", 5, shuf, ts, src, len(src) + 16, comp, bs)
                     refchunk = rc[:r].copy()
-                _check_chunk(glib, chunk, ts, len(src), cbs // ts, seed=ts + 100 * shuf + bs,
+                _check_chunk(glib, chunk, src, ts, len(src), cbs // ts, seed=ts + 100 * shuf + bs,
                              ref=ref_if_built if refchunk is not None else None, refchunk=refchunk)
 
 
@@ -310,7 +351,7 @@ def test_getitems_goldens_gpu(glib, cuda, monkeypatch):
     want = np.arange(1000000, dtype=np.int32).view(np.uint8)
     for f in GOLDENS:
         chunk = np.fromfile(f, np.uint8)
-        ranges = _check_chunk(glib, chunk, 4, 4000000, int(chunk[8:12].view(np.int32)[0]) // 4, seed=len(f))
+        ranges = _check_chunk(glib, chunk, want, 4, 4000000, int(chunk[8:12].view(np.int32)[0]) // 4, seed=len(f))
         r, out = _getitems(glib, chunk, ranges, sum(n for _, n in ranges) * 4)
         assert (out[:r] == np.concatenate([want[4 * s:4 * (s + n)] for s, n in ranges])).all(), f
 
@@ -321,7 +362,7 @@ def test_getitems_memcpyed_gpu(glib, cuda):
         src = gen("rand", n, seed=n)
         r, c = compress(glib, "blosc_compress_ctx", clevel, 1, ts, src, n + 16, "lz4")
         assert r == n + 16 and c[2] & 0x2
-        _check_chunk(glib, c[:r].copy(), ts, n, max(n // ts // 3, 1), seed=n)
+        _check_chunk(glib, c[:r].copy(), src, ts, n, max(n // ts // 3, 1), seed=n)
 
 
 @pytest.mark.gpu
@@ -349,7 +390,8 @@ def test_getitems_pointer_kinds_gpu(pkg, cuda, clevel):
 
 
 @pytest.mark.gpu
-def test_getitems_one_pass_gpu(pkg, cuda):
+def test_getitems_launches_gpu(pkg, cuda):
+    """one decode, one unfilter and one gather launch per call with host lists; one range has no gather"""
     src = bench_words(32 << 20)
     r, c = compress(pkg.lib, "blosc_compress_ctx", 5, 1, 4, src, len(src) + 16, "lz4")
     chunk = cuda.from_numpy(c[:r].copy()).cuda()
@@ -365,12 +407,13 @@ def test_getitems_one_pass_gpu(pkg, cuda):
             assert pkg.getitems(chunk, st, np.full(k, 64), out) == 64 * 4 * k
             grown.append(pkg.launch_count() - before)
             prof = pkg.prof_get()
-            assert prof["decode"][1] == 1 and prof["gather"][1] == 1 and prof["unfilter"][1] == 1, prof
+            gathers = 0 if k == 1 else 1                          # one range: no gather, as blosc_getitem
+            assert prof["decode"][1] == 1 and prof["gather"][1] == gathers and prof["unfilter"][1] == 1, prof
             want = np.concatenate([src[4 * s:4 * (s + 64)] for s in st])
             assert (out.cpu().numpy() == want).all()
     finally:
         pkg.set_profiling(False)
-    assert grown == [3, 3, 3]
+    assert grown == [2, 3, 3]
 
 
 @pytest.mark.gpu
@@ -423,4 +466,4 @@ def test_frame_getitems_gpu(glib, pkg, cuda, dev):
         assert pkg.frame_getitems(d_frame, fb, [s for s, _ in ranges], [n for _, n in ranges], h_out) == len(want)
         assert (h_out == want).all()
     else:
-        _check_frame(glib, frame, fb, 4, len(src) // 4, 250000, seed=4)
+        _check_frame(glib, frame, fb, src, 4, len(src) // 4, 250000, seed=4)
