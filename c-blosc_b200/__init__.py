@@ -172,7 +172,8 @@ def frame_getitem(frame, framesize, start, nitems, dest):
 
 def frame_getitems(frame, framesize, starts, nitems, dest):
     """getitems over a frame (blosc_b200_frame_getitems); ranges may cross chunk boundaries.  starts / nitems may be
-    int64 or uint64 CUDA tensors (copied to the host for the plan)."""
+    int64 or uint64 CUDA tensors: on the device of the call, the read is then planned on the GPU (on another device,
+    they are copied to the host for the plan)."""
     st, n = _ranges(starts, nitems, "uint64", ("torch.int64", "torch.uint64"))
     return int(lib.blosc_b200_frame_getitems(_ptr(frame), framesize, st[2], st[1], n[1], _ptr(dest)))
 

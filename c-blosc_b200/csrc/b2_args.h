@@ -191,6 +191,14 @@ static inline B2_HD int b2_range_check(int start, int nitems, int typesize, long
   return 0;
 }
 
+/* The frame's check of one range against its `total` items, the one statement of it: the host plan of frame getitems
+ * (blosc_b200.c frame_getitems_host) and its GPU plan (dev_chunk.cuh fplan_check_kernel) both call it.  Nonzero: the
+ * range is out of bounds.  No sum is formed, so nothing wraps at the u64 extremes. */
+static inline B2_HD int b2_frame_range_bad(unsigned long long start, unsigned long long nitems,
+                                           unsigned long long total) {
+  return start > total || nitems > total - start;
+}
+
 /* What the GPU plan of getitems leaves for the host, read back with one small copy */
 typedef struct GetitemsPlan {
   unsigned bad;          /* index of the first failing range; 0xffffffff when every range is valid */
@@ -226,11 +234,50 @@ typedef struct PlanArgs {
   GatherRange* ranges;   /* [nranges + 1] the gather table, in request order, empty ranges included */
   GetitemsPlan* rec;     /* zeroed but for rec->bad = 0xffffffff */
   PlanScan scan[3];      /* PLAN_COVER, PLAN_SLOT, PLAN_POS */
+  const long long* dsts; /* NULL: range r lands at its position in dest; else at dsts[r] (frame pieces) */
 } PlanArgs;
 enum { PLAN_COVER = 0, PLAN_SLOT = 1, PLAN_POS = 2 };
 #define PLAN_THREADS 256
 #define PLAN_ITEMS 8
 #define PLAN_TILE (PLAN_THREADS * PLAN_ITEMS)
+
+/* What the GPU plan of frame getitems leaves for the host, read back with one small copy */
+typedef struct FramePlan {
+  unsigned long long bad;    /* index of the first failing range; all ones when every range is valid */
+  long long total;           /* bytes of all ranges */
+  long long npieces;         /* pieces of all chunks */
+  long long ntouched;        /* chunks with at least one piece */
+} FramePlan;
+
+/* One touched chunk: its pieces are [base, base + count) of the piece lists */
+typedef struct FrameTouch {
+  long long chunk, base, count;
+} FrameTouch;
+
+/* frame getitems planned on the GPU from device-resident range lists: every range is cut at the chunk boundaries into
+ * pieces, and each chunk's pieces are gathered into one bucket of the piece lists, which the chunk plan (PlanArgs with
+ * dsts) then reads like range lists of its own.  Kernels: fplan_check_kernel, the scans FPLAN_DST over the ranges and
+ * FPLAN_COUNT, FPLAN_BASE, FPLAN_TOUCH over the chunks, then (once the host knows how many pieces there are)
+ * fplan_scatter_kernel. */
+typedef struct FramePlanArgs {
+  const unsigned long long* starts;   /* NULL: every start is 0 (only the counts are checked) */
+  const unsigned long long* nitems;
+  long long nranges;
+  unsigned long long total_items;     /* the frame's nbytes / typesize */
+  long long ipc;                      /* items per chunk */
+  int typesize;
+  long long nchunks;
+  long long* dst;          /* [nranges] bytes of each range (0 when it fails), then its offset in dest */
+  long long* count;        /* [nchunks + 1], zeroed: +1 at each range's first chunk, -1 after its last; then pieces */
+  long long* cursor;       /* [nchunks] the first free slot of each chunk's bucket */
+  FrameTouch* touched;     /* [nchunks] the touched chunks, ascending */
+  int* pstart;             /* [npieces] first item of each piece inside its chunk */
+  int* pnitems;            /* [npieces] its items */
+  long long* pdst;         /* [npieces] its offset in dest */
+  FramePlan* rec;          /* zeroed but for rec->bad = all ones */
+  PlanScan scan[4];        /* FPLAN_DST .. FPLAN_TOUCH, at [mode - FPLAN_DST] */
+} FramePlanArgs;
+enum { FPLAN_DST = 3, FPLAN_COUNT = 4, FPLAN_BASE = 5, FPLAN_TOUCH = 6 };
 
 #ifdef __cplusplus
 }

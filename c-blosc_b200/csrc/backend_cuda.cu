@@ -395,3 +395,42 @@ extern "C" int b2_launch_plan(const PlanArgs* a, b2_stream_t s) {
   CK(cudaGetLastError());
   return 0;
 }
+
+/* the frame plan, counted as plan launches: the per-range check and the range scan, then the three chunk scans (none
+ * for a frame without chunks); the scatter is a launch of its own, made once the host has sized the piece lists */
+static unsigned range_ctas(long long n) {
+  long long ctas = (n + PLAN_THREADS - 1) / PLAN_THREADS;
+  if (ctas > (long long)num_sms() * 8) ctas = (long long)num_sms() * 8;
+  return (unsigned)ctas;
+}
+
+template <int MODE>
+static int launch_fplan_scan(const FramePlanArgs* a, long long n, b2_stream_t s) {
+  ProfScope ps(B2_K_PLAN, s->s);
+  plan_scan_kernel<MODE><<<(unsigned)((n + PLAN_TILE - 1) / PLAN_TILE), PLAN_THREADS, 0, s->s>>>(*a, n);
+  CK(cudaGetLastError());
+  return 0;
+}
+
+extern "C" int b2_launch_fplan(const FramePlanArgs* a, b2_stream_t s) {
+  if (a->nranges <= 0) return 0;
+  {
+    ProfScope ps(B2_K_PLAN, s->s);
+    fplan_check_kernel<<<range_ctas(a->nranges), PLAN_THREADS, 0, s->s>>>(*a);
+    CK(cudaGetLastError());
+  }
+  if (launch_fplan_scan<FPLAN_DST>(a, a->nranges, s)) return -1;
+  if (a->nchunks <= 0) return 0;
+  if (launch_fplan_scan<FPLAN_COUNT>(a, a->nchunks, s) || launch_fplan_scan<FPLAN_BASE>(a, a->nchunks, s) ||
+      launch_fplan_scan<FPLAN_TOUCH>(a, a->nchunks, s))
+    return -1;
+  return 0;
+}
+
+extern "C" int b2_launch_fplan_scatter(const FramePlanArgs* a, b2_stream_t s) {
+  if (a->nranges <= 0) return 0;
+  ProfScope ps(B2_K_PLAN, s->s);
+  fplan_scatter_kernel<<<range_ctas(a->nranges), PLAN_THREADS, 0, s->s>>>(*a);
+  CK(cudaGetLastError());
+  return 0;
+}

@@ -133,6 +133,8 @@ typedef struct {
   b2_buf in, filt, slots, out, csizes, needs, bstarts;
   b2_buf prev, segs, ptail;   /* segment-parallel LZ4 parse (dev_lz4fast.cuh) */
   b2_buf plan;          /* getitems planned on the GPU: its scratch */
+  b2_buf fplan, fpieces, fstage;   /* frame getitems planned on the GPU: its scratch, the piece lists and a host dest's
+                                    * staging, live while the chunk plan uses the buffers above */
   int* d_result;        /* B2_R_* words (b2_args.h): cbytes, fits, status, work-queue and done counters */
   int* h_result;        /* pinned mirror */
   unsigned queue_base;  /* tickets drawn from the B2_R_QUEUE counter so far (dev_chunk.cuh next_stream) */
@@ -166,6 +168,7 @@ static void ws_teardown(b2_ws* w) {
   buf_free(&w->in); buf_free(&w->filt); buf_free(&w->slots); buf_free(&w->out);
   buf_free(&w->csizes); buf_free(&w->needs); buf_free(&w->bstarts);
   buf_free(&w->prev); buf_free(&w->segs); buf_free(&w->ptail); buf_free(&w->plan);
+  buf_free(&w->fplan); buf_free(&w->fpieces); buf_free(&w->fstage);
   for (k = 0; k < B2_STAGE_DEPTH; k++) {
     if (w->stage[k]) b2_pinned_free(w->stage[k]);
     if (w->stage_ev[k]) b2_event_destroy(w->stage_ev[k]);
@@ -265,6 +268,7 @@ int blosc_free_resources(void) {                              /* blosc.h:411 */
     buf_free(&w->in); buf_free(&w->filt); buf_free(&w->slots); buf_free(&w->out);
     buf_free(&w->csizes); buf_free(&w->needs); buf_free(&w->bstarts);
     buf_free(&w->prev); buf_free(&w->segs); buf_free(&w->ptail); buf_free(&w->plan);
+    buf_free(&w->fplan); buf_free(&w->fpieces); buf_free(&w->fstage);
   }
   pthread_mutex_unlock(&g_ws_mutex);
   return 0;
@@ -950,11 +954,12 @@ int blosc_decompress_ctx(const void* src, void* dest, size_t destsize, int numin
   return decompress_impl(src, dest, destsize, numinternalthreads, -1, -1);
 }
 
-/* the chunk-header checks of blosc_getitem (blosc.c:1574-1631), with its return codes; 0 when the chunk is readable */
-static int getitem_header(const void* src, int src_dev, long long max_cbytes, b2_hdr* h, int* codec) {
+/* the chunk-header checks of blosc_getitem (blosc.c:1574-1631), with its return codes; 0 when the chunk is readable.
+ * A caller that holds a workspace passes it for the header's copy (NULL: one is taken when src is device memory). */
+static int getitem_header(b2_ws* w, const void* src, int src_dev, long long max_cbytes, b2_hdr* h, int* codec) {
   uint8_t hb[16];
   int rc;
-  if (copy_some(hb, 0, src, src_dev, 16)) return -1;
+  if (w ? copy_any(hb, 0, src, src_dev, 16, w->stream) : copy_some(hb, 0, src, src_dev, 16)) return -1;
   parse_header(hb, h);
   if (max_cbytes >= 0 && (h->cbytes < BLOSC_MAX_OVERHEAD || h->cbytes > max_cbytes)) return -1;
   if (h->version != BLOSC_VERSION_FORMAT) return -9;
@@ -1139,7 +1144,7 @@ static long long getitems_chunk(const void* src, long long max_cbytes, int n, co
 
   if (n <= 0) return 0;
   src_dev = b2_ptr_is_device(src);
-  rc = getitem_header(src, src_dev, max_cbytes, &h, &codec);
+  rc = getitem_header(NULL, src, src_dev, max_cbytes, &h, &codec);
   if (rc) return rc;
   tab = (GatherRange*)malloc(sizeof(GatherRange) * ((size_t)n + 1));
   lo_b = (long long*)malloc(2 * sizeof(long long) * (size_t)n);
@@ -1255,17 +1260,19 @@ static int stage_memcpyed_blocks(b2_ws* w, const b2_hdr* h, const uint8_t* hs, c
   return 0;
 }
 
-#define B2_R_PLAN 8   /* h_result words 8..13 receive the GPU plan's record (GetitemsPlan) */
+#define B2_R_PLAN 8   /* h_result words 8..15 receive a GPU plan's record (GetitemsPlan, FramePlan) */
 #define B2_AL(x) (((x) + 15) & ~(size_t)15)
 
 /* The GPU plan (dev_chunk.cuh plan_*_kernel), for range lists of which at least one is in device memory (a host one is
- * uploaded).  It builds the gather table in w->segs and the touched-block list in w->bstarts, both as the host plan
- * would (the table keeps empty ranges, which copy nothing), and the host reads back one small record.  A failing range
- * is reported by getitem_range on that range alone, so the code and the message are the host plan's.  A host chunk
- * also has the block list read back, to stage only the touched blocks. */
-static long long getitems_gpu(const void* src, int src_dev, const b2_hdr* h, int codec, int n, const int* starts,
-                              int starts_dev, const int* nitems, int nitems_dev, void* dest) {
-  const int dest_dev = b2_ptr_is_device(dest);
+ * uploaded), on the caller's workspace.  It builds the gather table in w->segs and the touched-block list in
+ * w->bstarts, both as the host plan would (the table keeps empty ranges, which copy nothing), and the host reads back
+ * one small record.  A failing range is reported by getitem_range on that range alone, so the code and the message
+ * are the host plan's.  A host chunk also has the block list read back, to stage only the touched blocks.  dsts NULL:
+ * the ranges land back to back in dest; else range r lands at dest + dsts[r] (device lists, device dest: frame
+ * pieces). */
+static long long getitems_gpu(b2_ws* w, const void* src, int src_dev, const b2_hdr* h, int codec, int n,
+                              const int* starts, int starts_dev, const int* nitems, int nitems_dev,
+                              const long long* dsts, void* dest, int dest_dev) {
   const int memcpyed = (h->flags & BLOSC_MEMCPYED) != 0, in_place = memcpyed && src_dev;
   const size_t tb = ((size_t)h->nblocks + PLAN_TILE - 1) / PLAN_TILE, tr = ((size_t)n + PLAN_TILE - 1) / PLAN_TILE;
   /* one scratch: the record, the tickets, the tile flags and the difference array, all zeroed; then the tiles' values,
@@ -1278,8 +1285,6 @@ static long long getitems_gpu(const void* src, int src_dev, const b2_hdr* h, int
   const long long at0 = 0;
   long long result = -1;
   int* hblocks = NULL;
-  b2_ws* w = ws_acquire();
-  if (!w) return -1;
   do {
     PlanArgs pa;
     GetitemsPlan rec;
@@ -1300,7 +1305,7 @@ static long long getitems_gpu(const void* src, int src_dev, const b2_hdr* h, int
     pa.nranges = n; pa.typesize = h->typesize; pa.blocksize = h->blocksize; pa.nblocks = h->nblocks;
     pa.leftover = h->leftover > 0; pa.nbytes = h->nbytes; pa.in_place = in_place;
     pa.len = (long long*)(base + o_len); pa.cover = (int*)(base + o_cover); pa.slot = (int*)(base + o_slot);
-    pa.blocks = (int*)w->bstarts.p; pa.ranges = (GatherRange*)w->segs.p; pa.rec = (GetitemsPlan*)base;
+    pa.blocks = (int*)w->bstarts.p; pa.ranges = (GatherRange*)w->segs.p; pa.rec = (GetitemsPlan*)base; pa.dsts = dsts;
     for (k = 0; k < 3; k++) {
       const size_t tiles = k < 2 ? tb : tr;
       const size_t flags_at = o_flag + 4 * (k < 2 ? k * tb : 2 * tb);
@@ -1339,13 +1344,14 @@ static long long getitems_gpu(const void* src, int src_dev, const b2_hdr* h, int
     result = getitems_run(w, h, codec, d_src, d_chunk, rec.nlisted, rec.has_left, n, rec.total, dest, dest_dev, NULL,
                           &at0, 1);
   } while (0);
-  ws_release(w);
   free(hblocks);
   return result;
 }
 
 long long blosc_b200_getitems(const void* src, int nranges, const int* starts, const int* nitems, void* dest) {
   b2_hdr h;
+  b2_ws* w;
+  long long result;
   int starts_dev, nitems_dev, src_dev, dev, codec = 0, rc;
   if (nranges <= 0) return 0;
   starts_dev = b2_ptr_is_device(starts); nitems_dev = b2_ptr_is_device(nitems);
@@ -1357,9 +1363,13 @@ long long blosc_b200_getitems(const void* src, int nranges, const int* starts, c
     fprintf(stderr, "blosc_b200: starts / nitems are not on device %d, where the call runs\n", dev);
     return -1;
   }
-  rc = getitem_header(src, src_dev, -1, &h, &codec);
+  rc = getitem_header(NULL, src, src_dev, -1, &h, &codec);
   if (rc) return rc;
-  return getitems_gpu(src, src_dev, &h, codec, nranges, starts, starts_dev, nitems, nitems_dev, dest);
+  if (!(w = ws_acquire())) return -1;
+  result = getitems_gpu(w, src, src_dev, &h, codec, nranges, starts, starts_dev, nitems, nitems_dev, NULL, dest,
+                        b2_ptr_is_device(dest));
+  ws_release(w);
+  return result;
 }
 
 /* ------------------------------------------------------------------------- */
@@ -1664,7 +1674,7 @@ static long long frame_getitems_host(const void* frame, size_t framesize, size_t
     if (ts == 0 || cs % ts) break;
     ipc = cs / ts;                                     /* items per chunk */
     for (r = 0; r < nranges; r++) {
-      if (starts[r] > nb / ts || nitems[r] > nb / ts - starts[r]) { fprintf(stderr, "`start`+`nitems` out of bounds"); break; }
+      if (b2_frame_range_bad(starts[r], nitems[r], nb / ts)) { fprintf(stderr, "`start`+`nitems` out of bounds"); break; }
       npieces += nitems[r] ? (starts[r] + nitems[r] - 1) / ipc - starts[r] / ipc + 1 : 0;
     }
     if (r < nranges) break;
@@ -1711,16 +1721,124 @@ long long blosc_b200_frame_getitem(const void* frame, size_t framesize, size_t s
   return frame_getitems_host(frame, framesize, 1, &start, &nitems, dest);
 }
 
-/* Range lists in device memory are copied to the host (one copy each), and the frame is planned there */
+/* The GPU plan of a frame (dev_chunk.cuh fplan_*_kernel), for range lists of which at least one is in device memory
+ * (a host one is uploaded).  It checks every range as frame_getitems_host does, cuts the ranges into pieces and
+ * gathers each chunk's pieces into a bucket of device piece lists; the host reads back one small record and then the
+ * list of touched chunks.  Each touched chunk, in ascending order, then runs the chunk's GPU plan on its bucket, every
+ * piece landing at its own dest offset: in dest itself when it is device memory, else in a device staging buffer that
+ * is copied to dest at the end.  Neither the lists nor the pieces travel to the host. */
+static long long frame_getitems_gpu(const void* frame, size_t framesize, size_t nranges, const size_t* starts,
+                                    int starts_dev, const size_t* nitems, int nitems_dev, void* dest) {
+  size_t nb = 0, cs = 0, nc = 0, ts = 1;
+  uint64_t* off = NULL;
+  uint8_t hb[16];
+  const int frame_dev = b2_ptr_is_device(frame), dest_dev = b2_ptr_is_device(dest);
+  FrameTouch* touched = NULL;
+  long long result = -1;
+  b2_ws* w;
+  if (frame_open(frame, framesize, &nb, &cs, &nc, &off)) return -1;
+  if (nc > 0) {                                                  /* as frame_getitems_host: the typesize of chunk 0 */
+    if (copy_some(hb, 0, (const uint8_t*)frame + off[0], frame_dev, 16)) { free(off); return -1; }
+    ts = hb[3];
+    if (ts == 0 || cs % ts) { free(off); return -1; }
+  }
+  if (nranges > ((size_t)-1) / 64 || !(w = ws_acquire())) { free(off); return -1; }
+  do {
+    /* one scratch: the record, the tickets, the tile flags and the difference array over chunks, all zeroed; then the
+     * tiles' values, the range offsets, the bucket cursors, the touched chunks and an uploaded host list */
+    const size_t tr = (nranges + PLAN_TILE - 1) / PLAN_TILE, tc = (nc + PLAN_TILE - 1) / PLAN_TILE, tiles = tr + 3 * tc;
+    const size_t o_tk = 32, o_flag = 64, o_count = B2_AL(o_flag + 4 * tiles), zeroed = B2_AL(o_count + 8 * (nc + 1));
+    const size_t o_vals = zeroed, o_dst = B2_AL(o_vals + 16 * tiles), o_cursor = B2_AL(o_dst + 8 * nranges);
+    const size_t o_touch = B2_AL(o_cursor + 8 * nc), o_up = B2_AL(o_touch + sizeof(FrameTouch) * nc);
+    FramePlanArgs fa;
+    FramePlan rec;
+    uint8_t* base;
+    uint8_t* d_dest;
+    long long sum = 0, t, done;
+    int k;
+    if (buf_ensure(&w->fplan, o_up + 8 * nranges)) break;
+    base = (uint8_t*)w->fplan.p;
+    memset(&fa, 0, sizeof fa);
+    fa.starts = (const unsigned long long*)starts; fa.nitems = (const unsigned long long*)nitems;
+    if (!starts_dev || !nitems_dev) {                                      /* the host list joins the device one */
+      if (h2d_any(w, base + o_up, starts_dev ? (const void*)nitems : (const void*)starts, 8 * nranges)) break;
+      if (starts_dev) fa.nitems = (const unsigned long long*)(base + o_up);
+      else fa.starts = (const unsigned long long*)(base + o_up);
+    }
+    if (nc == 0) fa.starts = NULL;              /* an empty frame: only the counts are looked at, as on the host */
+    if (b2_memset_dev(base, 0, zeroed, w->stream) || b2_memset_dev(base, 0xff, 8, w->stream)) break;
+    fa.nranges = (long long)nranges; fa.total_items = nb / ts; fa.ipc = (long long)(cs / ts); fa.typesize = (int)ts;
+    fa.nchunks = (long long)nc;
+    fa.dst = (long long*)(base + o_dst); fa.count = (long long*)(base + o_count); fa.cursor = (long long*)(base + o_cursor);
+    fa.touched = (FrameTouch*)(base + o_touch); fa.rec = (FramePlan*)base;
+    for (k = 0; k < 4; k++) {                           /* FPLAN_DST over the ranges, the other three over the chunks */
+      const size_t before = k == 0 ? 0 : tr + (size_t)(k - 1) * tc, width = k == 0 ? tr : tc;
+      fa.scan[k].ticket = (unsigned*)(base + o_tk) + k;
+      fa.scan[k].flag = (unsigned*)(base + o_flag) + before;
+      fa.scan[k].agg = base + o_vals + 16 * before;
+      fa.scan[k].inc = base + o_vals + 16 * before + 8 * width;
+    }
+    if (b2_launch_fplan(&fa, w->stream)) break;
+    if (b2_copy_d2h(w->h_result + B2_R_PLAN, base, sizeof rec, w->stream) || b2_stream_sync(w->stream)) break;
+    memcpy(&rec, w->h_result + B2_R_PLAN, sizeof rec);
+    if (rec.bad != ~0ull) {                                                /* frame_getitems_host's verdict */
+      if (nc > 0) fprintf(stderr, "`start`+`nitems` out of bounds");
+      break;
+    }
+    if (rec.npieces == 0) { result = 0; break; }
+    if (buf_ensure(&w->fpieces, 16 * (size_t)rec.npieces)) break;
+    fa.pdst = (long long*)w->fpieces.p; fa.pstart = (int*)(fa.pdst + rec.npieces); fa.pnitems = fa.pstart + rec.npieces;
+    if (b2_launch_fplan_scatter(&fa, w->stream)) break;
+    if (!(touched = (FrameTouch*)malloc(sizeof(FrameTouch) * (size_t)rec.ntouched))) break;
+    if (d2h_any(w, touched, base + o_touch, sizeof(FrameTouch) * (size_t)rec.ntouched)) break;
+    if (dest_dev) d_dest = (uint8_t*)dest;
+    else {
+      if (buf_ensure(&w->fstage, (size_t)rec.total + 64)) break;
+      d_dest = (uint8_t*)w->fstage.p;
+    }
+    for (t = 0; t < rec.ntouched; t++) {              /* the chunks in ascending order; the first failure decides */
+      const FrameTouch ch = touched[t];
+      const uint8_t* chunk = (const uint8_t*)frame + off[ch.chunk];
+      b2_hdr h;
+      int codec = 0, rc;
+      long long got = 0;
+      rc = getitem_header(w, chunk, frame_dev, (long long)(off[ch.chunk + 1] - off[ch.chunk]), &h, &codec);
+      if (rc) { result = rc; break; }
+      if ((size_t)h.typesize != ts) break;        /* its items are not the frame's: the pieces would not fit in dest */
+      for (done = 0; done < ch.count; done += INT_MAX) {     /* the chunk plan counts its ranges in int */
+        const int n = ch.count - done < INT_MAX ? (int)(ch.count - done) : INT_MAX;
+        const long long at = ch.base + done;
+        got = getitems_gpu(w, chunk, frame_dev, &h, codec, n, fa.pstart + at, 1, fa.pnitems + at, 1, fa.pdst + at,
+                           d_dest, 1);
+        if (got < 0) break;
+        sum += got;
+      }
+      if (got < 0) { result = got; break; }
+    }
+    if (t < rec.ntouched || sum != rec.total) break;
+    if (!dest_dev && d2h_any(w, dest, d_dest, (size_t)rec.total)) break;
+    result = rec.total;
+  } while (0);
+  ws_release(w);
+  free(touched); free(off);
+  return result;
+}
+
+/* Range lists in device memory are planned on the GPU when they are on the device the call runs on: that of the frame
+ * or of dest when either is device memory, else the current one.  Lists on another device are copied to the host (one
+ * copy each), and the frame is planned there. */
 long long blosc_b200_frame_getitems(const void* frame, size_t framesize, size_t nranges, const size_t* starts,
                                     const size_t* nitems, void* dest) {
   size_t* h = NULL;
   long long result = -1;
-  int starts_dev, nitems_dev;
+  int starts_dev, nitems_dev, dev;
   if (nranges == 0) return 0;
   if (!backend_ready()) return -1;
   starts_dev = b2_ptr_is_device(starts); nitems_dev = b2_ptr_is_device(nitems);
   if (!starts_dev && !nitems_dev) return frame_getitems_host(frame, framesize, nranges, starts, nitems, dest);
+  dev = b2_ptr_is_device(frame) ? b2_ptr_device(frame) : b2_ptr_is_device(dest) ? b2_ptr_device(dest) : b2_get_device();
+  if ((!starts_dev || b2_ptr_device(starts) == dev) && (!nitems_dev || b2_ptr_device(nitems) == dev))
+    return frame_getitems_gpu(frame, framesize, nranges, starts, starts_dev, nitems, nitems_dev, dest);
   if (nranges > ((size_t)-1) / (2 * sizeof(size_t)) || !(h = (size_t*)malloc(2 * sizeof(size_t) * nranges))) return -1;
   if (!copy_some(h, 0, starts, starts_dev, sizeof(size_t) * nranges) &&
       !copy_some(h + nranges, 0, nitems, nitems_dev, sizeof(size_t) * nranges))

@@ -14,6 +14,9 @@
  *   gather_kernel, plan_check_kernel, plan_scan_kernel
  *                   many item ranges of one chunk (blosc_b200_getitems): the copy out of
  *                   the decoded blocks, and its plan when the range lists are device memory
+ *   fplan_check_kernel, fplan_scatter_kernel (+ plan_scan_kernel)
+ *                   the same over a frame (blosc_b200_frame_getitems): the ranges cut into
+ *                   one piece list per chunk, each read by the chunk plan
  */
 #pragma once
 #include "b2_args.h"
@@ -835,11 +838,57 @@ __global__ void __launch_bounds__(PLAN_THREADS) plan_check_kernel(PlanArgs a) {
   }
 }
 
-/* The three scans of the plan, one device-wide exclusive scan each: PLAN_COVER turns the difference array into each
- * block's coverage (in place), PLAN_SLOT numbers the covered blocks and lists them, PLAN_POS makes each range's
- * position in dest from its length and writes its gather entry. */
-template <int MODE> struct PlanVal { typedef int T; };
-template <> struct PlanVal<PLAN_POS> { typedef long long T; };
+/* The frame plan (FramePlanArgs) in front of the chunk plan, for frame range lists in device memory.
+ * fplan_check_kernel, one thread per range: the frame's check (b2_frame_range_bad), the first failing index by
+ * atomicMin, each range's byte length, and its chunk interval marked in a difference array, as plan_check_kernel marks
+ * blocks.  An empty range touches no chunk. */
+__global__ void __launch_bounds__(PLAN_THREADS) fplan_check_kernel(FramePlanArgs a) {
+  const unsigned long long ipc = (unsigned long long)a.ipc;
+  for (long long r = (long long)blockIdx.x * PLAN_THREADS + threadIdx.x; r < a.nranges;
+       r += (long long)gridDim.x * PLAN_THREADS) {
+    const unsigned long long s = a.starts ? a.starts[r] : 0, n = a.nitems[r];
+    if (b2_frame_range_bad(s, n, a.total_items)) {
+      atomicMin(&a.rec->bad, (unsigned long long)r);
+      a.dst[r] = 0;
+      continue;
+    }
+    a.dst[r] = (long long)n * a.typesize;
+    if (n > 0) {
+      atomicAdd((unsigned long long*)a.count + s / ipc, 1ull);
+      atomicAdd((unsigned long long*)a.count + (s + n - 1) / ipc + 1, ~0ull);
+    }
+  }
+}
+
+/* fplan_scatter_kernel, one thread per range, once the scans have run: the range's pieces, one per chunk it touches,
+ * each into a slot of its chunk's bucket taken from the chunk's cursor.  The order inside a bucket depends on timing;
+ * every piece carries its own dest offset, so the bytes written do not. */
+__global__ void __launch_bounds__(PLAN_THREADS) fplan_scatter_kernel(FramePlanArgs a) {
+  const unsigned long long ipc = (unsigned long long)a.ipc;
+  for (long long r = (long long)blockIdx.x * PLAN_THREADS + threadIdx.x; r < a.nranges;
+       r += (long long)gridDim.x * PLAN_THREADS) {
+    const unsigned long long end = a.starts[r] + a.nitems[r];
+    long long dst = a.dst[r];
+    for (unsigned long long at = a.starts[r], c = at / ipc; at < end; c++) {
+      const unsigned long long stop = (c + 1) * ipc < end ? (c + 1) * ipc : end;
+      const long long slot = (long long)atomicAdd((unsigned long long*)a.cursor + c, 1ull);
+      a.pstart[slot] = (int)(at - c * ipc);
+      a.pnitems[slot] = (int)(stop - at);
+      a.pdst[slot] = dst;
+      dst += (long long)(stop - at) * a.typesize;
+      at = stop;
+    }
+  }
+}
+
+/* The scans of the plans, one device-wide exclusive scan each.  Chunk plan: PLAN_COVER turns the difference array into
+ * each block's coverage (in place), PLAN_SLOT numbers the covered blocks and lists them, PLAN_POS makes each range's
+ * position from its length and writes its gather entry.  Frame plan: FPLAN_DST makes each range's offset in dest from
+ * its length (in place), FPLAN_COUNT turns the difference array into each chunk's pieces (in place), FPLAN_BASE makes
+ * each chunk's bucket base (its cursor) and FPLAN_TOUCH lists the chunks with pieces. */
+template <int MODE> struct PlanVal { typedef long long T; };
+template <> struct PlanVal<PLAN_COVER> { typedef int T; };
+template <> struct PlanVal<PLAN_SLOT> { typedef int T; };
 
 template <int MODE> DEV typename PlanVal<MODE>::T plan_load(const PlanArgs& a, long long i) {
   if constexpr (MODE == PLAN_COVER) return a.cover[i];
@@ -855,7 +904,8 @@ template <int MODE, typename T> DEV void plan_store(const PlanArgs& a, long long
     if (i == n - 1) { a.rec->nlisted = excl + x; a.rec->has_left = x && a.leftover; }
   } else {
     GatherRange g;
-    g.pos = g.dst = excl;
+    g.pos = excl;
+    g.dst = a.dsts ? a.dsts[i] : excl;
     g.src = 0;
     if (x > 0) {                       /* where the range starts in the gather's source */
       const long long lo = (long long)a.starts[i] * a.typesize;
@@ -875,13 +925,39 @@ template <int MODE, typename T> DEV void plan_store(const PlanArgs& a, long long
   }
 }
 
+template <int MODE> DEV long long plan_load(const FramePlanArgs& a, long long i) {
+  if constexpr (MODE == FPLAN_DST) return a.dst[i];
+  else if constexpr (MODE == FPLAN_TOUCH) return a.count[i] > 0;
+  else return a.count[i];
+}
+
+template <int MODE, typename T> DEV void plan_store(const FramePlanArgs& a, long long i, long long n, T excl, T x) {
+  if constexpr (MODE == FPLAN_DST) {
+    a.dst[i] = excl;
+    if (i == n - 1) a.rec->total = excl + x;
+  } else if constexpr (MODE == FPLAN_COUNT) {
+    a.count[i] = excl + x;
+  } else if constexpr (MODE == FPLAN_BASE) {
+    a.cursor[i] = excl;
+    if (i == n - 1) a.rec->npieces = excl + x;
+  } else {
+    if (x) {
+      FrameTouch t;
+      t.chunk = i; t.base = a.cursor[i]; t.count = a.count[i];
+      a.touched[excl] = t;
+    }
+    if (i == n - 1) a.rec->ntouched = excl + x;
+  }
+}
+
 /* Single pass with decoupled look-back: each CTA takes the next tile (PLAN_TILE items, PLAN_ITEMS consecutive ones
  * per thread) from a counter, so the tiles before it have started; it publishes its aggregate, then warp 0 walks back
- * 32 tiles at a time, summing aggregates up to the nearest tile that has published its inclusive prefix. */
-template <int MODE>
-__global__ void __launch_bounds__(PLAN_THREADS) plan_scan_kernel(PlanArgs a, long long n) {
+ * 32 tiles at a time, summing aggregates up to the nearest tile that has published its inclusive prefix.  A is
+ * PlanArgs or FramePlanArgs, whose tile states are indexed from PLAN_COVER and FPLAN_DST. */
+template <int MODE, class A>
+__global__ void __launch_bounds__(PLAN_THREADS) plan_scan_kernel(A a, long long n) {
   typedef typename PlanVal<MODE>::T T;
-  const PlanScan& st = a.scan[MODE];
+  const PlanScan& st = a.scan[MODE < FPLAN_DST ? MODE : MODE - FPLAN_DST];
   __shared__ T s_warp[PLAN_THREADS / 32];
   __shared__ T s_prefix;
   __shared__ unsigned s_tile;
@@ -975,6 +1051,32 @@ extern "C" int b2_launch_plan(const PlanArgs* a, b2_stream_t) {
   const long long nr = a->nranges;
   simt::launch(simt::Dim3((unsigned)((nr + PLAN_TILE - 1) / PLAN_TILE)), simt::Dim3(PLAN_THREADS), 0,
                [&] { plan_scan_kernel<PLAN_POS>(args, nr); });
+  g_emu_plan_launches++;
+  return 0;
+}
+
+/* ... and of the frame plan's kernels, the same way; they count as plan launches */
+static unsigned emu_tiles(long long n) { return (unsigned)((n + PLAN_TILE - 1) / PLAN_TILE); }
+static unsigned emu_range_ctas(long long n) { return (unsigned)(n > 2 * PLAN_THREADS ? 3 : (n + PLAN_THREADS - 1) / PLAN_THREADS); }
+extern "C" int b2_launch_fplan(const FramePlanArgs* a, b2_stream_t) {
+  if (a->nranges <= 0) return 0;
+  FramePlanArgs args = *a;
+  const long long nr = a->nranges, nc = a->nchunks;
+  simt::launch(simt::Dim3(emu_range_ctas(nr)), simt::Dim3(PLAN_THREADS), 0, [&] { fplan_check_kernel(args); });
+  simt::launch(simt::Dim3(emu_tiles(nr)), simt::Dim3(PLAN_THREADS), 0, [&] { plan_scan_kernel<FPLAN_DST>(args, nr); });
+  g_emu_plan_launches += 2;
+  if (nc > 0) {
+    simt::launch(simt::Dim3(emu_tiles(nc)), simt::Dim3(PLAN_THREADS), 0, [&] { plan_scan_kernel<FPLAN_COUNT>(args, nc); });
+    simt::launch(simt::Dim3(emu_tiles(nc)), simt::Dim3(PLAN_THREADS), 0, [&] { plan_scan_kernel<FPLAN_BASE>(args, nc); });
+    simt::launch(simt::Dim3(emu_tiles(nc)), simt::Dim3(PLAN_THREADS), 0, [&] { plan_scan_kernel<FPLAN_TOUCH>(args, nc); });
+    g_emu_plan_launches += 3;
+  }
+  return 0;
+}
+extern "C" int b2_launch_fplan_scatter(const FramePlanArgs* a, b2_stream_t) {
+  if (a->nranges <= 0) return 0;
+  FramePlanArgs args = *a;
+  simt::launch(simt::Dim3(emu_range_ctas(a->nranges)), simt::Dim3(PLAN_THREADS), 0, [&] { fplan_scatter_kernel(args); });
   g_emu_plan_launches++;
   return 0;
 }

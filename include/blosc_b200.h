@@ -180,7 +180,10 @@ long long blosc_b200_frame_decompress(const void* frame, size_t framesize, void*
 long long blosc_b200_frame_getitem(const void* frame, size_t framesize, size_t start, size_t nitems, void* dest);
 /* blosc_b200_getitems over a frame: ranges may cross chunk boundaries, as in blosc_b200_frame_getitem, and are
  * written back to back into dest in request order.  Every range is checked before anything is read.  starts / nitems
- * may be host or device memory; device lists are copied to the host, where the frame is planned. */
+ * may be host or device memory.  When either is device memory and every device list is on the call's device (that of
+ * frame or dest when either is device memory, else the one chosen with blosc_b200_set_device), the frame is planned on
+ * the GPU: the ranges are cut into one piece list per chunk there, and neither list is copied to the host.  Device
+ * lists on another device are copied to the host, where the frame is planned. */
 long long blosc_b200_frame_getitems(const void* frame, size_t framesize, size_t nranges, const size_t* starts,
                                     const size_t* nitems, void* dest);
 int       blosc_b200_frame_info(const void* frame, size_t framesize, size_t* nbytes, size_t* cbytes,
