@@ -67,6 +67,10 @@ def _load(path: str) -> C.CDLL:
     lib.blosc_b200_getitems.argtypes = [vp, ci, vp, vp, vp]
     lib.blosc_b200_frame_getitems.restype = ll
     lib.blosc_b200_frame_getitems.argtypes = [vp, sz, sz, vp, vp, vp]
+    lib.blosc_b200_getslice.restype = ll
+    lib.blosc_b200_getslice.argtypes = [vp, ci, vp, vp, vp, vp]
+    lib.blosc_b200_frame_getslice.restype = ll
+    lib.blosc_b200_frame_getslice.argtypes = [vp, sz, ci, vp, vp, vp, vp]
     lib.blosc_b200_frame_info.restype = ci
     lib.blosc_b200_frame_info.argtypes = [vp, sz, C.POINTER(sz), C.POINTER(sz), C.POINTER(sz), C.POINTER(sz)]
     lib.blosc_b200_frame_chunk.restype = ll
@@ -146,6 +150,23 @@ def getitems(src, starts, nitems, dest):
     return int(lib.blosc_b200_getitems(_ptr(src), st[2], st[1], n[1], _ptr(dest)))
 
 
+def _box(shape, start, stop):
+    """shape / start / stop (sequences of ints) as three int64 host arrays of one length"""
+    import numpy as np
+    g = [np.ascontiguousarray(v, dtype=np.int64).reshape(-1) for v in (shape, start, stop)]
+    if not g[0].size == g[1].size == g[2].size:
+        raise ValueError(f"shape, start and stop have {g[0].size}, {g[1].size} and {g[2].size} entries")
+    return g
+
+
+def getslice(src, shape, start, stop, dest):
+    """A box of the C-order array of `shape` that the chunk holds (blosc_b200_getslice): items [start[k], stop[k]) of
+    each dimension, written to `dest` as one contiguous C-order array.  Returns the bytes written, or a negative code
+    (dest is then untouched)."""
+    sh, st, sp = _box(shape, start, stop)
+    return int(lib.blosc_b200_getslice(_ptr(src), sh.size, sh.ctypes.data, st.ctypes.data, sp.ctypes.data, _ptr(dest)))
+
+
 def _name(compressor):
     return compressor.encode() if isinstance(compressor, str) else compressor
 
@@ -176,6 +197,13 @@ def frame_getitems(frame, framesize, starts, nitems, dest):
     they are copied to the host for the plan)."""
     st, n = _ranges(starts, nitems, "uint64", ("torch.int64", "torch.uint64"))
     return int(lib.blosc_b200_frame_getitems(_ptr(frame), framesize, st[2], st[1], n[1], _ptr(dest)))
+
+
+def frame_getslice(frame, framesize, shape, start, stop, dest):
+    """getslice over the array a frame holds (blosc_b200_frame_getslice); the box may cross chunk boundaries."""
+    sh, st, sp = _box(shape, start, stop)
+    return int(lib.blosc_b200_frame_getslice(_ptr(frame), framesize, sh.size, sh.ctypes.data, st.ctypes.data,
+                                             sp.ctypes.data, _ptr(dest)))
 
 
 def frame_info(frame, framesize):

@@ -279,6 +279,133 @@ typedef struct FramePlanArgs {
 } FramePlanArgs;
 enum { FPLAN_DST = 3, FPLAN_COUNT = 4, FPLAN_BASE = 5, FPLAN_TOUCH = 6 };
 
+/* A box of an N-d C-order array (blosc_b200_getslice): items [start[k], stop[k]) of each dimension, none of them empty.
+ * The host builds it after merging every dimension whose box covers its whole extent into the dimension before it, so
+ * the innermost run of consecutive flat items is as long as the box allows.  Its arithmetic is the three functions
+ * below, shared by the host (which touched chunks, where their output starts) and the kernels (which blocks a chunk's
+ * part touches, where each output byte comes from).  Every loop runs over the fixed B2_BOX_MAXDIM with a guard, so the
+ * kernels index the box with constants only. */
+#define B2_BOX_MAXDIM 8
+typedef struct B2Box {
+  int ndim;                           /* dimensions after merging, 1..B2_BOX_MAXDIM */
+  int pad;
+  long long start[B2_BOX_MAXDIM];
+  long long stop[B2_BOX_MAXDIM];
+  long long stride[B2_BOX_MAXDIM];    /* flat items per step of dimension k: the product of the shape after k */
+  long long inner[B2_BOX_MAXDIM];     /* box items per step of dimension k: the product of the extents after k */
+  long long run;                      /* items of one innermost run: the extent of the last dimension */
+  long long nitems;                   /* items of the whole array: b2_box_next's end sentinel */
+  long long count;                    /* items of the box */
+} B2Box;
+
+/* a / b for a >= 0, b > 0.  On the device it makes no call to the 64-bit division routine, whose saved registers
+ * would spill in the box kernels: a 32-bit division when both fit, else a double estimate refined once in double and
+ * corrected by one in exact integer arithmetic (the remainders are below 2^63, so the unsigned products are exact). */
+static inline B2_HD long long b2_box_div(long long a, long long b) {
+#ifdef __CUDA_ARCH__
+  long long q, r;
+  if ((((unsigned long long)a | (unsigned long long)b) >> 32) == 0) return (long long)((unsigned)a / (unsigned)b);
+  q = (long long)((double)a / (double)b);
+  r = (long long)((unsigned long long)a - (unsigned long long)q * (unsigned long long)b);
+  q += (long long)((double)r / (double)b);
+  r = (long long)((unsigned long long)a - (unsigned long long)q * (unsigned long long)b);
+  return r < 0 ? q - 1 : r >= b ? q + 1 : q;
+#else
+  return a / b;
+#endif
+}
+
+/* The smallest flat index >= x (0 <= x <= nitems) that lies in the box; nitems when there is none */
+static inline B2_HD long long b2_box_next(const B2Box* b, long long x) {
+  long long c[B2_BOX_MAXDIM], r = x, v = 0;
+  int k, bad = -1, below = 0, p = -1;
+#pragma unroll
+  for (k = 0; k < B2_BOX_MAXDIM; k++) {
+    c[k] = 0;
+    if (k < b->ndim) {
+      c[k] = b2_box_div(r, b->stride[k]);
+      r -= c[k] * b->stride[k];
+      if (bad < 0 && (c[k] < b->start[k] || c[k] >= b->stop[k])) { bad = k; below = c[k] < b->start[k]; }
+    }
+  }
+  if (bad < 0) return x;
+  if (below) {                      /* dimension `bad` moves up to its start, the ones after it to theirs */
+    p = bad;
+#pragma unroll
+    for (k = 0; k < B2_BOX_MAXDIM; k++) if (k == bad) v = b->start[k];
+  } else {                          /* past the box in `bad`: carry into the last dimension before it that has room */
+#pragma unroll
+    for (k = B2_BOX_MAXDIM - 1; k >= 0; k--)
+      if (p < 0 && k < bad && c[k] + 1 < b->stop[k]) { p = k; v = c[k] + 1; }
+    if (p < 0) return b->nitems;
+  }
+  r = 0;
+#pragma unroll
+  for (k = 0; k < B2_BOX_MAXDIM; k++)
+    if (k < b->ndim) r += (k < p ? c[k] : k == p ? v : b->start[k]) * b->stride[k];
+  return r;
+}
+
+/* How many box items have a flat index < x (0 <= x <= nitems) */
+static inline B2_HD long long b2_box_rank(const B2Box* b, long long x) {
+  long long r = x, rank = 0;
+  int k;
+#pragma unroll
+  for (k = 0; k < B2_BOX_MAXDIM; k++) {
+    if (k < b->ndim) {
+      const long long c = b2_box_div(r, b->stride[k]);
+      r -= c * b->stride[k];
+      if (c < b->start[k]) return rank;
+      if (c >= b->stop[k]) return rank + (b->stop[k] - b->start[k]) * b->inner[k];
+      rank += (c - b->start[k]) * b->inner[k];
+    }
+  }
+  return rank;
+}
+
+/* The flat index of box item p (0 <= p < count, C order inside the box) */
+static inline B2_HD long long b2_box_unrank(const B2Box* b, long long p) {
+  long long f = 0;
+  int k;
+#pragma unroll
+  for (k = B2_BOX_MAXDIM - 1; k >= 0; k--) {
+    if (k < b->ndim) {
+      long long q = p;
+      if (k > 0) {
+        const long long e = b->stop[k] - b->start[k];
+        p = b2_box_div(p, e);
+        q -= p * e;
+      }
+      f += (b->start[k] + q) * b->stride[k];
+    }
+  }
+  return f;
+}
+
+/* The plan of one chunk's part of a box: box_touch_kernel marks in plan.cover every block that holds a byte of it, then
+ * the PLAN_SLOT scan of the getitems plan (plan.cover, slot, blocks, rec, leftover, scan[PLAN_SLOT]) lists them.  The
+ * chunk holds the array's flat items [window, window + nbytes / typesize). */
+typedef struct BoxPlanArgs {
+  B2Box box;
+  long long window;
+  PlanArgs plan;
+} BoxPlanArgs;
+
+/* box_gather_kernel: box items [p0, p0 + total / typesize) in C order, all inside the chunk's window, to dst.  slot
+ * NULL: src is the chunk's bytes in place (a memcpyed payload); else block b of the chunk is at src + slot[b] *
+ * blocksize (the compact scratch of the listed blocks). */
+typedef struct BoxGatherArgs {
+  B2Box box;
+  long long window;
+  long long p0;
+  long long total;            /* bytes to write */
+  int typesize, blocksize;
+  const int* slot;
+  const uint8_t* src;
+  uint8_t* dst;
+  const int* status;          /* NULL, or the decode verdict: the gather writes nothing when it is negative */
+} BoxGatherArgs;
+
 #ifdef __cplusplus
 }
 #endif

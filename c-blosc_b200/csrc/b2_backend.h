@@ -59,6 +59,9 @@ int  b2_launch_plan(const PlanArgs* a, b2_stream_t s);      /* plan_check_kernel
 int  b2_launch_fplan(const FramePlanArgs* a, b2_stream_t s);           /* fplan_check_kernel + plan_scan_kernel x 2
                                                                         * (x 4 when the frame has chunks) */
 int  b2_launch_fplan_scatter(const FramePlanArgs* a, b2_stream_t s);   /* fplan_scatter_kernel: the piece lists */
+int  b2_launch_box_plan(const BoxPlanArgs* a, b2_stream_t s);          /* box_touch_kernel + plan_scan_kernel<PLAN_SLOT>:
+                                                                        * the blocks a chunk's part of a box touches */
+int  b2_launch_box_gather(const BoxGatherArgs* a, b2_stream_t s);      /* box_gather_kernel (getslice) */
 
 /* profiling: per-kernel-kind CUDA-event timing (off by default) */
 enum { B2_K_FILTER = 0, B2_K_ENCODE, B2_K_SCAN, B2_K_COMPACT, B2_K_DECODE, B2_K_UNFILTER, B2_K_INDEX, B2_K_PARSE, B2_K_ZENC, B2_K_DENC, B2_K_SENC, B2_K_GATHER, B2_K_PLAN, B2_K_COUNT };

@@ -434,3 +434,30 @@ extern "C" int b2_launch_fplan_scatter(const FramePlanArgs* a, b2_stream_t s) {
   CK(cudaGetLastError());
   return 0;
 }
+
+/* the box plan of getslice, counted as plan launches: box_touch_kernel, one thread per block, then the PLAN_SLOT scan of
+ * the getitems plan over the blocks */
+extern "C" int b2_launch_box_plan(const BoxPlanArgs* a, b2_stream_t s) {
+  const long long nb = a->plan.nblocks;
+  if (nb <= 0) return 0;
+  {
+    ProfScope ps(B2_K_PLAN, s->s);
+    box_touch_kernel<<<(unsigned)((nb + PLAN_THREADS - 1) / PLAN_THREADS), PLAN_THREADS, 0, s->s>>>(*a);
+    CK(cudaGetLastError());
+  }
+  ProfScope ps(B2_K_PLAN, s->s);
+  plan_scan_kernel<PLAN_SLOT><<<(unsigned)((nb + PLAN_TILE - 1) / PLAN_TILE), PLAN_THREADS, 0, s->s>>>(a->plan, nb);
+  CK(cudaGetLastError());
+  return 0;
+}
+
+/* the box gather of getslice, counted as a gather launch */
+extern "C" int b2_launch_box_gather(const BoxGatherArgs* a, b2_stream_t s) {
+  if (a->total <= 0) return 0;
+  long long ctas = (a->total + (long long)GATHER_WARPS * GATHER_SPAN - 1) / ((long long)GATHER_WARPS * GATHER_SPAN);
+  if (ctas > (long long)num_sms() * 8) ctas = (long long)num_sms() * 8;
+  ProfScope ps(B2_K_GATHER, s->s);
+  box_gather_kernel<<<(unsigned)ctas, GATHER_WARPS * 32, 0, s->s>>>(*a);
+  CK(cudaGetLastError());
+  return 0;
+}

@@ -12,6 +12,7 @@
 #include "../../include/blosc_b200.h"
 
 #include <errno.h>
+#include <limits.h>
 #include <pthread.h>
 #include <stdio.h>
 #include <stdlib.h>
@@ -1373,6 +1374,185 @@ long long blosc_b200_getitems(const void* src, int nranges, const int* starts, c
 }
 
 /* ------------------------------------------------------------------------- */
+/* boxes of an N-d array (blosc_b200_getslice, blosc_b200_frame_getslice)     */
+/* ------------------------------------------------------------------------- */
+/* A box needs no list of its runs: the blocks it touches and the source of every output byte follow from the box
+ * itself (B2Box, b2_args.h).  A chunk's part of a box is planned by box_touch_kernel and the PLAN_SLOT scan, its
+ * touched blocks are decoded and unfiltered into the compact scratch as getitems decodes them, and box_gather_kernel
+ * writes it: a fixed number of launches, one record read-back and one status sync, whatever the number of runs. */
+
+/* The checks that need no chunk: ndim, the shape and its product (*nitems), the box inside the shape.  -1 with a
+ * message when one fails. */
+static int box_geometry(int ndim, const int64_t* shape, const int64_t* start, const int64_t* stop, long long* nitems) {
+  long long prod = 1;
+  int k, zero = 0;
+  if (ndim < 1 || ndim > B2_BOX_MAXDIM) {
+    fprintf(stderr, "blosc_b200: ndim %d is not in 1..%d\n", ndim, B2_BOX_MAXDIM);
+    return -1;
+  }
+  for (k = 0; k < ndim; k++) {
+    if (shape[k] < 0) { fprintf(stderr, "blosc_b200: shape[%d] = %lld is negative\n", k, (long long)shape[k]); return -1; }
+    zero |= shape[k] == 0;
+  }
+  for (k = 0; k < ndim && !zero; k++) {
+    if (prod > LLONG_MAX / shape[k]) { fprintf(stderr, "blosc_b200: the product of the shape overflows int64\n"); return -1; }
+    prod *= shape[k];
+  }
+  for (k = 0; k < ndim; k++)
+    if (start[k] < 0 || start[k] > stop[k] || stop[k] > shape[k]) {
+      fprintf(stderr, "blosc_b200: box [%lld, %lld) of dimension %d is not inside [0, %lld)\n", (long long)start[k],
+              (long long)stop[k], k, (long long)shape[k]);
+      return -1;
+    }
+  *nitems = zero ? 0 : prod;
+  return 0;
+}
+
+/* the array's items times the typesize against the bytes that hold it; -1 with a message when they differ */
+static int box_nbytes(long long nitems, long long typesize, unsigned long long nbytes) {
+  if (nbytes % (unsigned long long)typesize || nbytes / (unsigned long long)typesize != (unsigned long long)nitems) {
+    fprintf(stderr, "blosc_b200: %lld items of %lld bytes are not the %llu bytes of the data\n", nitems, typesize, nbytes);
+    return -1;
+  }
+  return 0;
+}
+
+static int box_empty(int ndim, const int64_t* start, const int64_t* stop) {
+  int k;
+  for (k = 0; k < ndim; k++) if (start[k] == stop[k]) return 1;
+  return 0;
+}
+
+/* The canonical box of a non-empty, checked one: every dimension that the box covers whole is merged into the one
+ * before it, so the innermost run is as long as it can be. */
+static void box_build(int ndim, const int64_t* shape, const int64_t* start, const int64_t* stop, long long nitems,
+                      B2Box* b) {
+  long long sh[B2_BOX_MAXDIM];
+  int k, n = 0;
+  memset(b, 0, sizeof *b);
+  for (k = 0; k < ndim; k++) {
+    if (n > 0 && start[k] == 0 && stop[k] == shape[k]) {
+      sh[n - 1] *= shape[k]; b->start[n - 1] *= shape[k]; b->stop[n - 1] *= shape[k];
+    } else {
+      sh[n] = shape[k]; b->start[n] = start[k]; b->stop[n] = stop[k];
+      n++;
+    }
+  }
+  b->ndim = n;
+  b->stride[n - 1] = 1; b->inner[n - 1] = 1;
+  for (k = n - 2; k >= 0; k--) {
+    b->stride[k] = b->stride[k + 1] * sh[k + 1];
+    b->inner[k] = b->inner[k + 1] * (b->stop[k + 1] - b->start[k + 1]);
+  }
+  b->run = b->stop[n - 1] - b->start[n - 1];
+  b->count = b->inner[0] * (b->stop[0] - b->start[0]);
+  b->nitems = nitems;
+}
+
+/* One chunk's part of a box: the chunk (header h, checked) holds the array's flat items [window, window + nbytes /
+ * typesize); the box items among them land, in C order, at d_dst (device memory).  Returns the bytes written, blosc_d's
+ * code when a touched block fails to decode (nothing is written then), or -1. */
+static long long getslice_chunk(b2_ws* w, const void* src, int src_dev, const b2_hdr* h, int codec, const B2Box* box,
+                                long long window, uint8_t* d_dst) {
+  const int memcpyed = (h->flags & BLOSC_MEMCPYED) != 0;
+  const long long ts = h->typesize, p0 = b2_box_rank(box, window);
+  const long long total = (b2_box_rank(box, window + h->nbytes / ts) - p0) * ts;
+  /* the plan's scratch: the record, the ticket and the tile flags, zeroed; then the tiles' values, cover and slot */
+  const size_t tb = ((size_t)h->nblocks + PLAN_TILE - 1) / PLAN_TILE;
+  const size_t o_tk = 32, o_flag = 64, zeroed = B2_AL(o_flag + 4 * tb), o_vals = zeroed;
+  const size_t o_cover = B2_AL(o_vals + 8 * tb), o_slot = B2_AL(o_cover + 4 * (size_t)h->nblocks);
+  BoxGatherArgs ga;
+  int* hblocks = NULL;
+  long long result = -1;
+  if (total == 0) return 0;
+  memset(&ga, 0, sizeof ga);
+  ga.box = *box; ga.window = window; ga.p0 = p0; ga.total = total;
+  ga.typesize = h->typesize; ga.blocksize = h->blocksize; ga.dst = d_dst;
+  do {
+    if (memcpyed && src_dev) ga.src = (const uint8_t*)src + 16;            /* the payload, read in place: no plan */
+    else {
+      BoxPlanArgs bp;
+      GetitemsPlan rec;
+      uint8_t* base;
+      const uint8_t* d_chunk = (const uint8_t*)src;
+      if (buf_ensure(&w->plan, o_slot + 4 * (size_t)h->nblocks) || buf_ensure(&w->bstarts, 4 * (size_t)h->nblocks + 64))
+        break;
+      base = (uint8_t*)w->plan.p;
+      if (b2_memset_dev(base, 0, zeroed, w->stream)) break;
+      memset(&bp, 0, sizeof bp);
+      bp.box = *box; bp.window = window;
+      bp.plan.typesize = h->typesize; bp.plan.blocksize = h->blocksize; bp.plan.nblocks = h->nblocks;
+      bp.plan.leftover = h->leftover > 0; bp.plan.nbytes = h->nbytes;
+      bp.plan.cover = (int*)(base + o_cover); bp.plan.slot = (int*)(base + o_slot);
+      bp.plan.blocks = (int*)w->bstarts.p; bp.plan.rec = (GetitemsPlan*)base;
+      bp.plan.scan[PLAN_SLOT].ticket = (unsigned*)(base + o_tk);
+      bp.plan.scan[PLAN_SLOT].flag = (unsigned*)(base + o_flag);
+      bp.plan.scan[PLAN_SLOT].agg = base + o_vals;
+      bp.plan.scan[PLAN_SLOT].inc = base + o_vals + 4 * tb;
+      if (b2_launch_box_plan(&bp, w->stream)) break;
+      if (b2_copy_d2h(w->h_result + B2_R_PLAN, base, sizeof rec, w->stream) || b2_stream_sync(w->stream)) break;
+      memcpy(&rec, w->h_result + B2_R_PLAN, sizeof rec);
+      ga.slot = bp.plan.slot;
+      if (!src_dev) {                                                      /* stage the touched blocks only */
+        if (!(hblocks = (int*)malloc(4 * (size_t)rec.nlisted))) break;
+        if (d2h_any(w, hblocks, w->bstarts.p, 4 * (size_t)rec.nlisted)) break;
+        if (memcpyed ? stage_memcpyed_blocks(w, h, (const uint8_t*)src, hblocks, rec.nlisted)
+                     : stage_blocks(w, h, (const uint8_t*)src, hblocks, rec.nlisted))
+          break;
+        d_chunk = (const uint8_t*)w->in.p;
+      }
+      if (memcpyed) ga.src = d_chunk;                  /* a host payload: listed block j staged at j * blocksize */
+      else {
+        if (buf_ensure(&w->out, (size_t)rec.nlisted * (size_t)h->blocksize + 64)) break;
+        if (launch_decode_blocks(w, h, codec, d_chunk, 0, rec.nlisted, (const int*)w->bstarts.p, rec.has_left,
+                                 (uint8_t*)w->out.p))
+          break;
+        ga.src = (const uint8_t*)w->out.p;
+        ga.status = w->d_result + B2_R_STATUS_OUT;
+      }
+    }
+    if (b2_launch_box_gather(&ga, w->stream)) { ws_reset_counters(w); break; }
+    if (b2_copy_d2h(w->h_result + B2_R_STATUS_OUT, w->d_result + B2_R_STATUS_OUT, 4, w->stream) || b2_stream_sync(w->stream)) {
+      ws_reset_counters(w);
+      break;
+    }
+    if (ga.status && w->h_result[B2_R_STATUS_OUT] < 0) { result = w->h_result[B2_R_STATUS_OUT]; break; }
+    result = total;
+  } while (0);
+  free(hblocks);
+  return result;
+}
+
+long long blosc_b200_getslice(const void* src, int ndim, const int64_t* shape, const int64_t* start,
+                              const int64_t* stop, void* dest) {
+  b2_hdr h;
+  B2Box box;
+  b2_ws* w;
+  long long nitems = 0, result = -1;
+  int src_dev, dest_dev, codec = 0, rc;
+  if (box_geometry(ndim, shape, start, stop, &nitems)) return -1;
+  src_dev = b2_ptr_is_device(src);
+  rc = getitem_header(NULL, src, src_dev, -1, &h, &codec);
+  if (rc) return rc;
+  if (box_nbytes(nitems, h.typesize, (unsigned long long)h.nbytes)) return -1;
+  if (box_empty(ndim, start, stop)) return 0;
+  box_build(ndim, shape, start, stop, nitems, &box);
+  dest_dev = b2_ptr_is_device(dest);
+  if (!(w = ws_acquire())) return -1;
+  do {                                                 /* a host dest: staged in device memory, copied out once */
+    uint8_t* d_dst = (uint8_t*)dest;
+    if (!dest_dev) {
+      if (buf_ensure(&w->slots, (size_t)(box.count * h.typesize) + 64)) break;
+      d_dst = (uint8_t*)w->slots.p;
+    }
+    result = getslice_chunk(w, src, src_dev, &h, codec, &box, 0, d_dst);
+    if (result > 0 && !dest_dev && d2h_any(w, dest, d_dst, (size_t)result)) result = -1;
+  } while (0);
+  ws_release(w);
+  return result;
+}
+
+/* ------------------------------------------------------------------------- */
 /* frames: buffers larger than one chunk (SURVEY.md section 8, row f3)           */
 /* ------------------------------------------------------------------------- */
 /* A Blosc-1 chunk holds at most INT_MAX-16 bytes (blosc.h:40) and a single call leaves most of
@@ -1844,6 +2024,72 @@ long long blosc_b200_frame_getitems(const void* frame, size_t framesize, size_t 
       !copy_some(h + nranges, 0, nitems, nitems_dev, sizeof(size_t) * nranges))
     result = frame_getitems_host(frame, framesize, nranges, h, h + nranges, dest);
   free(h);
+  return result;
+}
+
+/* A box of the array a frame holds, in items of chunk 0's typesize: the touched chunks and where each one's part lands
+ * in dest follow from the box (b2_box_next, b2_box_rank on the chunks' item windows), and each touched chunk, in
+ * ascending order, is read by the chunk path; the first failure decides the result.  A host dest is staged in device
+ * memory and copied out once, so it is untouched on a failure. */
+long long blosc_b200_frame_getslice(const void* frame, size_t framesize, int ndim, const int64_t* shape,
+                                    const int64_t* start, const int64_t* stop, void* dest) {
+  size_t nb = 0, cs = 0, nc = 0, c;
+  uint64_t* off = NULL;
+  uint8_t hb[16];
+  long long nitems = 0, ts = 1, ipc, sum = 0, got = 0, result = -1;
+  int frame_dev, dest_dev;
+  B2Box box;
+  b2_ws* w;
+  if (!backend_ready()) return -1;
+  if (box_geometry(ndim, shape, start, stop, &nitems)) return -1;
+  if (frame_open(frame, framesize, &nb, &cs, &nc, &off)) return -1;
+  frame_dev = b2_ptr_is_device(frame);
+  dest_dev = b2_ptr_is_device(dest);
+  if (nc > 0) {                                              /* as frame_getitems: the typesize of chunk 0 */
+    if (copy_some(hb, 0, (const uint8_t*)frame + off[0], frame_dev, 16)) { free(off); return -1; }
+    ts = hb[3];
+    if (ts == 0 || cs % (size_t)ts) {
+      fprintf(stderr, "blosc_b200: chunk 0's typesize %lld does not divide the frame's chunksize\n", ts);
+      free(off);
+      return -1;
+    }
+  }
+  if (box_nbytes(nitems, ts, (unsigned long long)nb)) { free(off); return -1; }
+  if (box_empty(ndim, start, stop)) { free(off); return 0; }
+  box_build(ndim, shape, start, stop, nitems, &box);
+  ipc = (long long)cs / ts;
+  if (!(w = ws_acquire())) { free(off); return -1; }
+  do {
+    uint8_t* d_dst = (uint8_t*)dest;
+    if (!dest_dev) {
+      if (buf_ensure(&w->fstage, (size_t)(box.count * ts) + 64)) break;
+      d_dst = (uint8_t*)w->fstage.p;
+    }
+    for (c = 0; c < nc; c++) {
+      const long long w0 = (long long)c * ipc, w1 = w0 + ipc < nitems ? w0 + ipc : nitems;
+      const uint8_t* chunk = (const uint8_t*)frame + off[c];
+      b2_hdr h;
+      int codec = 0;
+      if (b2_box_next(&box, w0) >= w1) continue;                          /* no box item in this chunk */
+      got = getitem_header(w, chunk, frame_dev, (long long)(off[c + 1] - off[c]), &h, &codec);
+      if (got) break;
+      if (h.typesize != ts || h.nbytes != (w1 - w0) * ts) {
+        fprintf(stderr, "blosc_b200: chunk %zu holds %d items of %d bytes, not the frame's %lld of %lld\n", c,
+                h.nbytes / h.typesize, h.typesize, w1 - w0, ts);
+        got = -1;
+        break;
+      }
+      got = getslice_chunk(w, chunk, frame_dev, &h, codec, &box, w0, d_dst + b2_box_rank(&box, w0) * ts);
+      if (got < 0) break;
+      sum += got;
+    }
+    if (c < nc) { result = got; break; }
+    if (sum != box.count * ts) break;
+    if (!dest_dev && d2h_any(w, dest, d_dst, (size_t)sum)) break;
+    result = sum;
+  } while (0);
+  ws_release(w);
+  free(off);
   return result;
 }
 

@@ -17,6 +17,9 @@
  *   fplan_check_kernel, fplan_scatter_kernel (+ plan_scan_kernel)
  *                   the same over a frame (blosc_b200_frame_getitems): the ranges cut into
  *                   one piece list per chunk, each read by the chunk plan
+ *   box_touch_kernel, box_gather_kernel (+ plan_scan_kernel<PLAN_SLOT>)
+ *                   a box of an N-d array (blosc_b200_getslice): the touched blocks and the
+ *                   copy out of them, both from the box alone (B2Box, b2_args.h)
  */
 #pragma once
 #include "b2_args.h"
@@ -1081,6 +1084,100 @@ extern "C" int b2_launch_fplan_scatter(const FramePlanArgs* a, b2_stream_t) {
   return 0;
 }
 extern "C" int b2_ptr_device(const void*) { return 0; }
+#endif
+
+
+/* blosc_b200_getslice: a box of an N-d array (B2Box), planned and gathered from the box alone, with no per-run state.
+ * box_touch_kernel, one thread per block of the chunk: the block is touched when some box item has a byte in it.  The
+ * test is on bytes, so it holds when the blocksize is not a multiple of the typesize. */
+__global__ void __launch_bounds__(PLAN_THREADS) box_touch_kernel(BoxPlanArgs a) {
+  const long long ts = a.plan.typesize, bs = a.plan.blocksize;
+  for (long long b = (long long)blockIdx.x * PLAN_THREADS + threadIdx.x; b < a.plan.nblocks;
+       b += (long long)gridDim.x * PLAN_THREADS) {
+    const long long lo = b * bs, hi = lo + bs < a.plan.nbytes ? lo + bs : a.plan.nbytes;
+    a.plan.cover[b] = b2_box_next(&a.box, a.window + b2_box_div(lo, ts)) < a.window + b2_box_div(hi + ts - 1, ts);
+  }
+}
+
+/* box_gather_kernel: output-driven like gather_kernel, warp job k covering output bytes [k * GATHER_SPAN, (k + 1) *
+ * GATHER_SPAN).  Runs of BOX_SHORT_RUN bytes or more are copied by the whole warp, one run piece at a time, each piece
+ * cut at block edges.  Shorter runs are copied by one lane each: lane l takes every 32nd run that starts in the job's
+ * bytes (the job of byte 0 also takes the run that the chunk's part starts inside), so no run is split between two
+ * lanes.  Either way a run's source is the unrank of its first item. */
+#define BOX_SHORT_RUN 64
+__global__ void __launch_bounds__(GATHER_WARPS * 32) box_gather_kernel(BoxGatherArgs a) {
+  if (a.status && ld_cg_i32(a.status) < 0) return;       /* a stream failed to decode: dest stays untouched */
+  const long long ts = a.typesize, runb = a.box.run * ts, g0 = a.p0 * ts, end = g0 + a.total;
+  const unsigned bs = (unsigned)a.blocksize;              /* chunk offsets are below 2^31 */
+  const int lane = lane_id();
+  const long long warps = (long long)gridDim.x * GATHER_WARPS;
+  for (long long lo = ((long long)blockIdx.x * GATHER_WARPS + (threadIdx.x >> 5)) * GATHER_SPAN; lo < a.total;
+       lo += warps * GATHER_SPAN) {
+    const long long hi = lo + GATHER_SPAN < a.total ? lo + GATHER_SPAN : a.total;
+    if (runb >= BOX_SHORT_RUN) {
+      for (long long o = lo; o < hi;) {
+        const long long g = g0 + o, k = b2_box_div(g, runb), u = g - k * runb;
+        unsigned s = (unsigned)((b2_box_unrank(&a.box, k * a.box.run) - a.window) * ts + u);
+        long long n = runb - u < hi - o ? runb - u : hi - o;
+        while (n > 0) {
+          int m = (int)n;
+          const u8* from = a.src + s;
+          if (a.slot) {
+            const unsigned blk = s / bs, left = (blk + 1) * bs - s;
+            if ((unsigned)m > left) m = (int)left;
+            from = a.src + (long long)a.slot[blk] * bs + (s - blk * bs);
+          }
+          warp_copy_vec(a.dst + o, from, m);
+          o += m; s += (unsigned)m; n -= m;
+        }
+      }
+    } else {
+      const long long ka = b2_box_div(lo == 0 ? g0 : g0 + lo + runb - 1, runb), kb = b2_box_div(g0 + hi + runb - 1, runb);
+      for (long long k = ka + lane; k < kb; k += 32) {
+        const long long gs = k * runb > g0 ? k * runb : g0, ge = (k + 1) * runb < end ? (k + 1) * runb : end;
+        unsigned s = (unsigned)((b2_box_unrank(&a.box, k * a.box.run) - a.window) * ts + (gs - k * runb));
+        u8* out = a.dst + (gs - g0);
+        const int n = (int)(ge - gs);
+        if (!a.slot) {
+          for (int x = 0; x < n; x++) out[x] = a.src[s + x];
+        } else {
+          unsigned bend = 0;
+          const u8* base = a.src;
+          for (int x = 0; x < n; x++, s++) {
+            if (s >= bend) {
+              const unsigned blk = s / bs;
+              bend = (blk + 1) * bs;
+              base = a.src + (long long)a.slot[blk] * bs - (long long)blk * bs;
+            }
+            out[x] = base[s];
+          }
+        }
+      }
+    }
+  }
+}
+
+#ifdef SIMT_EMU
+/* The emulator's launchers of the box kernels: a few CTAs each, so that the grid-stride loops run.  The plan's two
+ * launches count as plan launches, the gather as a gather launch. */
+extern "C" int b2_launch_box_plan(const BoxPlanArgs* a, b2_stream_t) {
+  if (a->plan.nblocks <= 0) return 0;
+  BoxPlanArgs args = *a;
+  const long long nb = a->plan.nblocks;
+  simt::launch(simt::Dim3(emu_range_ctas(nb)), simt::Dim3(PLAN_THREADS), 0, [&] { box_touch_kernel(args); });
+  simt::launch(simt::Dim3(emu_tiles(nb)), simt::Dim3(PLAN_THREADS), 0, [&] { plan_scan_kernel<PLAN_SLOT>(args.plan, nb); });
+  g_emu_plan_launches += 2;
+  return 0;
+}
+extern "C" int b2_launch_box_gather(const BoxGatherArgs* a, b2_stream_t) {
+  if (a->total <= 0) return 0;
+  long long ctas = (a->total + (long long)GATHER_WARPS * GATHER_SPAN - 1) / ((long long)GATHER_WARPS * GATHER_SPAN);
+  if (ctas > 3) ctas = 3;
+  g_emu_gather_launches++;
+  BoxGatherArgs args = *a;
+  simt::launch(simt::Dim3((unsigned)ctas), simt::Dim3(GATHER_WARPS * 32), 0, [&] { box_gather_kernel(args); });
+  return 0;
+}
 #endif
 
 

@@ -162,6 +162,20 @@ int blosc_b200_filter(int mode, size_t typesize, size_t blocksize, const void* s
  * other non-blocking streams must be synchronised first, as src must. */
 long long blosc_b200_getitems(const void* src, int nranges, const int* starts, const int* nitems, void* dest);
 
+/* A box of an N-d array in one call.  The chunk holds a C-order array of `shape` (ndim entries, 1..8) in items of the
+ * chunk's typesize; items [start[k], stop[k]) of each dimension k are written to dest as one contiguous C-order array
+ * of extents stop - start (numpy: a[start[0]:stop[0], ..., start[ndim-1]:stop[ndim-1]], made contiguous).  shape /
+ * start / stop are host memory; src / dest are host or device memory, and the call runs on the device getitems would
+ * use.  Only the blocks that hold a byte of the box are decoded, and the read is planned on the GPU from the box
+ * alone: the launches do not grow with the number of innermost runs.  Returns the bytes written, prod(stop - start) *
+ * typesize; 0 for an empty box, with nothing launched.  -1 with a message on stderr, before anything is launched or
+ * written, when ndim is not in 1..8, a shape entry is negative or their product overflows int64, the product times the
+ * typesize is not the chunk's nbytes, or start[k] > stop[k] or stop[k] > shape[k] (or start[k] < 0).  The chunk header
+ * is checked as blosc_getitem checks it, with its codes.  A touched block that fails to decode returns blosc_d's code
+ * and leaves dest untouched. */
+long long blosc_b200_getslice(const void* src, int ndim, const int64_t* shape, const int64_t* start,
+                              const int64_t* stop, void* dest);
+
 /* Frames: buffers larger than one chunk (a Blosc-1 chunk holds at most BLOSC_MAX_BUFFERSIZE
  * bytes, blosc.h:40).  The buffer is cut into `chunksize`-byte pieces (0 = 256 MiB; rounded down
  * to a multiple of typesize), each compressed exactly as blosc_compress_ctx() would with
@@ -186,6 +200,14 @@ long long blosc_b200_frame_getitem(const void* frame, size_t framesize, size_t s
  * lists on another device are copied to the host, where the frame is planned. */
 long long blosc_b200_frame_getitems(const void* frame, size_t framesize, size_t nranges, const size_t* starts,
                                     const size_t* nitems, void* dest);
+/* blosc_b200_getslice over a frame: the whole frame holds the C-order array, in items of chunk 0's typesize (as
+ * frame_getitems reads them).  The box may cross chunk boundaries; the chunks it touches are read in ascending order,
+ * each as one blosc_b200_getslice part, and the first failure decides the result: its header code, blosc_d's code, or
+ * -1 for a touched chunk whose typesize differs from chunk 0's.  On a failure a host dest is untouched; a device dest
+ * may hold the parts of earlier chunks.  The geometry is checked as in blosc_b200_getslice, against the frame's
+ * nbytes. */
+long long blosc_b200_frame_getslice(const void* frame, size_t framesize, int ndim, const int64_t* shape,
+                                    const int64_t* start, const int64_t* stop, void* dest);
 int       blosc_b200_frame_info(const void* frame, size_t framesize, size_t* nbytes, size_t* cbytes,
                                 size_t* chunksize, size_t* nchunks);
 long long blosc_b200_frame_chunk(const void* frame, size_t framesize, size_t i, size_t* chunk_cbytes);
