@@ -162,14 +162,19 @@ static int backend_ready(void) {
 
 static void buf_free(b2_buf* b) { if (b->p) b2_dev_free(b->p); b->p = NULL; b->cap = 0; }
 
-/* Everything a slot owns; the caller holds the slot (in_use) and the slot's device need not be current
- * (device and page-locked allocations are freed by address) */
-static void ws_teardown(b2_ws* w) {
-  int k;
+/* the device scratch of a slot; its stream, result words and bounce slices stay */
+static void ws_free_bufs(b2_ws* w) {
   buf_free(&w->in); buf_free(&w->filt); buf_free(&w->slots); buf_free(&w->out);
   buf_free(&w->csizes); buf_free(&w->needs); buf_free(&w->bstarts);
   buf_free(&w->prev); buf_free(&w->segs); buf_free(&w->ptail); buf_free(&w->plan);
   buf_free(&w->fplan); buf_free(&w->fpieces); buf_free(&w->fstage);
+}
+
+/* Everything a slot owns; the caller holds the slot (in_use) and the slot's device need not be current
+ * (device and page-locked allocations are freed by address) */
+static void ws_teardown(b2_ws* w) {
+  int k;
+  ws_free_bufs(w);
   for (k = 0; k < B2_STAGE_DEPTH; k++) {
     if (w->stage[k]) b2_pinned_free(w->stage[k]);
     if (w->stage_ev[k]) b2_event_destroy(w->stage_ev[k]);
@@ -266,10 +271,7 @@ int blosc_free_resources(void) {                              /* blosc.h:411 */
   for (i = 0; i < B2_MAX_WS; i++) {
     b2_ws* w = &g_ws[i];
     if (w->in_use || !w->ready) continue;
-    buf_free(&w->in); buf_free(&w->filt); buf_free(&w->slots); buf_free(&w->out);
-    buf_free(&w->csizes); buf_free(&w->needs); buf_free(&w->bstarts);
-    buf_free(&w->prev); buf_free(&w->segs); buf_free(&w->ptail); buf_free(&w->plan);
-    buf_free(&w->fplan); buf_free(&w->fpieces); buf_free(&w->fstage);
+    ws_free_bufs(w);
   }
   pthread_mutex_unlock(&g_ws_mutex);
   return 0;
@@ -553,6 +555,13 @@ static int d2h_any(b2_ws* w, void* dst, const void* src, size_t n) {
     }
   }
   return 0;
+}
+
+/* Where a read writes n bytes: dest itself when it is device memory, else `stage`, which the caller copies to dest once
+ * at the end (d2h_any), so that a failed read leaves dest untouched.  NULL when the staging buffer cannot be had. */
+static uint8_t* stage_dest(b2_buf* stage, void* dest, int dest_dev, size_t n) {
+  if (dest_dev) return (uint8_t*)dest;
+  return buf_ensure(stage, n + 64) ? NULL : (uint8_t*)stage->p;
 }
 
 static void make_header(uint8_t* h, int versionlz, int flags, int typesize, int32_t nbytes, int32_t blocksize,
@@ -875,17 +884,24 @@ static int launch_decode_blocks(b2_ws* w, const b2_hdr* h, int codec, const uint
   return 0;
 }
 
+/* Wait for the launches so far and read their decode verdict: 0, blosc_d's negative code, or -1 when the copy or the
+ * sync fails (the counters are reset then).  status NULL: nothing was decoded, and the word, possibly stale, is not
+ * looked at. */
+static int read_verdict(b2_ws* w, const int* status) {
+  if (b2_copy_d2h(w->h_result + B2_R_STATUS_OUT, w->d_result + B2_R_STATUS_OUT, 4, w->stream) || b2_stream_sync(w->stream)) {
+    ws_reset_counters(w);
+    return -1;
+  }
+  return status && w->h_result[B2_R_STATUS_OUT] < 0 ? w->h_result[B2_R_STATUS_OUT] : 0;
+}
+
 /* Decode blocks [first, first+count) of a chunk that is already on the device into `d_out`
  * (device), which represents buffer offsets [first*blocksize, ...).  Shared by decompress and a one-range read. */
 static int decode_blocks(b2_ws* w, const b2_hdr* h, int codec, const uint8_t* d_chunk, int first, int count,
                          uint8_t* d_out) {
   const int has_left = h->leftover > 0 && first + count == h->nblocks;
   if (launch_decode_blocks(w, h, codec, d_chunk, first, count, NULL, has_left, d_out)) return -1;
-  if (b2_copy_d2h(w->h_result + B2_R_STATUS_OUT, w->d_result + B2_R_STATUS_OUT, 4, w->stream) || b2_stream_sync(w->stream)) {
-    ws_reset_counters(w);
-    return -1;
-  }
-  return w->h_result[B2_R_STATUS_OUT] < 0 ? w->h_result[B2_R_STATUS_OUT] : 0;
+  return read_verdict(w, w->d_result + B2_R_STATUS_OUT);
 }
 
 /* max_cbytes >= 0 (frames): the chunk lives in a slot of that many bytes and must decode to exactly
@@ -1069,6 +1085,58 @@ static int stage_blocks(b2_ws* w, const b2_hdr* h, const uint8_t* hs, const int*
   return rc;
 }
 
+/* Stage the payload of a memcpyed host chunk that the listed blocks cover, block j of the list at j * blocksize of
+ * w->in; runs of consecutive blocks are copied as one. */
+static int stage_memcpyed_blocks(b2_ws* w, const b2_hdr* h, const uint8_t* hs, const int* blocks, int count) {
+  const long long bs = h->blocksize;
+  int i = 0, j;
+  if (buf_ensure(&w->in, (size_t)count * (size_t)bs + 64)) return -1;
+  while (i < count) {
+    long long end;
+    for (j = i + 1; j < count && blocks[j] == blocks[j - 1] + 1; j++) {}
+    end = ((long long)blocks[j - 1] + 1) * bs;
+    if (end > h->nbytes) end = h->nbytes;
+    if (h2d_any(w, (uint8_t*)w->in.p + i * bs, hs + 16 + blocks[i] * bs, (size_t)(end - blocks[i] * bs))) return -1;
+    i = j;
+  }
+  return 0;
+}
+
+/* The gather's source for the touched blocks of a checked chunk, listed in ascending order in w->bstarts (has_left: the
+ * last is the short last block).  A memcpyed device chunk is read in place; a host chunk has the list read back and its
+ * listed blocks staged; a compressed chunk's are then decoded into the compact scratch w->out, and *status is the
+ * verdict the gather must check (else NULL). */
+static int touched_source(b2_ws* w, const void* src, int src_dev, const b2_hdr* h, int codec, int count, int has_left,
+                          const uint8_t** d_src, const int** status) {
+  const int memcpyed = (h->flags & BLOSC_MEMCPYED) != 0;
+  const uint8_t* d_chunk = (const uint8_t*)src;
+  int* hblocks = NULL;
+  int rc = -1;
+  *status = NULL;
+  if (memcpyed && src_dev) { *d_src = d_chunk + 16; return 0; }
+  do {
+    if (!src_dev) {
+      if (!(hblocks = (int*)malloc(4 * (size_t)count))) break;
+      if (d2h_any(w, hblocks, w->bstarts.p, 4 * (size_t)count)) break;
+      if (memcpyed ? stage_memcpyed_blocks(w, h, (const uint8_t*)src, hblocks, count)
+                   : stage_blocks(w, h, (const uint8_t*)src, hblocks, count))
+        break;
+      d_chunk = (const uint8_t*)w->in.p;
+    }
+    if (memcpyed) *d_src = d_chunk;
+    else {
+      if (buf_ensure(&w->out, (size_t)count * (size_t)h->blocksize + 64)) break;
+      if (launch_decode_blocks(w, h, codec, d_chunk, 0, count, (const int*)w->bstarts.p, has_left, (uint8_t*)w->out.p))
+        break;
+      *d_src = (const uint8_t*)w->out.p;
+      *status = w->d_result + B2_R_STATUS_OUT;
+    }
+    rc = 0;
+  } while (0);
+  free(hblocks);
+  return rc;
+}
+
 /* The range table of the gather, in one copy.  A host dest receives the ranges packed, from a device staging buffer
  * (w->slots), so their destinations become their positions in it. */
 static int upload_ranges(b2_ws* w, GatherRange* tab, int nr, long long total, int dest_dev) {
@@ -1081,39 +1149,26 @@ static int upload_ranges(b2_ws* w, GatherRange* tab, int nr, long long total, in
   return b2_copy_h2d(w->segs.p, tab, sizeof(GatherRange) * ((size_t)nr + 1), w->stream);
 }
 
-/* The execution tail of getitems, shared by its host plan and its GPU plan.  On entry the gather table (nr + 1
- * entries; dst = pos when dest is host memory) is in w->segs, and w->slots has room for `total` bytes when dest is host
- * memory.  d_src is the gather's source when it is already on the device (a memcpyed chunk); when it is NULL the
- * `count` blocks listed in w->bstarts (ascending; has_left: the last is the chunk's short last block) are decoded and
- * unfiltered from d_chunk into a compact scratch.  A host dest then receives the ranges from w->slots: at dest +
- * at_b[0] when `contiguous`, else range r at dest + at_b[r] (tab: the table on the host).  Returns total, or blosc_d's
- * code when a stream fails to decode (dest is then untouched). */
-static long long getitems_run(b2_ws* w, const b2_hdr* h, int codec, const uint8_t* d_src, const uint8_t* d_chunk,
-                              int count, int has_left, int nr, long long total, void* dest, int dest_dev,
-                              const GatherRange* tab, const long long* at_b, int contiguous) {
+/* The execution tail of getitems, shared by its host plan and its GPU plan: the gather of `nr` ranges from d_src
+ * (status: the verdict it checks, or NULL; see touched_source), the verdict, and a host dest's copy out.  On entry the
+ * gather table (nr + 1 entries; dst = pos when dest is host memory) is in w->segs, and w->slots has room for `total`
+ * bytes when dest is host memory.  A host dest then receives the ranges from w->slots: all of them at dest + at_b[0]
+ * when tab is NULL, else range r at dest + at_b[r] (tab: the table on the host).  Returns total, or blosc_d's code when
+ * a stream fails to decode (dest is then untouched). */
+static long long getitems_run(b2_ws* w, const uint8_t* d_src, const int* status, int nr, long long total, void* dest,
+                              int dest_dev, const GatherRange* tab, const long long* at_b) {
   GatherArgs ga;
-  const int* status = NULL;
   long long result = -1;
   uint8_t* tmp = NULL;
-  int r;
+  int r, rc;
   memset(&ga, 0, sizeof ga);
   do {
-    if (!d_src) {
-      if (buf_ensure(&w->out, (size_t)count * (size_t)h->blocksize + 64)) break;
-      if (launch_decode_blocks(w, h, codec, d_chunk, 0, count, (const int*)w->bstarts.p, has_left, (uint8_t*)w->out.p)) break;
-      d_src = (const uint8_t*)w->out.p;
-      status = w->d_result + B2_R_STATUS_OUT;
-    }
     ga.src = d_src; ga.dst = dest_dev ? (uint8_t*)dest : (uint8_t*)w->slots.p; ga.ranges = (const GatherRange*)w->segs.p;
     ga.nranges = nr; ga.total = total; ga.status = status;
     if (b2_launch_gather(&ga, w->stream)) { ws_reset_counters(w); break; }
-    if (b2_copy_d2h(w->h_result + B2_R_STATUS_OUT, w->d_result + B2_R_STATUS_OUT, 4, w->stream) || b2_stream_sync(w->stream)) {
-      ws_reset_counters(w);
-      break;
-    }
-    if (status && w->h_result[B2_R_STATUS_OUT] < 0) { result = w->h_result[B2_R_STATUS_OUT]; break; }
+    if ((rc = read_verdict(w, status)) < 0) { result = rc; break; }
     if (!dest_dev) {
-      if (contiguous) {
+      if (!tab) {
         if (d2h_any(w, (uint8_t*)dest + at_b[0], w->slots.p, (size_t)total)) break;
       } else {                                                             /* scattered (frame pieces) */
         if (!(tmp = (uint8_t*)malloc((size_t)total))) break;
@@ -1178,8 +1233,7 @@ static long long getitems_chunk(const void* src, long long max_cbytes, int n, co
   if (!w) { free(tab); free(lo_b); return -1; }
   do {
     const uint8_t* d_src = NULL;
-    const uint8_t* d_chunk = NULL;
-    int count = 0, has_left = 0;
+    const int* status = NULL;
     if (h.flags & BLOSC_MEMCPYED) {
       if (src_dev) d_src = (const uint8_t*)src + 16;                       /* ranges read the payload in place */
       else {                                                               /* the ranges, packed, cross PCIe once */
@@ -1195,7 +1249,8 @@ static long long getitems_chunk(const void* src, long long max_cbytes, int n, co
     } else {
       /* the touched blocks: one interval of block numbers per range, merged, then listed in ascending order */
       const int bs = h.blocksize;
-      int nv, k;
+      const uint8_t* d_chunk = (const uint8_t*)src;
+      int nv, k, count = 0;
       if (!(iv = (b2_iv*)malloc(sizeof(b2_iv) * (size_t)nr))) break;
       for (r = 0; r < nr; r++) {
         iv[r].lo = lo_b[r] / bs;
@@ -1208,8 +1263,9 @@ static long long getitems_chunk(const void* src, long long max_cbytes, int n, co
         long long b;
         for (b = iv[k].lo; b < iv[k].hi; b++) blocks[count++] = (int)b;
       }
-      if (src_dev) d_chunk = (const uint8_t*)src;
-      else {
+      /* a host chunk is staged before the uploads below: after them, 4096 ranges of a pinned host chunk read 15 % slower
+       * on an H100 (700 W) */
+      if (!src_dev) {
         if (stage_blocks(w, &h, (const uint8_t*)src, blocks, count)) break;
         d_chunk = (const uint8_t*)w->in.p;
       }
@@ -1231,9 +1287,11 @@ static long long getitems_chunk(const void* src, long long max_cbytes, int n, co
       if (buf_ensure(&w->bstarts, sizeof(int) * (size_t)count + 64)) break;
       if (b2_copy_h2d(w->bstarts.p, blocks, sizeof(int) * (size_t)count, w->stream)) break;
       if (upload_ranges(w, tab, nr, total, dest_dev)) break;      /* before the decode: a pageable copy would wait for it */
-      has_left = h.leftover > 0 && blocks[count - 1] == h.nblocks - 1;
+      if (touched_source(w, d_chunk, 1, &h, codec, count, h.leftover > 0 && blocks[count - 1] == h.nblocks - 1, &d_src,
+                         &status))
+        break;
     }
-    result = getitems_run(w, &h, codec, d_src, d_chunk, count, has_left, nr, total, dest, dest_dev, tab, at_b, contiguous);
+    result = getitems_run(w, d_src, status, nr, total, dest, dest_dev, contiguous ? NULL : tab, at_b);
   } while (0);
   ws_release(w);
   free(tab); free(lo_b); free(iv); free(blocks); free(tmp);
@@ -1244,109 +1302,91 @@ int blosc_getitem(const void* src, int start, int nitems, void* dest) {         
   return (int)getitems_chunk(src, -1, 1, &start, &nitems, NULL, dest);
 }
 
-/* Stage the payload of a memcpyed host chunk that the listed blocks cover, block j of the list at j * blocksize of
- * w->in; runs of consecutive blocks are copied as one. */
-static int stage_memcpyed_blocks(b2_ws* w, const b2_hdr* h, const uint8_t* hs, const int* blocks, int count) {
-  const long long bs = h->blocksize;
-  int i = 0, j;
-  if (buf_ensure(&w->in, (size_t)count * (size_t)bs + 64)) return -1;
-  while (i < count) {
-    long long end;
-    for (j = i + 1; j < count && blocks[j] == blocks[j - 1] + 1; j++) {}
-    end = ((long long)blocks[j - 1] + 1) * bs;
-    if (end > h->nbytes) end = h->nbytes;
-    if (h2d_any(w, (uint8_t*)w->in.p + i * bs, hs + 16 + blocks[i] * bs, (size_t)(end - blocks[i] * bs))) return -1;
-    i = j;
-  }
+#define B2_R_PLAN 8   /* h_result words 8..15 receive a GPU plan's record (GetitemsPlan, FramePlan) */
+#define B2_AL(x) (((x) + 15) & ~(size_t)15)
+
+/* Wait for a GPU plan and read the first n bytes of its record, at d_rec, into *rec */
+static int read_plan(b2_ws* w, const void* d_rec, void* rec, size_t n) {
+  if (b2_copy_d2h(w->h_result + B2_R_PLAN, d_rec, n, w->stream) || b2_stream_sync(w->stream)) return -1;
+  memcpy(rec, w->h_result + B2_R_PLAN, n);
   return 0;
 }
 
-#define B2_R_PLAN 8   /* h_result words 8..15 receive a GPU plan's record (GetitemsPlan, FramePlan) */
-#define B2_AL(x) (((x) + 15) & ~(size_t)15)
+/* The tile state of one scan of `tiles` tiles: its ticket and flags (both zeroed by the caller), then the tiles'
+ * aggregates and inclusive prefixes of `width` bytes each, back to back from `vals` */
+static PlanScan plan_scan(uint8_t* ticket, uint8_t* flags, uint8_t* vals, size_t width, size_t tiles) {
+  PlanScan s;
+  s.ticket = (unsigned*)ticket; s.flag = (unsigned*)flags; s.agg = vals; s.inc = vals + width * tiles;
+  return s;
+}
+
+/* The scratch of a chunk's GPU plan in w->plan, for n ranges (0: a box), and the fields of *pa that describe the chunk
+ * or point into it: the record, the tickets, the tile flags and the difference array, all zeroed; then the tiles'
+ * values, the range lengths and the block slots; the block list in w->bstarts unless in_place.  Returns the room for
+ * one uploaded host list of n ints, or NULL. */
+static uint8_t* plan_scratch(b2_ws* w, const b2_hdr* h, int n, int in_place, PlanArgs* pa) {
+  const size_t tb = ((size_t)h->nblocks + PLAN_TILE - 1) / PLAN_TILE, tr = ((size_t)n + PLAN_TILE - 1) / PLAN_TILE;
+  const size_t o_tk = 32, o_flag = 64, o_cover = B2_AL(o_flag + 4 * (2 * tb + tr));
+  const size_t zeroed = B2_AL(o_cover + 4 * ((size_t)h->nblocks + 1));
+  const size_t o_vals = zeroed, o_len = B2_AL(o_vals + 4 * 4 * tb + 8 * 2 * tr);
+  const size_t o_slot = B2_AL(o_len + 8 * (size_t)n), o_up = B2_AL(o_slot + 4 * (size_t)h->nblocks);
+  uint8_t* base;
+  if (buf_ensure(&w->plan, o_up + 4 * (size_t)n)) return NULL;
+  if (!in_place && buf_ensure(&w->bstarts, 4 * (size_t)h->nblocks + 64)) return NULL;
+  base = (uint8_t*)w->plan.p;
+  if (b2_memset_dev(base, 0, zeroed, w->stream)) return NULL;
+  memset(pa, 0, sizeof *pa);
+  pa->typesize = h->typesize; pa->blocksize = h->blocksize; pa->nblocks = h->nblocks;
+  pa->leftover = h->leftover > 0; pa->nbytes = h->nbytes; pa->in_place = in_place;
+  pa->len = (long long*)(base + o_len); pa->cover = (int*)(base + o_cover); pa->slot = (int*)(base + o_slot);
+  pa->blocks = (int*)w->bstarts.p; pa->rec = (GetitemsPlan*)base;
+  pa->scan[PLAN_COVER] = plan_scan(base + o_tk, base + o_flag, base + o_vals, 4, tb);
+  pa->scan[PLAN_SLOT] = plan_scan(base + o_tk + 4, base + o_flag + 4 * tb, base + o_vals + 8 * tb, 4, tb);
+  pa->scan[PLAN_POS] = plan_scan(base + o_tk + 8, base + o_flag + 8 * tb, base + o_vals + 16 * tb, 8, tr);
+  return base + o_up;
+}
+
+/* A range list as a GPU plan reads it: the list itself when it is in device memory, else its copy in `room` (NULL when
+ * the upload fails).  At most one of a call's two lists is in host memory, so one room serves both. */
+static const void* dev_list(b2_ws* w, const void* list, int list_dev, size_t bytes, void* room) {
+  if (list_dev) return list;
+  return h2d_any(w, room, list, bytes) ? NULL : room;
+}
 
 /* The GPU plan (dev_chunk.cuh plan_*_kernel), for range lists of which at least one is in device memory (a host one is
  * uploaded), on the caller's workspace.  It builds the gather table in w->segs and the touched-block list in
  * w->bstarts, both as the host plan would (the table keeps empty ranges, which copy nothing), and the host reads back
  * one small record.  A failing range is reported by getitem_range on that range alone, so the code and the message
- * are the host plan's.  A host chunk also has the block list read back, to stage only the touched blocks.  dsts NULL:
- * the ranges land back to back in dest; else range r lands at dest + dsts[r] (device lists, device dest: frame
- * pieces). */
+ * are the host plan's.  dsts NULL: the ranges land back to back in dest; else range r lands at dest + dsts[r] (device
+ * lists, device dest: frame pieces). */
 static long long getitems_gpu(b2_ws* w, const void* src, int src_dev, const b2_hdr* h, int codec, int n,
                               const int* starts, int starts_dev, const int* nitems, int nitems_dev,
                               const long long* dsts, void* dest, int dest_dev) {
-  const int memcpyed = (h->flags & BLOSC_MEMCPYED) != 0, in_place = memcpyed && src_dev;
-  const size_t tb = ((size_t)h->nblocks + PLAN_TILE - 1) / PLAN_TILE, tr = ((size_t)n + PLAN_TILE - 1) / PLAN_TILE;
-  /* one scratch: the record, the tickets, the tile flags and the difference array, all zeroed; then the tiles' values,
-   * the range lengths, the block slots and an uploaded host list */
-  const size_t o_tk = 32, o_flag = 64, o_cover = B2_AL(o_flag + 4 * (2 * tb + tr));
-  const size_t zeroed = B2_AL(o_cover + 4 * ((size_t)h->nblocks + 1));
-  const size_t o_vals = zeroed, o_len = B2_AL(o_vals + 4 * 4 * tb + 8 * 2 * tr);
-  const size_t o_slot = B2_AL(o_len + 8 * (size_t)n), o_up = B2_AL(o_slot + 4 * (size_t)h->nblocks);
-  const size_t need = o_up + 4 * (size_t)n;
   const long long at0 = 0;
-  long long result = -1;
-  int* hblocks = NULL;
-  do {
-    PlanArgs pa;
-    GetitemsPlan rec;
-    uint8_t* base;
-    const uint8_t* d_src = NULL;
-    const uint8_t* d_chunk = NULL;
-    int k;
-    if (buf_ensure(&w->plan, need) || buf_ensure(&w->segs, sizeof(GatherRange) * ((size_t)n + 1) + 64)) break;
-    if (!in_place && buf_ensure(&w->bstarts, 4 * (size_t)h->nblocks + 64)) break;
-    base = (uint8_t*)w->plan.p;
-    memset(&pa, 0, sizeof pa);
-    pa.starts = starts; pa.nitems = nitems;
-    if (!starts_dev || !nitems_dev) {                                      /* the host list joins the device one */
-      if (h2d_any(w, base + o_up, starts_dev ? (const void*)nitems : (const void*)starts, 4 * (size_t)n)) break;
-      if (starts_dev) pa.nitems = (const int*)(base + o_up); else pa.starts = (const int*)(base + o_up);
-    }
-    if (b2_memset_dev(base, 0, zeroed, w->stream) || b2_memset_dev(base, 0xff, 4, w->stream)) break;
-    pa.nranges = n; pa.typesize = h->typesize; pa.blocksize = h->blocksize; pa.nblocks = h->nblocks;
-    pa.leftover = h->leftover > 0; pa.nbytes = h->nbytes; pa.in_place = in_place;
-    pa.len = (long long*)(base + o_len); pa.cover = (int*)(base + o_cover); pa.slot = (int*)(base + o_slot);
-    pa.blocks = (int*)w->bstarts.p; pa.ranges = (GatherRange*)w->segs.p; pa.rec = (GetitemsPlan*)base; pa.dsts = dsts;
-    for (k = 0; k < 3; k++) {
-      const size_t tiles = k < 2 ? tb : tr;
-      const size_t flags_at = o_flag + 4 * (k < 2 ? k * tb : 2 * tb);
-      const size_t vals_at = o_vals + (k < 2 ? 2 * 4 * k * tb : 4 * 4 * tb), width = k < 2 ? 4 : 8;
-      pa.scan[k].ticket = (unsigned*)(base + o_tk) + k;
-      pa.scan[k].flag = (unsigned*)(base + flags_at);
-      pa.scan[k].agg = base + vals_at;
-      pa.scan[k].inc = base + vals_at + width * tiles;
-    }
-    if (b2_launch_plan(&pa, w->stream)) break;
-    if (b2_copy_d2h(w->h_result + B2_R_PLAN, base, sizeof rec, w->stream) || b2_stream_sync(w->stream)) break;
-    memcpy(&rec, w->h_result + B2_R_PLAN, sizeof rec);
-    if (rec.bad != 0xffffffffu) {                                          /* blosc_getitem's verdict on that range */
-      int s, c;
-      long long lo, hi;
-      if (copy_any(&s, 0, starts + rec.bad, starts_dev, 4, w->stream) ||
-          copy_any(&c, 0, nitems + rec.bad, nitems_dev, 4, w->stream)) break;
+  PlanArgs pa;
+  GetitemsPlan rec;
+  const uint8_t* d_src;
+  const int* status;
+  uint8_t* up = plan_scratch(w, h, n, (h->flags & BLOSC_MEMCPYED) && src_dev, &pa);
+  if (!up || buf_ensure(&w->segs, sizeof(GatherRange) * ((size_t)n + 1) + 64)) return -1;
+  if (!(pa.starts = (const int*)dev_list(w, starts, starts_dev, 4 * (size_t)n, up)) ||
+      !(pa.nitems = (const int*)dev_list(w, nitems, nitems_dev, 4 * (size_t)n, up)))
+    return -1;
+  if (b2_memset_dev(pa.rec, 0xff, 4, w->stream)) return -1;
+  pa.nranges = n; pa.ranges = (GatherRange*)w->segs.p; pa.dsts = dsts;
+  if (b2_launch_plan(&pa, w->stream) || read_plan(w, pa.rec, &rec, sizeof rec)) return -1;
+  if (rec.bad != 0xffffffffu) {                                            /* blosc_getitem's verdict on that range */
+    int s, c;
+    long long lo, hi;
+    if (!copy_any(&s, 0, starts + rec.bad, starts_dev, 4, w->stream) &&
+        !copy_any(&c, 0, nitems + rec.bad, nitems_dev, 4, w->stream))
       getitem_range(h, s, c, &lo, &hi);
-      break;
-    }
-    if (rec.total == 0) { result = 0; break; }
-    if (!dest_dev && buf_ensure(&w->slots, (size_t)rec.total + 64)) break;
-    if (in_place) d_src = (const uint8_t*)src + 16;
-    else if (src_dev) d_chunk = (const uint8_t*)src;
-    else {                                                                 /* stage the touched blocks only */
-      if (!(hblocks = (int*)malloc(4 * (size_t)rec.nlisted))) break;
-      if (d2h_any(w, hblocks, w->bstarts.p, 4 * (size_t)rec.nlisted)) break;
-      if (memcpyed) {
-        if (stage_memcpyed_blocks(w, h, (const uint8_t*)src, hblocks, rec.nlisted)) break;
-        d_src = (const uint8_t*)w->in.p;
-      } else {
-        if (stage_blocks(w, h, (const uint8_t*)src, hblocks, rec.nlisted)) break;
-        d_chunk = (const uint8_t*)w->in.p;
-      }
-    }
-    result = getitems_run(w, h, codec, d_src, d_chunk, rec.nlisted, rec.has_left, n, rec.total, dest, dest_dev, NULL,
-                          &at0, 1);
-  } while (0);
-  free(hblocks);
-  return result;
+    return -1;
+  }
+  if (rec.total == 0) return 0;
+  if (!dest_dev && buf_ensure(&w->slots, (size_t)rec.total + 64)) return -1;
+  if (touched_source(w, src, src_dev, h, codec, rec.nlisted, rec.has_left, &d_src, &status)) return -1;
+  return getitems_run(w, d_src, status, n, rec.total, dest, dest_dev, NULL, &at0);
 }
 
 long long blosc_b200_getitems(const void* src, int nranges, const int* starts, const int* nitems, void* dest) {
@@ -1454,73 +1494,27 @@ static void box_build(int ndim, const int64_t* shape, const int64_t* start, cons
  * code when a touched block fails to decode (nothing is written then), or -1. */
 static long long getslice_chunk(b2_ws* w, const void* src, int src_dev, const b2_hdr* h, int codec, const B2Box* box,
                                 long long window, uint8_t* d_dst) {
-  const int memcpyed = (h->flags & BLOSC_MEMCPYED) != 0;
   const long long ts = h->typesize, p0 = b2_box_rank(box, window);
   const long long total = (b2_box_rank(box, window + h->nbytes / ts) - p0) * ts;
-  /* the plan's scratch: the record, the ticket and the tile flags, zeroed; then the tiles' values, cover and slot */
-  const size_t tb = ((size_t)h->nblocks + PLAN_TILE - 1) / PLAN_TILE;
-  const size_t o_tk = 32, o_flag = 64, zeroed = B2_AL(o_flag + 4 * tb), o_vals = zeroed;
-  const size_t o_cover = B2_AL(o_vals + 8 * tb), o_slot = B2_AL(o_cover + 4 * (size_t)h->nblocks);
+  GetitemsPlan rec = {0};
   BoxGatherArgs ga;
-  int* hblocks = NULL;
-  long long result = -1;
+  int rc;
   if (total == 0) return 0;
   memset(&ga, 0, sizeof ga);
   ga.box = *box; ga.window = window; ga.p0 = p0; ga.total = total;
   ga.typesize = h->typesize; ga.blocksize = h->blocksize; ga.dst = d_dst;
-  do {
-    if (memcpyed && src_dev) ga.src = (const uint8_t*)src + 16;            /* the payload, read in place: no plan */
-    else {
-      BoxPlanArgs bp;
-      GetitemsPlan rec;
-      uint8_t* base;
-      const uint8_t* d_chunk = (const uint8_t*)src;
-      if (buf_ensure(&w->plan, o_slot + 4 * (size_t)h->nblocks) || buf_ensure(&w->bstarts, 4 * (size_t)h->nblocks + 64))
-        break;
-      base = (uint8_t*)w->plan.p;
-      if (b2_memset_dev(base, 0, zeroed, w->stream)) break;
-      memset(&bp, 0, sizeof bp);
-      bp.box = *box; bp.window = window;
-      bp.plan.typesize = h->typesize; bp.plan.blocksize = h->blocksize; bp.plan.nblocks = h->nblocks;
-      bp.plan.leftover = h->leftover > 0; bp.plan.nbytes = h->nbytes;
-      bp.plan.cover = (int*)(base + o_cover); bp.plan.slot = (int*)(base + o_slot);
-      bp.plan.blocks = (int*)w->bstarts.p; bp.plan.rec = (GetitemsPlan*)base;
-      bp.plan.scan[PLAN_SLOT].ticket = (unsigned*)(base + o_tk);
-      bp.plan.scan[PLAN_SLOT].flag = (unsigned*)(base + o_flag);
-      bp.plan.scan[PLAN_SLOT].agg = base + o_vals;
-      bp.plan.scan[PLAN_SLOT].inc = base + o_vals + 4 * tb;
-      if (b2_launch_box_plan(&bp, w->stream)) break;
-      if (b2_copy_d2h(w->h_result + B2_R_PLAN, base, sizeof rec, w->stream) || b2_stream_sync(w->stream)) break;
-      memcpy(&rec, w->h_result + B2_R_PLAN, sizeof rec);
-      ga.slot = bp.plan.slot;
-      if (!src_dev) {                                                      /* stage the touched blocks only */
-        if (!(hblocks = (int*)malloc(4 * (size_t)rec.nlisted))) break;
-        if (d2h_any(w, hblocks, w->bstarts.p, 4 * (size_t)rec.nlisted)) break;
-        if (memcpyed ? stage_memcpyed_blocks(w, h, (const uint8_t*)src, hblocks, rec.nlisted)
-                     : stage_blocks(w, h, (const uint8_t*)src, hblocks, rec.nlisted))
-          break;
-        d_chunk = (const uint8_t*)w->in.p;
-      }
-      if (memcpyed) ga.src = d_chunk;                  /* a host payload: listed block j staged at j * blocksize */
-      else {
-        if (buf_ensure(&w->out, (size_t)rec.nlisted * (size_t)h->blocksize + 64)) break;
-        if (launch_decode_blocks(w, h, codec, d_chunk, 0, rec.nlisted, (const int*)w->bstarts.p, rec.has_left,
-                                 (uint8_t*)w->out.p))
-          break;
-        ga.src = (const uint8_t*)w->out.p;
-        ga.status = w->d_result + B2_R_STATUS_OUT;
-      }
-    }
-    if (b2_launch_box_gather(&ga, w->stream)) { ws_reset_counters(w); break; }
-    if (b2_copy_d2h(w->h_result + B2_R_STATUS_OUT, w->d_result + B2_R_STATUS_OUT, 4, w->stream) || b2_stream_sync(w->stream)) {
-      ws_reset_counters(w);
-      break;
-    }
-    if (ga.status && w->h_result[B2_R_STATUS_OUT] < 0) { result = w->h_result[B2_R_STATUS_OUT]; break; }
-    result = total;
-  } while (0);
-  free(hblocks);
-  return result;
+  if (!((h->flags & BLOSC_MEMCPYED) && src_dev)) {            /* a memcpyed device chunk is read in place: no plan */
+    BoxPlanArgs bp;
+    bp.box = *box; bp.window = window;
+    if (!plan_scratch(w, h, 0, 0, &bp.plan) || b2_launch_box_plan(&bp, w->stream) ||
+        read_plan(w, bp.plan.rec, &rec, sizeof rec))
+      return -1;
+    ga.slot = bp.plan.slot;
+  }
+  if (touched_source(w, src, src_dev, h, codec, rec.nlisted, rec.has_left, &ga.src, &ga.status)) return -1;
+  if (b2_launch_box_gather(&ga, w->stream)) { ws_reset_counters(w); return -1; }
+  rc = read_verdict(w, ga.status);
+  return rc < 0 ? rc : total;
 }
 
 long long blosc_b200_getslice(const void* src, int ndim, const int64_t* shape, const int64_t* start,
@@ -1528,6 +1522,7 @@ long long blosc_b200_getslice(const void* src, int ndim, const int64_t* shape, c
   b2_hdr h;
   B2Box box;
   b2_ws* w;
+  uint8_t* d_dst;
   long long nitems = 0, result = -1;
   int src_dev, dest_dev, codec = 0, rc;
   if (box_geometry(ndim, shape, start, stop, &nitems)) return -1;
@@ -1539,15 +1534,10 @@ long long blosc_b200_getslice(const void* src, int ndim, const int64_t* shape, c
   box_build(ndim, shape, start, stop, nitems, &box);
   dest_dev = b2_ptr_is_device(dest);
   if (!(w = ws_acquire())) return -1;
-  do {                                                 /* a host dest: staged in device memory, copied out once */
-    uint8_t* d_dst = (uint8_t*)dest;
-    if (!dest_dev) {
-      if (buf_ensure(&w->slots, (size_t)(box.count * h.typesize) + 64)) break;
-      d_dst = (uint8_t*)w->slots.p;
-    }
+  if ((d_dst = stage_dest(&w->slots, dest, dest_dev, (size_t)(box.count * h.typesize)))) {
     result = getslice_chunk(w, src, src_dev, &h, codec, &box, 0, d_dst);
     if (result > 0 && !dest_dev && d2h_any(w, dest, d_dst, (size_t)result)) result = -1;
-  } while (0);
+  }
   ws_release(w);
   return result;
 }
@@ -1745,9 +1735,16 @@ long long blosc_b200_frame_compress(int clevel, int doshuffle, size_t typesize, 
   return (long long)j.cursor;
 }
 
-/* reads and validates the index; *offsets is malloc'ed (nchunks+1 entries, the last one = cbytes) */
-static int frame_open(const void* frame, size_t framesize, size_t* nbytes, size_t* chunksize, size_t* nchunks,
-                      uint64_t** offsets) {
+/* An opened frame: its index, and (frame_open_items) the items its chunks hold */
+typedef struct {
+  size_t nbytes, chunksize, nchunks;
+  uint64_t* off;            /* [nchunks + 1] chunk offsets, malloc'ed; off[nchunks] is the frame's cbytes */
+  int dev;                  /* the frame is in device memory */
+  size_t typesize, ipc;     /* chunk 0's typesize (1 in a frame with no chunk) and the items per chunk */
+} b2_frame;
+
+/* reads and validates the index into *f */
+static int frame_open(const void* frame, size_t framesize, b2_frame* f) {
   uint8_t hb[B2_FRAME_HDR];
   uint8_t* raw;
   uint64_t* off;
@@ -1758,11 +1755,11 @@ static int frame_open(const void* frame, size_t framesize, size_t* nbytes, size_
   if (framesize < B2_FRAME_HDR || copy_some(hb, 0, frame, dev, B2_FRAME_HDR)) return -1;
   do {
     if (memcmp(hb, "B2FR", 4) != 0 || hb[4] != 1) break;
-    *nbytes = (size_t)rd_u64(hb + 8); cbytes = rd_u64(hb + 16);
-    *chunksize = rd_u32(hb + 24); n = rd_u32(hb + 28);
+    f->nbytes = (size_t)rd_u64(hb + 8); cbytes = rd_u64(hb + 16);
+    f->chunksize = rd_u32(hb + 24); n = rd_u32(hb + 28);
     if (cbytes > framesize || cbytes < B2_FRAME_HDR + 8 * (uint64_t)n) break;
-    if (*nbytes > 0 && (*chunksize == 0 || *chunksize > BLOSC_MAX_BUFFERSIZE)) break;
-    if (n != (*nbytes ? (*nbytes + *chunksize - 1) / *chunksize : 0)) break;
+    if (f->nbytes > 0 && (f->chunksize == 0 || f->chunksize > BLOSC_MAX_BUFFERSIZE)) break;
+    if (n != (f->nbytes ? (f->nbytes + f->chunksize - 1) / f->chunksize : 0)) break;
     raw = (uint8_t*)malloc(8 * n + 8);
     off = (uint64_t*)malloc(8 * (n + 1));
     if (!raw || !off) { free(raw); free(off); break; }
@@ -1774,53 +1771,75 @@ static int frame_open(const void* frame, size_t framesize, size_t* nbytes, size_
     for (k = 0; k < n; k++)                /* chunks in order, at least a header each, inside the frame */
       if (off[k] < B2_FRAME_HDR + 8 * (uint64_t)n || off[k + 1] < off[k] + BLOSC_MAX_OVERHEAD || off[k + 1] > cbytes) rc = -1;
     if (rc) { free(off); break; }
-    *nchunks = n; *offsets = off;
+    f->nchunks = n; f->off = off; f->dev = dev;
   } while (0);
   return rc;
 }
 
+/* frame_open, then the typesize of chunk 0 and the items per chunk.  -1 when the frame cannot be read, -2 when that
+ * typesize (left in f->typesize) does not divide the chunksize; f->off is freed on a failure. */
+static int frame_open_items(const void* frame, size_t framesize, b2_frame* f) {
+  uint8_t hb[16];
+  if (frame_open(frame, framesize, f)) return -1;
+  f->typesize = 1;
+  if (f->nchunks > 0) {
+    if (copy_some(hb, 0, (const uint8_t*)frame + f->off[0], f->dev, 16)) { free(f->off); return -1; }
+    f->typesize = hb[3];
+    if (f->typesize == 0 || f->chunksize % f->typesize) { free(f->off); return -2; }
+  }
+  f->ipc = f->chunksize / f->typesize;
+  return 0;
+}
+
+/* The header of chunk c of an opened frame, checked as blosc_getitem checks it, within the chunk's slot: 0,
+ * getitem_header's code, or 1 when the chunk's typesize is not the frame's (its items would not fit in dest) */
+static int frame_chunk_header(b2_ws* w, const void* frame, const b2_frame* f, size_t c, b2_hdr* h, int* codec) {
+  const int rc = getitem_header(w, (const uint8_t*)frame + f->off[c], f->dev, (long long)(f->off[c + 1] - f->off[c]), h,
+                                codec);
+  if (rc) return rc;
+  return (size_t)h->typesize != f->typesize;
+}
+
 int blosc_b200_frame_info(const void* frame, size_t framesize, size_t* nbytes, size_t* cbytes, size_t* chunksize,
                           size_t* nchunks) {
-  size_t nb = 0, cs = 0, nc = 0;
-  uint64_t* off = NULL;
+  b2_frame f;
   if (!backend_ready()) return -1;
-  if (frame_open(frame, framesize, &nb, &cs, &nc, &off)) return -1;
-  if (nbytes) *nbytes = nb;
-  if (cbytes) *cbytes = (size_t)off[nc];
-  if (chunksize) *chunksize = cs;
-  if (nchunks) *nchunks = nc;
-  free(off);
+  if (frame_open(frame, framesize, &f)) return -1;
+  if (nbytes) *nbytes = f.nbytes;
+  if (cbytes) *cbytes = (size_t)f.off[f.nchunks];
+  if (chunksize) *chunksize = f.chunksize;
+  if (nchunks) *nchunks = f.nchunks;
+  free(f.off);
   return 0;
 }
 
 long long blosc_b200_frame_chunk(const void* frame, size_t framesize, size_t i, size_t* chunk_cbytes) {
-  size_t nb = 0, cs = 0, nc = 0;
-  uint64_t* off = NULL;
+  b2_frame f;
   long long r;
   if (!backend_ready()) return -1;
-  if (frame_open(frame, framesize, &nb, &cs, &nc, &off)) return -1;
-  if (i >= nc) { free(off); return -1; }
-  if (chunk_cbytes) *chunk_cbytes = (size_t)(off[i + 1] - off[i]);
-  r = (long long)off[i];
-  free(off);
+  if (frame_open(frame, framesize, &f)) return -1;
+  if (i >= f.nchunks) { free(f.off); return -1; }
+  if (chunk_cbytes) *chunk_cbytes = (size_t)(f.off[i + 1] - f.off[i]);
+  r = (long long)f.off[i];
+  free(f.off);
   return r;
 }
 
 long long blosc_b200_frame_decompress(const void* frame, size_t framesize, void* dest, size_t destsize,
                                       int numinternalthreads) {
   b2_frame_job j;
-  size_t nb = 0, cs = 0, nc = 0;
-  uint64_t* off = NULL;
+  b2_frame f;
   int rc;
   if (!backend_ready()) return -1;
-  if (frame_open(frame, framesize, &nb, &cs, &nc, &off)) return -1;
-  if (nb > destsize) { free(off); return -1; }
+  if (frame_open(frame, framesize, &f)) return -1;
+  if (f.nbytes > destsize) { free(f.off); return -1; }
   memset(&j, 0, sizeof j);
-  j.nchunks = (int)nc; j.workers = frame_workers((int)nc); j.nthreads = numinternalthreads;
-  j.chunksize = cs; j.nbytes = nb; j.frame = (const uint8_t*)frame; j.dest = (uint8_t*)dest; j.offsets = off;
-  rc = nc ? frame_run(&j, frame_decompress_worker) : 0;
-  free(off);
-  return rc ? -1 : (long long)nb;
+  j.nchunks = (int)f.nchunks; j.workers = frame_workers((int)f.nchunks); j.nthreads = numinternalthreads;
+  j.chunksize = f.chunksize; j.nbytes = f.nbytes; j.frame = (const uint8_t*)frame; j.dest = (uint8_t*)dest;
+  j.offsets = f.off;
+  rc = f.nchunks ? frame_run(&j, frame_decompress_worker) : 0;
+  free(f.off);
+  return rc ? -1 : (long long)f.nbytes;
 }
 
 /* One piece of a frame range: the part that falls in one chunk */
@@ -1837,24 +1856,20 @@ static int cmp_piece(const void* a, const void* b) {
  * offset. */
 static long long frame_getitems_host(const void* frame, size_t framesize, size_t nranges, const size_t* starts,
                                      const size_t* nitems, void* dest) {
-  size_t nb = 0, cs = 0, nc = 0, ts = 0, ipc, r, npieces = 0, i, j;
-  uint64_t* off = NULL;
-  uint8_t hb[16];
+  size_t r, npieces = 0, i, j;
+  b2_frame f;
   b2_piece* pieces = NULL;
   long long result = -1, at = 0;
-  if (frame_open(frame, framesize, &nb, &cs, &nc, &off)) return -1;
+  if (frame_open_items(frame, framesize, &f)) return -1;
   do {
-    if (nc == 0) {
+    const size_t ts = f.typesize, ipc = f.ipc;
+    if (f.nchunks == 0) {
       for (r = 0; r < nranges && nitems[r] == 0; r++) {}
       result = r == nranges ? 0 : -1;
       break;
     }
-    if (copy_some(hb, 0, (const uint8_t*)frame + off[0], b2_ptr_is_device(frame), 16)) break;
-    ts = hb[3];
-    if (ts == 0 || cs % ts) break;
-    ipc = cs / ts;                                     /* items per chunk */
     for (r = 0; r < nranges; r++) {
-      if (b2_frame_range_bad(starts[r], nitems[r], nb / ts)) { fprintf(stderr, "`start`+`nitems` out of bounds"); break; }
+      if (b2_frame_range_bad(starts[r], nitems[r], f.nbytes / ts)) { fprintf(stderr, "`start`+`nitems` out of bounds"); break; }
       npieces += nitems[r] ? (starts[r] + nitems[r] - 1) / ipc - starts[r] / ipc + 1 : 0;
     }
     if (r < nranges) break;
@@ -1885,14 +1900,15 @@ static long long frame_getitems_host(const void* frame, size_t framesize, size_t
       dsts = (long long*)malloc(sizeof(long long) * (j - i));
       if (!st || !dsts) { free(st); free(dsts); result = -1; break; }
       for (k = i; k < j; k++) { st[k - i] = pieces[k].start; st[j - i + k - i] = pieces[k].nitems; dsts[k - i] = pieces[k].dst; }
-      rc = getitems_chunk((const uint8_t*)frame + off[pieces[i].chunk], (long long)(off[pieces[i].chunk + 1] - off[pieces[i].chunk]),
-                          (int)(j - i), st, st + (j - i), dsts, dest);
+      rc = getitems_chunk((const uint8_t*)frame + f.off[pieces[i].chunk],
+                          (long long)(f.off[pieces[i].chunk + 1] - f.off[pieces[i].chunk]), (int)(j - i), st, st + (j - i),
+                          dsts, dest);
       free(st); free(dsts);
       if (rc != want) { result = rc < 0 ? rc : -1; break; }
       result += rc;
     }
   } while (0);
-  free(pieces); free(off);
+  free(pieces); free(f.off);
   return result;
 }
 
@@ -1909,27 +1925,21 @@ long long blosc_b200_frame_getitem(const void* frame, size_t framesize, size_t s
  * is copied to dest at the end.  Neither the lists nor the pieces travel to the host. */
 static long long frame_getitems_gpu(const void* frame, size_t framesize, size_t nranges, const size_t* starts,
                                     int starts_dev, const size_t* nitems, int nitems_dev, void* dest) {
-  size_t nb = 0, cs = 0, nc = 0, ts = 1;
-  uint64_t* off = NULL;
-  uint8_t hb[16];
-  const int frame_dev = b2_ptr_is_device(frame), dest_dev = b2_ptr_is_device(dest);
+  const int dest_dev = b2_ptr_is_device(dest);
+  b2_frame f;
   FrameTouch* touched = NULL;
   long long result = -1;
   b2_ws* w;
-  if (frame_open(frame, framesize, &nb, &cs, &nc, &off)) return -1;
-  if (nc > 0) {                                                  /* as frame_getitems_host: the typesize of chunk 0 */
-    if (copy_some(hb, 0, (const uint8_t*)frame + off[0], frame_dev, 16)) { free(off); return -1; }
-    ts = hb[3];
-    if (ts == 0 || cs % ts) { free(off); return -1; }
-  }
-  if (nranges > ((size_t)-1) / 64 || !(w = ws_acquire())) { free(off); return -1; }
+  if (frame_open_items(frame, framesize, &f)) return -1;
+  if (nranges > ((size_t)-1) / 64 || !(w = ws_acquire())) { free(f.off); return -1; }
   do {
     /* one scratch: the record, the tickets, the tile flags and the difference array over chunks, all zeroed; then the
      * tiles' values, the range offsets, the bucket cursors, the touched chunks and an uploaded host list */
-    const size_t tr = (nranges + PLAN_TILE - 1) / PLAN_TILE, tc = (nc + PLAN_TILE - 1) / PLAN_TILE, tiles = tr + 3 * tc;
-    const size_t o_tk = 32, o_flag = 64, o_count = B2_AL(o_flag + 4 * tiles), zeroed = B2_AL(o_count + 8 * (nc + 1));
-    const size_t o_vals = zeroed, o_dst = B2_AL(o_vals + 16 * tiles), o_cursor = B2_AL(o_dst + 8 * nranges);
-    const size_t o_touch = B2_AL(o_cursor + 8 * nc), o_up = B2_AL(o_touch + sizeof(FrameTouch) * nc);
+    const size_t nc = f.nchunks, tr = (nranges + PLAN_TILE - 1) / PLAN_TILE, tc = (nc + PLAN_TILE - 1) / PLAN_TILE;
+    const size_t tiles = tr + 3 * tc, o_tk = 32, o_flag = 64, o_count = B2_AL(o_flag + 4 * tiles);
+    const size_t zeroed = B2_AL(o_count + 8 * (nc + 1)), o_vals = zeroed, o_dst = B2_AL(o_vals + 16 * tiles);
+    const size_t o_cursor = B2_AL(o_dst + 8 * nranges), o_touch = B2_AL(o_cursor + 8 * nc);
+    const size_t o_up = B2_AL(o_touch + sizeof(FrameTouch) * nc);
     FramePlanArgs fa;
     FramePlan rec;
     uint8_t* base;
@@ -1939,28 +1949,21 @@ static long long frame_getitems_gpu(const void* frame, size_t framesize, size_t 
     if (buf_ensure(&w->fplan, o_up + 8 * nranges)) break;
     base = (uint8_t*)w->fplan.p;
     memset(&fa, 0, sizeof fa);
-    fa.starts = (const unsigned long long*)starts; fa.nitems = (const unsigned long long*)nitems;
-    if (!starts_dev || !nitems_dev) {                                      /* the host list joins the device one */
-      if (h2d_any(w, base + o_up, starts_dev ? (const void*)nitems : (const void*)starts, 8 * nranges)) break;
-      if (starts_dev) fa.nitems = (const unsigned long long*)(base + o_up);
-      else fa.starts = (const unsigned long long*)(base + o_up);
-    }
+    if (!(fa.starts = (const unsigned long long*)dev_list(w, starts, starts_dev, 8 * nranges, base + o_up)) ||
+        !(fa.nitems = (const unsigned long long*)dev_list(w, nitems, nitems_dev, 8 * nranges, base + o_up)))
+      break;
     if (nc == 0) fa.starts = NULL;              /* an empty frame: only the counts are looked at, as on the host */
     if (b2_memset_dev(base, 0, zeroed, w->stream) || b2_memset_dev(base, 0xff, 8, w->stream)) break;
-    fa.nranges = (long long)nranges; fa.total_items = nb / ts; fa.ipc = (long long)(cs / ts); fa.typesize = (int)ts;
-    fa.nchunks = (long long)nc;
+    fa.nranges = (long long)nranges; fa.total_items = f.nbytes / f.typesize; fa.ipc = (long long)f.ipc;
+    fa.typesize = (int)f.typesize; fa.nchunks = (long long)nc;
     fa.dst = (long long*)(base + o_dst); fa.count = (long long*)(base + o_count); fa.cursor = (long long*)(base + o_cursor);
     fa.touched = (FrameTouch*)(base + o_touch); fa.rec = (FramePlan*)base;
     for (k = 0; k < 4; k++) {                           /* FPLAN_DST over the ranges, the other three over the chunks */
-      const size_t before = k == 0 ? 0 : tr + (size_t)(k - 1) * tc, width = k == 0 ? tr : tc;
-      fa.scan[k].ticket = (unsigned*)(base + o_tk) + k;
-      fa.scan[k].flag = (unsigned*)(base + o_flag) + before;
-      fa.scan[k].agg = base + o_vals + 16 * before;
-      fa.scan[k].inc = base + o_vals + 16 * before + 8 * width;
+      const size_t before = k == 0 ? 0 : tr + (size_t)(k - 1) * tc;
+      fa.scan[k] = plan_scan(base + o_tk + 4 * k, base + o_flag + 4 * before, base + o_vals + 16 * before, 8,
+                             k == 0 ? tr : tc);
     }
-    if (b2_launch_fplan(&fa, w->stream)) break;
-    if (b2_copy_d2h(w->h_result + B2_R_PLAN, base, sizeof rec, w->stream) || b2_stream_sync(w->stream)) break;
-    memcpy(&rec, w->h_result + B2_R_PLAN, sizeof rec);
+    if (b2_launch_fplan(&fa, w->stream) || read_plan(w, base, &rec, sizeof rec)) break;
     if (rec.bad != ~0ull) {                                                /* frame_getitems_host's verdict */
       if (nc > 0) fprintf(stderr, "`start`+`nitems` out of bounds");
       break;
@@ -1971,25 +1974,19 @@ static long long frame_getitems_gpu(const void* frame, size_t framesize, size_t 
     if (b2_launch_fplan_scatter(&fa, w->stream)) break;
     if (!(touched = (FrameTouch*)malloc(sizeof(FrameTouch) * (size_t)rec.ntouched))) break;
     if (d2h_any(w, touched, base + o_touch, sizeof(FrameTouch) * (size_t)rec.ntouched)) break;
-    if (dest_dev) d_dest = (uint8_t*)dest;
-    else {
-      if (buf_ensure(&w->fstage, (size_t)rec.total + 64)) break;
-      d_dest = (uint8_t*)w->fstage.p;
-    }
+    if (!(d_dest = stage_dest(&w->fstage, dest, dest_dev, (size_t)rec.total))) break;
     for (t = 0; t < rec.ntouched; t++) {              /* the chunks in ascending order; the first failure decides */
       const FrameTouch ch = touched[t];
-      const uint8_t* chunk = (const uint8_t*)frame + off[ch.chunk];
       b2_hdr h;
       int codec = 0, rc;
       long long got = 0;
-      rc = getitem_header(w, chunk, frame_dev, (long long)(off[ch.chunk + 1] - off[ch.chunk]), &h, &codec);
-      if (rc) { result = rc; break; }
-      if ((size_t)h.typesize != ts) break;        /* its items are not the frame's: the pieces would not fit in dest */
+      rc = frame_chunk_header(w, frame, &f, (size_t)ch.chunk, &h, &codec);
+      if (rc) { if (rc < 0) result = rc; break; }
       for (done = 0; done < ch.count; done += INT_MAX) {     /* the chunk plan counts its ranges in int */
         const int n = ch.count - done < INT_MAX ? (int)(ch.count - done) : INT_MAX;
         const long long at = ch.base + done;
-        got = getitems_gpu(w, chunk, frame_dev, &h, codec, n, fa.pstart + at, 1, fa.pnitems + at, 1, fa.pdst + at,
-                           d_dest, 1);
+        got = getitems_gpu(w, (const uint8_t*)frame + f.off[ch.chunk], f.dev, &h, codec, n, fa.pstart + at, 1,
+                           fa.pnitems + at, 1, fa.pdst + at, d_dest, 1);
         if (got < 0) break;
         sum += got;
       }
@@ -2000,7 +1997,7 @@ static long long frame_getitems_gpu(const void* frame, size_t framesize, size_t 
     result = rec.total;
   } while (0);
   ws_release(w);
-  free(touched); free(off);
+  free(touched); free(f.off);
   return result;
 }
 
@@ -2033,63 +2030,52 @@ long long blosc_b200_frame_getitems(const void* frame, size_t framesize, size_t 
  * memory and copied out once, so it is untouched on a failure. */
 long long blosc_b200_frame_getslice(const void* frame, size_t framesize, int ndim, const int64_t* shape,
                                     const int64_t* start, const int64_t* stop, void* dest) {
-  size_t nb = 0, cs = 0, nc = 0, c;
-  uint64_t* off = NULL;
-  uint8_t hb[16];
-  long long nitems = 0, ts = 1, ipc, sum = 0, got = 0, result = -1;
-  int frame_dev, dest_dev;
+  size_t c;
+  b2_frame f;
+  long long nitems = 0, ts, ipc, sum = 0, got = 0, result = -1;
+  int dest_dev, rc;
   B2Box box;
   b2_ws* w;
+  uint8_t* d_dst;
   if (!backend_ready()) return -1;
   if (box_geometry(ndim, shape, start, stop, &nitems)) return -1;
-  if (frame_open(frame, framesize, &nb, &cs, &nc, &off)) return -1;
-  frame_dev = b2_ptr_is_device(frame);
+  rc = frame_open_items(frame, framesize, &f);
+  if (rc == -2)
+    fprintf(stderr, "blosc_b200: chunk 0's typesize %lld does not divide the frame's chunksize\n", (long long)f.typesize);
+  if (rc) return -1;
+  ts = (long long)f.typesize; ipc = (long long)f.ipc;
   dest_dev = b2_ptr_is_device(dest);
-  if (nc > 0) {                                              /* as frame_getitems: the typesize of chunk 0 */
-    if (copy_some(hb, 0, (const uint8_t*)frame + off[0], frame_dev, 16)) { free(off); return -1; }
-    ts = hb[3];
-    if (ts == 0 || cs % (size_t)ts) {
-      fprintf(stderr, "blosc_b200: chunk 0's typesize %lld does not divide the frame's chunksize\n", ts);
-      free(off);
-      return -1;
-    }
-  }
-  if (box_nbytes(nitems, ts, (unsigned long long)nb)) { free(off); return -1; }
-  if (box_empty(ndim, start, stop)) { free(off); return 0; }
+  if (box_nbytes(nitems, ts, (unsigned long long)f.nbytes)) { free(f.off); return -1; }
+  if (box_empty(ndim, start, stop)) { free(f.off); return 0; }
   box_build(ndim, shape, start, stop, nitems, &box);
-  ipc = (long long)cs / ts;
-  if (!(w = ws_acquire())) { free(off); return -1; }
+  if (!(w = ws_acquire())) { free(f.off); return -1; }
   do {
-    uint8_t* d_dst = (uint8_t*)dest;
-    if (!dest_dev) {
-      if (buf_ensure(&w->fstage, (size_t)(box.count * ts) + 64)) break;
-      d_dst = (uint8_t*)w->fstage.p;
-    }
-    for (c = 0; c < nc; c++) {
+    if (!(d_dst = stage_dest(&w->fstage, dest, dest_dev, (size_t)(box.count * ts)))) break;
+    for (c = 0; c < f.nchunks; c++) {
       const long long w0 = (long long)c * ipc, w1 = w0 + ipc < nitems ? w0 + ipc : nitems;
-      const uint8_t* chunk = (const uint8_t*)frame + off[c];
       b2_hdr h;
       int codec = 0;
       if (b2_box_next(&box, w0) >= w1) continue;                          /* no box item in this chunk */
-      got = getitem_header(w, chunk, frame_dev, (long long)(off[c + 1] - off[c]), &h, &codec);
-      if (got) break;
-      if (h.typesize != ts || h.nbytes != (w1 - w0) * ts) {
+      got = frame_chunk_header(w, frame, &f, c, &h, &codec);
+      if (got < 0) break;
+      if (got || h.nbytes != (w1 - w0) * ts) {
         fprintf(stderr, "blosc_b200: chunk %zu holds %d items of %d bytes, not the frame's %lld of %lld\n", c,
                 h.nbytes / h.typesize, h.typesize, w1 - w0, ts);
         got = -1;
         break;
       }
-      got = getslice_chunk(w, chunk, frame_dev, &h, codec, &box, w0, d_dst + b2_box_rank(&box, w0) * ts);
+      got = getslice_chunk(w, (const uint8_t*)frame + f.off[c], f.dev, &h, codec, &box, w0,
+                           d_dst + b2_box_rank(&box, w0) * ts);
       if (got < 0) break;
       sum += got;
     }
-    if (c < nc) { result = got; break; }
+    if (c < f.nchunks) { result = got; break; }
     if (sum != box.count * ts) break;
     if (!dest_dev && d2h_any(w, dest, d_dst, (size_t)sum)) break;
     result = sum;
   } while (0);
   ws_release(w);
-  free(off);
+  free(f.off);
   return result;
 }
 
