@@ -71,6 +71,10 @@ def _load(path: str) -> C.CDLL:
     lib.blosc_b200_getslice.argtypes = [vp, ci, vp, vp, vp, vp]
     lib.blosc_b200_frame_getslice.restype = ll
     lib.blosc_b200_frame_getslice.argtypes = [vp, sz, ci, vp, vp, vp, vp]
+    lib.blosc_b200_getslices.restype = ll
+    lib.blosc_b200_getslices.argtypes = [vp, ci, vp, vp, ll, vp, vp]
+    lib.blosc_b200_frame_getslices.restype = ll
+    lib.blosc_b200_frame_getslices.argtypes = [vp, sz, ci, vp, vp, ll, vp, vp]
     lib.blosc_b200_frame_info.restype = ci
     lib.blosc_b200_frame_info.argtypes = [vp, sz, C.POINTER(sz), C.POINTER(sz), C.POINTER(sz), C.POINTER(sz)]
     lib.blosc_b200_frame_chunk.restype = ll
@@ -167,6 +171,31 @@ def getslice(src, shape, start, stop, dest):
     return int(lib.blosc_b200_getslice(_ptr(src), sh.size, sh.ctypes.data, st.ctypes.data, sp.ctypes.data, _ptr(dest)))
 
 
+def _boxes(shape, extent, starts):
+    """shape / extent as two int64 host arrays of one length, and the corners as (array or tensor to keep alive, its
+    address, their number); `starts` has shape (K, ndim)"""
+    import numpy as np
+    sh, ex = (np.ascontiguousarray(v, dtype=np.int64).reshape(-1) for v in (shape, extent))
+    if sh.size != ex.size:
+        raise ValueError(f"shape and extent have {sh.size} and {ex.size} entries")
+    dims = tuple(starts.shape) if hasattr(starts, "shape") else np.shape(starts)
+    if dims == (0,):                                    # an empty sequence: no boxes
+        dims = (0, sh.size)
+    if len(dims) != 2 or dims[1] != sh.size:
+        raise ValueError(f"starts must have shape (K, {sh.size}), not {dims}")
+    st = _range_list(starts, "int64", ("torch.int64",))
+    return sh, ex, (st[0], st[1], dims[0])
+
+
+def getslices(src, shape, extent, starts, dest):
+    """K boxes of one extent of the C-order array of `shape` that the chunk holds (blosc_b200_getslices): box i covers
+    items [starts[i][k], starts[i][k] + extent[k]) of each dimension and lands at dest + i * B, B its bytes, so `dest`
+    is the stack of the K slices.  starts: (K, ndim), an int64 CUDA tensor (on the device of the call), a numpy array
+    or a sequence.  Returns the bytes written, or a negative code (dest is then untouched)."""
+    sh, ex, st = _boxes(shape, extent, starts)
+    return int(lib.blosc_b200_getslices(_ptr(src), sh.size, sh.ctypes.data, ex.ctypes.data, st[2], st[1], _ptr(dest)))
+
+
 def _name(compressor):
     return compressor.encode() if isinstance(compressor, str) else compressor
 
@@ -204,6 +233,13 @@ def frame_getslice(frame, framesize, shape, start, stop, dest):
     sh, st, sp = _box(shape, start, stop)
     return int(lib.blosc_b200_frame_getslice(_ptr(frame), framesize, sh.size, sh.ctypes.data, st.ctypes.data,
                                              sp.ctypes.data, _ptr(dest)))
+
+
+def frame_getslices(frame, framesize, shape, extent, starts, dest):
+    """getslices over the array a frame holds (blosc_b200_frame_getslices); boxes may cross chunk boundaries."""
+    sh, ex, st = _boxes(shape, extent, starts)
+    return int(lib.blosc_b200_frame_getslices(_ptr(frame), framesize, sh.size, sh.ctypes.data, ex.ctypes.data, st[2],
+                                              st[1], _ptr(dest)))
 
 
 def frame_info(frame, framesize):

@@ -206,6 +206,7 @@ typedef struct GetitemsPlan {
   int has_left;          /* whether the chunk's short last block is one of them */
   int pad;
   long long total;       /* bytes of all ranges */
+  unsigned long long bad_box;   /* getslices: the first box whose corner fails (box_check_kernel); all ones when none */
 } GetitemsPlan;
 
 /* The tile state of one device-wide scan (dev_chunk.cuh plan_scan_kernel, single pass with decoupled look-back) */
@@ -405,6 +406,57 @@ typedef struct BoxGatherArgs {
   uint8_t* dst;
   const int* status;          /* NULL, or the decode verdict: the gather writes nothing when it is negative */
 } BoxGatherArgs;
+
+/* A batch of boxes of one extent (blosc_b200_getslices).  The box at the origin, `box` (start 0, stop = extent, after
+ * the same merge), is shared by all of them: box i is that box moved by the flat offset off[i] = sum of corner[k] *
+ * stride[k], so its items, ranks and unranks are the origin box's shifted by off[i] (box_next_at and the gather, in
+ * dev_chunk.cuh).  span: flat items from a box's first item to its last, the same for every box.
+ *
+ * box_check_kernel, one thread per box: box i's corner is starts[i][0..ndim) in the caller's dimensions, and it fails
+ * when a coordinate is below 0 or above hi[k] = shape[k] - extent[k].  The first failing box goes to *bad by
+ * atomicMin; every box's offset goes to off[i] (0 for a failing box, so the launches that follow stay in bounds).
+ * Frame only (touched != NULL): touched[c] = 1 for every chunk c, of ipc items, that holds an item of some box. */
+typedef struct BoxCheckArgs {
+  B2Box box;
+  const long long* starts;
+  long long nboxes, span;
+  int ndim, pad;
+  long long hi[B2_BOX_MAXDIM];
+  long long stride[B2_BOX_MAXDIM];    /* flat items per step of the caller's dimension k */
+  long long* off;
+  unsigned long long* bad;
+  int* touched;
+  long long ipc, nchunks;
+} BoxCheckArgs;
+
+/* The plan of one chunk's part of a batch: boxes_touch_kernel marks in plan.cover every block that holds a byte of some
+ * box (it only stores 1s; plan.cover starts zeroed), then the PLAN_SLOT scan lists them, as for one box.  Work item
+ * (i, j), j < per_box, tests the j-th block of box i's span inside the chunk, which holds the array's flat items
+ * [window, window + nbytes / typesize).  part != NULL (a frame): item (i, 0) also writes box i's part of the chunk,
+ * the bytes [part[2i], part[2i + 1]) of the box's output whose items lie in the chunk, for the gather. */
+typedef struct BoxesPlanArgs {
+  B2Box box;
+  const long long* off;
+  long long nboxes, per_box, span, window;
+  long long* part;
+  int in_place, pad;          /* a memcpyed device chunk: the parts only, no block is marked */
+  PlanArgs plan;
+} BoxesPlanArgs;
+
+/* boxes_gather_kernel: the batch's output, box i's C-order items at i * count * typesize, total bytes in all, to dst.
+ * part != NULL: the chunk holds only part of each box (a frame, BoxesPlanArgs.part), and box i's bytes outside it are
+ * skipped; NULL: the chunk holds every box.  slot / src / status as in BoxGatherArgs. */
+typedef struct BoxesGatherArgs {
+  B2Box box;
+  const long long* off;
+  const long long* part;
+  long long window, total;
+  int typesize, blocksize;
+  const int* slot;
+  const uint8_t* src;
+  uint8_t* dst;
+  const int* status;
+} BoxesGatherArgs;
 
 #ifdef __cplusplus
 }

@@ -461,3 +461,38 @@ extern "C" int b2_launch_box_gather(const BoxGatherArgs* a, b2_stream_t s) {
   CK(cudaGetLastError());
   return 0;
 }
+
+/* the batch of getslices: the corner check (one thread per box), then the plan of each chunk read (boxes_touch_kernel
+ * over (box, block of its span) work items and the PLAN_SLOT scan), counted as plan launches; the gather as a gather
+ * launch */
+extern "C" int b2_launch_box_check(const BoxCheckArgs* a, b2_stream_t s) {
+  if (a->nboxes <= 0) return 0;
+  ProfScope ps(B2_K_PLAN, s->s);
+  box_check_kernel<<<range_ctas(a->nboxes), PLAN_THREADS, 0, s->s>>>(*a);
+  CK(cudaGetLastError());
+  return 0;
+}
+
+extern "C" int b2_launch_boxes_plan(const BoxesPlanArgs* a, b2_stream_t s) {
+  const long long nb = a->plan.nblocks;
+  if (nb <= 0) return 0;
+  {
+    ProfScope ps(B2_K_PLAN, s->s);
+    boxes_touch_kernel<<<range_ctas(a->nboxes * a->per_box), PLAN_THREADS, 0, s->s>>>(*a);
+    CK(cudaGetLastError());
+  }
+  ProfScope ps(B2_K_PLAN, s->s);
+  plan_scan_kernel<PLAN_SLOT><<<(unsigned)((nb + PLAN_TILE - 1) / PLAN_TILE), PLAN_THREADS, 0, s->s>>>(a->plan, nb);
+  CK(cudaGetLastError());
+  return 0;
+}
+
+extern "C" int b2_launch_boxes_gather(const BoxesGatherArgs* a, b2_stream_t s) {
+  if (a->total <= 0) return 0;
+  long long ctas = (a->total + (long long)GATHER_WARPS * GATHER_SPAN - 1) / ((long long)GATHER_WARPS * GATHER_SPAN);
+  if (ctas > (long long)num_sms() * 8) ctas = (long long)num_sms() * 8;
+  ProfScope ps(B2_K_GATHER, s->s);
+  boxes_gather_kernel<<<(unsigned)ctas, GATHER_WARPS * 32, 0, s->s>>>(*a);
+  CK(cudaGetLastError());
+  return 0;
+}

@@ -1542,6 +1542,150 @@ long long blosc_b200_getslice(const void* src, int ndim, const int64_t* shape, c
   return result;
 }
 
+/* The checks of getslices that need no data: box_geometry on the box [0, extent), the count of boxes, and corners in
+ * device memory on the device the call runs on (that of data or dest when either is device memory, as for getitems).
+ * -1 with a message when one fails. */
+static const int64_t g_box_origin[B2_BOX_MAXDIM] = {0};
+
+static int boxes_geometry(int ndim, const int64_t* shape, const int64_t* extent, long long nboxes, const void* data,
+                          const void* dest, const int64_t* starts, long long* nitems) {
+  int dev;
+  if (box_geometry(ndim, shape, g_box_origin, extent, nitems)) return -1;
+  if (nboxes < 0) { fprintf(stderr, "blosc_b200: nboxes = %lld is negative\n", nboxes); return -1; }
+  if (nboxes == 0 || !b2_ptr_is_device(starts)) return 0;
+  dev = b2_ptr_is_device(data) ? b2_ptr_device(data) : b2_ptr_is_device(dest) ? b2_ptr_device(dest) : b2_get_device();
+  if (b2_ptr_device(starts) != dev) {
+    fprintf(stderr, "blosc_b200: starts are not on device %d, where the call runs\n", dev);
+    return -1;
+  }
+  return 0;
+}
+
+/* The sizes of a batch of nboxes boxes of `count` items: -1 with a message when its output bytes, or the corners,
+ * offsets and parts its plan keeps (8 * (ndim + 3) bytes a box at most), overflow int64 */
+static int boxes_nbytes(long long nboxes, int ndim, long long count, long long typesize) {
+  if (nboxes > LLONG_MAX / (8 * (ndim + 3)) || (count > 0 && nboxes > LLONG_MAX / (count * typesize))) {
+    fprintf(stderr, "blosc_b200: %lld boxes of %lld bytes overflow int64\n", nboxes, count * typesize);
+    return -1;
+  }
+  return 0;
+}
+
+/* The origin box of a batch (box_build at corner 0) and the check's arguments that follow from the geometry */
+static void boxes_build(int ndim, const int64_t* shape, const int64_t* extent, long long nitems, long long nboxes,
+                        B2Box* box, BoxCheckArgs* ck) {
+  int k;
+  box_build(ndim, shape, g_box_origin, extent, nitems, box);
+  memset(ck, 0, sizeof *ck);
+  ck->box = *box; ck->nboxes = nboxes; ck->ndim = ndim;
+  ck->span = b2_box_unrank(box, box->count - 1) + 1;
+  ck->stride[ndim - 1] = 1;
+  for (k = ndim - 2; k >= 0; k--) ck->stride[k] = ck->stride[k + 1] * shape[k + 1];
+  for (k = 0; k < ndim; k++) ck->hi[k] = shape[k] - extent[k];
+}
+
+/* The check's scratch in w->fplan, which the chunk plans leave alone: for a frame (nchunks > 0), the first failing box
+ * (all ones) and the touched flags of its chunks (zeroed); then the boxes' offsets, for a frame each box's part of the
+ * chunk being read (*part), and the caller's corners (uploaded when they are in host memory).  Fills ck's pointers but
+ * for a chunk's ck->bad, which the chunk plan's record holds.  Returns 0, or -1. */
+static int boxes_scratch(b2_ws* w, const int64_t* starts, long long nchunks, BoxCheckArgs* ck, long long** part) {
+  const size_t o_off = nchunks ? B2_AL(16 + 4 * (size_t)nchunks) : 0, o_part = B2_AL(o_off + 8 * (size_t)ck->nboxes);
+  const size_t o_up = o_part + (nchunks ? 16 * (size_t)ck->nboxes : 0), up = 8 * (size_t)ck->ndim * (size_t)ck->nboxes;
+  uint8_t* base;
+  if (buf_ensure(&w->fplan, o_up + up)) return -1;
+  base = (uint8_t*)w->fplan.p;
+  if (nchunks) {
+    if (b2_memset_dev(base, 0, o_off, w->stream) || b2_memset_dev(base, 0xff, 8, w->stream)) return -1;
+    ck->bad = (unsigned long long*)base; ck->touched = (int*)(base + 16); ck->nchunks = nchunks;
+  }
+  ck->off = (long long*)(base + o_off);
+  *part = nchunks ? (long long*)(base + o_part) : NULL;
+  ck->starts = (const long long*)dev_list(w, starts, b2_ptr_is_device(starts), up, base + o_up);
+  return ck->starts ? 0 : -1;
+}
+
+/* A failing corner: box i of the check's corners (device memory) is read back, and the message names the box, the
+ * first dimension whose coordinate fails and the interval it must lie in.  Returns -1. */
+static int box_bad_corner(b2_ws* w, const BoxCheckArgs* ck, unsigned long long i) {
+  long long c[B2_BOX_MAXDIM];
+  int k;
+  if (copy_any(c, 0, ck->starts + i * (unsigned long long)ck->ndim, 1, 8 * (size_t)ck->ndim, w->stream)) return -1;
+  for (k = 0; k < ck->ndim; k++)
+    if (c[k] < 0 || c[k] > ck->hi[k]) {
+      fprintf(stderr, "blosc_b200: box %llu starts at %lld in dimension %d, not in [0, %lld]\n", i, c[k], k, ck->hi[k]);
+      break;
+    }
+  return -1;
+}
+
+/* One chunk's part of a batch: the chunk (header h, checked) holds the array's flat items [window, window + nbytes /
+ * typesize); the boxes at the offsets ck->off land at d_dst (device memory), box i at i * count * typesize, total bytes
+ * in all; with part (room for two words a box: a frame), only each box's part in the chunk.  check: launch ck's corner
+ * check first, its verdict read back with the plan's record (a chunk call).  Returns total, blosc_d's code when a
+ * touched block fails to decode (nothing is written then), or -1. */
+static long long boxes_read(b2_ws* w, const void* src, int src_dev, const b2_hdr* h, int codec, BoxCheckArgs* ck,
+                            int check, long long window, long long* part, long long total, uint8_t* d_dst) {
+  const int in_place = (h->flags & BLOSC_MEMCPYED) && src_dev;   /* a memcpyed device chunk is read in place */
+  GetitemsPlan rec = {0};
+  BoxesPlanArgs bp;
+  BoxesGatherArgs ga;
+  int rc;
+  memset(&ga, 0, sizeof ga);
+  ga.box = ck->box; ga.off = ck->off; ga.part = part; ga.window = window;
+  ga.total = total; ga.typesize = h->typesize; ga.blocksize = h->blocksize; ga.dst = d_dst;
+  bp.box = ck->box; bp.off = ck->off; bp.nboxes = ck->nboxes; bp.span = ck->span; bp.window = window;
+  bp.part = part; bp.in_place = in_place; bp.pad = 0;
+  bp.per_box = (ck->span * h->typesize + h->blocksize - 1) / h->blocksize + 1;   /* the blocks one box can touch */
+  if (bp.per_box > h->nblocks) bp.per_box = h->nblocks;
+  if (bp.per_box > LLONG_MAX / ck->nboxes) {
+    fprintf(stderr, "blosc_b200: %lld boxes of %lld blocks each are too many to plan\n", ck->nboxes, bp.per_box);
+    return -1;
+  }
+  if (!in_place || check || part) {
+    if (!plan_scratch(w, h, 0, 0, &bp.plan)) return -1;
+    if (check) {
+      ck->bad = &bp.plan.rec->bad_box;
+      if (b2_memset_dev(ck->bad, 0xff, 8, w->stream) || b2_launch_box_check(ck, w->stream)) return -1;
+    }
+    if (((!in_place || part) && b2_launch_boxes_plan(&bp, w->stream)) || read_plan(w, bp.plan.rec, &rec, sizeof rec))
+      return -1;
+    if (check && rec.bad_box != ~0ull) return box_bad_corner(w, ck, rec.bad_box);
+    if (!in_place) ga.slot = bp.plan.slot;
+  }
+  if (touched_source(w, src, src_dev, h, codec, rec.nlisted, rec.has_left, &ga.src, &ga.status)) return -1;
+  if (b2_launch_boxes_gather(&ga, w->stream)) { ws_reset_counters(w); return -1; }
+  rc = read_verdict(w, ga.status);
+  return rc < 0 ? rc : total;
+}
+
+long long blosc_b200_getslices(const void* src, int ndim, const int64_t* shape, const int64_t* extent,
+                               long long nboxes, const int64_t* starts, void* dest) {
+  b2_hdr h;
+  B2Box box;
+  BoxCheckArgs ck;
+  b2_ws* w;
+  uint8_t* d_dst;
+  long long nitems = 0, nbytes, result = -1, *part = NULL;
+  int src_dev, dest_dev, codec = 0, rc;
+  if (boxes_geometry(ndim, shape, extent, nboxes, src, dest, starts, &nitems)) return -1;
+  src_dev = b2_ptr_is_device(src);
+  rc = getitem_header(NULL, src, src_dev, -1, &h, &codec);
+  if (rc) return rc;
+  if (box_nbytes(nitems, h.typesize, (unsigned long long)h.nbytes)) return -1;
+  if (nboxes == 0 || box_empty(ndim, g_box_origin, extent)) return 0;
+  boxes_build(ndim, shape, extent, nitems, nboxes, &box, &ck);
+  if (boxes_nbytes(nboxes, ndim, box.count, h.typesize)) return -1;
+  nbytes = nboxes * box.count * h.typesize;
+  dest_dev = b2_ptr_is_device(dest);
+  if (!(w = ws_acquire())) return -1;
+  if ((d_dst = stage_dest(&w->slots, dest, dest_dev, (size_t)nbytes)) && !boxes_scratch(w, starts, 0, &ck, &part)) {
+    result = boxes_read(w, src, src_dev, &h, codec, &ck, 1, 0, NULL, nbytes, d_dst);
+    if (result > 0 && !dest_dev && d2h_any(w, dest, d_dst, (size_t)result)) result = -1;
+  }
+  ws_release(w);
+  return result;
+}
+
 /* ------------------------------------------------------------------------- */
 /* frames: buffers larger than one chunk (SURVEY.md section 8, row f3)           */
 /* ------------------------------------------------------------------------- */
@@ -2075,6 +2219,67 @@ long long blosc_b200_frame_getslice(const void* frame, size_t framesize, int ndi
     result = sum;
   } while (0);
   ws_release(w);
+  free(f.off);
+  return result;
+}
+
+/* Boxes of the array a frame holds: one corner check over all of them, which also flags the chunks that hold an item
+ * of some box, read back with one sync; then each flagged chunk, in ascending order, reads its part of every box by
+ * the chunk path, clipped to the chunk, and the first failure decides the result.  A host dest is staged in device
+ * memory and copied out once. */
+long long blosc_b200_frame_getslices(const void* frame, size_t framesize, int ndim, const int64_t* shape,
+                                     const int64_t* extent, long long nboxes, const int64_t* starts, void* dest) {
+  size_t c;
+  b2_frame f;
+  long long nitems = 0, ts, ipc, nbytes, got = 0, result = -1;
+  int dest_dev, rc;
+  B2Box box;
+  BoxCheckArgs ck;
+  b2_ws* w;
+  uint8_t *d_dst, *head = NULL;
+  long long* part = NULL;
+  if (!backend_ready()) return -1;
+  if (boxes_geometry(ndim, shape, extent, nboxes, frame, dest, starts, &nitems)) return -1;
+  rc = frame_open_items(frame, framesize, &f);
+  if (rc == -2)
+    fprintf(stderr, "blosc_b200: chunk 0's typesize %lld does not divide the frame's chunksize\n", (long long)f.typesize);
+  if (rc) return -1;
+  ts = (long long)f.typesize; ipc = (long long)f.ipc;
+  dest_dev = b2_ptr_is_device(dest);
+  if (box_nbytes(nitems, ts, (unsigned long long)f.nbytes)) { free(f.off); return -1; }
+  if (nboxes == 0 || box_empty(ndim, g_box_origin, extent)) { free(f.off); return 0; }
+  boxes_build(ndim, shape, extent, nitems, nboxes, &box, &ck);
+  if (boxes_nbytes(nboxes, ndim, box.count, ts)) { free(f.off); return -1; }
+  nbytes = nboxes * box.count * ts;
+  ck.ipc = ipc;
+  if (!(w = ws_acquire())) { free(f.off); return -1; }
+  do {
+    if (!(d_dst = stage_dest(&w->fstage, dest, dest_dev, (size_t)nbytes))) break;
+    if (boxes_scratch(w, starts, (long long)f.nchunks, &ck, &part) || b2_launch_box_check(&ck, w->stream)) break;
+    if (!(head = (uint8_t*)malloc(16 + 4 * f.nchunks)) || d2h_any(w, head, ck.bad, 16 + 4 * f.nchunks)) break;
+    if (*(unsigned long long*)head != ~0ull) { box_bad_corner(w, &ck, *(unsigned long long*)head); break; }
+    for (c = 0; c < f.nchunks; c++) {
+      const long long w0 = (long long)c * ipc, w1 = w0 + ipc < nitems ? w0 + ipc : nitems;
+      b2_hdr h;
+      int codec = 0;
+      if (!((int*)(head + 16))[c]) continue;                               /* no box item in this chunk */
+      got = frame_chunk_header(w, frame, &f, c, &h, &codec);
+      if (got < 0) break;
+      if (got || h.nbytes != (w1 - w0) * ts) {
+        fprintf(stderr, "blosc_b200: chunk %zu holds %d items of %d bytes, not the frame's %lld of %lld\n", c,
+                h.nbytes / h.typesize, h.typesize, w1 - w0, ts);
+        got = -1;
+        break;
+      }
+      got = boxes_read(w, (const uint8_t*)frame + f.off[c], f.dev, &h, codec, &ck, 0, w0, part, nbytes, d_dst);
+      if (got < 0) break;
+    }
+    if (c < f.nchunks) { result = got; break; }
+    if (!dest_dev && d2h_any(w, dest, d_dst, (size_t)nbytes)) break;
+    result = nbytes;
+  } while (0);
+  ws_release(w);
+  free(head);
   free(f.off);
   return result;
 }

@@ -20,6 +20,10 @@
  *   box_touch_kernel, box_gather_kernel (+ plan_scan_kernel<PLAN_SLOT>)
  *                   a box of an N-d array (blosc_b200_getslice): the touched blocks and the
  *                   copy out of them, both from the box alone (B2Box, b2_args.h)
+ *   box_check_kernel, boxes_touch_kernel, boxes_gather_kernel (+ plan_scan_kernel<PLAN_SLOT>)
+ *                   a batch of boxes of one extent (blosc_b200_getslices): the corners' check,
+ *                   the blocks touched by any box and the copy out, from the origin box and one
+ *                   flat offset per box
  */
 #pragma once
 #include "b2_args.h"
@@ -1176,6 +1180,165 @@ extern "C" int b2_launch_box_gather(const BoxGatherArgs* a, b2_stream_t) {
   g_emu_gather_launches++;
   BoxGatherArgs args = *a;
   simt::launch(simt::Dim3((unsigned)ctas), simt::Dim3(GATHER_WARPS * 32), 0, [&] { box_gather_kernel(args); });
+  return 0;
+}
+#endif
+
+
+/* blosc_b200_getslices: K boxes of one extent, box i the origin box moved by off[i] flat items.  The first flat index
+ * >= x (0 <= x <= nitems) of box i, or nitems when there is none: the origin box's answer for x - off[i], moved back. */
+DEV long long box_next_at(const B2Box& b, long long off, long long x) {
+  const long long n = b2_box_next(&b, x > off ? x - off : 0);
+  return n < b.nitems ? n + off : b.nitems;
+}
+
+__global__ void __launch_bounds__(PLAN_THREADS) box_check_kernel(BoxCheckArgs a) {
+  for (long long i = (long long)blockIdx.x * PLAN_THREADS + threadIdx.x; i < a.nboxes;
+       i += (long long)gridDim.x * PLAN_THREADS) {
+    const long long* s = a.starts + i * a.ndim;
+    long long f0 = 0;
+    bool bad = false;
+#pragma unroll
+    for (int k = 0; k < B2_BOX_MAXDIM; k++)
+      if (k < a.ndim) {
+        const long long c = s[k];
+        if (c < 0 || c > a.hi[k]) bad = true;
+        f0 += c * a.stride[k];
+      }
+    if (bad) { atomicMin(a.bad, (unsigned long long)i); f0 = 0; }
+    a.off[i] = f0;
+    if (a.touched && !bad) {                     /* the chunks of the box's span that hold one of its items */
+      for (long long ch = b2_box_div(f0, a.ipc), last = b2_box_div(f0 + a.span - 1, a.ipc); ch <= last; ch++) {
+        const long long w1 = (ch + 1) * a.ipc < a.box.nitems ? (ch + 1) * a.ipc : a.box.nitems;
+        if (box_next_at(a.box, f0, ch * a.ipc) < w1) a.touched[ch] = 1;
+      }
+    }
+  }
+}
+
+/* boxes_touch_kernel, work item (box i, j): the j-th block of box i's span inside the chunk is touched when an item of
+ * the box has a byte in it, the byte test of box_touch_kernel.  Boxes that share a block store the same 1. */
+__global__ void __launch_bounds__(PLAN_THREADS) boxes_touch_kernel(BoxesPlanArgs a) {
+  const long long ts = a.plan.typesize, bs = a.plan.blocksize, nb = a.plan.nbytes, wend = a.window + b2_box_div(nb, ts);
+  for (long long t = (long long)blockIdx.x * PLAN_THREADS + threadIdx.x; t < a.nboxes * a.per_box;
+       t += (long long)gridDim.x * PLAN_THREADS) {
+    const long long i = b2_box_div(t, a.per_box), j = t - i * a.per_box, f0 = a.off[i];
+    if (a.part && j == 0) {                      /* box i's items of flat index in [window, wend), as output bytes */
+      const long long y0 = a.window > f0 ? a.window - f0 : 0, y1 = wend > f0 ? wend - f0 : 0;
+      a.part[2 * i] = b2_box_rank(&a.box, y0 < a.box.nitems ? y0 : a.box.nitems) * ts;
+      a.part[2 * i + 1] = b2_box_rank(&a.box, y1 < a.box.nitems ? y1 : a.box.nitems) * ts;
+    }
+    const long long x0 = f0 > a.window ? f0 : a.window, x1 = f0 + a.span < wend ? f0 + a.span : wend;
+    if (a.in_place || x0 >= x1) continue;
+    const long long lo = (b2_box_div((x0 - a.window) * ts, bs) + j) * bs;
+    if (lo >= (x1 - a.window) * ts) continue;
+    const long long hi = lo + bs < nb ? lo + bs : nb;
+    if (box_next_at(a.box, f0, a.window + b2_box_div(lo, ts)) < a.window + b2_box_div(hi + ts - 1, ts))
+      a.plan.cover[b2_box_div(lo, bs)] = 1;
+  }
+}
+
+/* boxes_gather_kernel: box_gather_kernel's walk over the batch's output bytes, one warp job per GATHER_SPAN bytes.  Run
+ * q belongs to box i = q / (count / run), and its source is the origin box's unrank of its first item plus off[i].
+ * A lane reads box i's offset (and, on a frame, its part of the chunk) again only when its box changes.  The parts
+ * come from the plan: ranking them here put two more division calls in the loop, and the kernel spilled. */
+__global__ void __launch_bounds__(GATHER_WARPS * 32) boxes_gather_kernel(BoxesGatherArgs a) {
+  if (a.status && ld_cg_i32(a.status) < 0) return;       /* a stream failed to decode: dest stays untouched */
+  const long long ts = a.typesize, runb = a.box.run * ts, boxb = a.box.count * ts;
+  const long long rpb = b2_box_div(a.box.count, a.box.run);      /* runs of a box */
+  const unsigned bs = (unsigned)a.blocksize;              /* chunk offsets are below 2^31 */
+  const int lane = lane_id();
+  const long long warps = (long long)gridDim.x * GATHER_WARPS;
+  long long cur = -1, f0 = 0, plo = 0, phi = boxb;       /* box cur's offset and its part [plo, phi) in bytes */
+  auto use_box = [&](long long i) {
+    if (i == cur) return;
+    cur = i;
+    f0 = a.off[i];
+    if (a.part) { plo = a.part[2 * i]; phi = a.part[2 * i + 1]; }
+  };
+  for (long long lo = ((long long)blockIdx.x * GATHER_WARPS + (threadIdx.x >> 5)) * GATHER_SPAN; lo < a.total;
+       lo += warps * GATHER_SPAN) {
+    const long long hi = lo + GATHER_SPAN < a.total ? lo + GATHER_SPAN : a.total;
+    if (runb >= BOX_SHORT_RUN) {
+      for (long long o = lo; o < hi;) {
+        const long long k = b2_box_div(o, runb), u = o - k * runb, i = b2_box_div(k, rpb);
+        use_box(i);
+        const long long gb = o - i * boxb;                 /* the byte's offset in its box */
+        if (gb < plo) { o += plo - gb; continue; }
+        if (gb >= phi) { o += boxb - gb; continue; }
+        unsigned s = (unsigned)((b2_box_unrank(&a.box, (k - i * rpb) * a.box.run) + f0 - a.window) * ts + u);
+        long long n = runb - u < hi - o ? runb - u : hi - o;
+        if (n > phi - gb) n = phi - gb;
+        while (n > 0) {
+          int m = (int)n;
+          const u8* from = a.src + s;
+          if (a.slot) {
+            const unsigned blk = s / bs, left = (blk + 1) * bs - s;
+            if ((unsigned)m > left) m = (int)left;
+            from = a.src + (long long)a.slot[blk] * bs + (s - blk * bs);
+          }
+          warp_copy_vec(a.dst + o, from, m);
+          o += m; s += (unsigned)m; n -= m;
+        }
+      }
+    } else {
+      const long long ka = b2_box_div(lo + runb - 1, runb), kb = b2_box_div(hi + runb - 1, runb);
+      for (long long k = ka + lane; k < kb; k += 32) {
+        const long long i = b2_box_div(k, rpb);
+        use_box(i);
+        long long gs = k * runb, ge = (k + 1) * runb;
+        if (gs < i * boxb + plo) gs = i * boxb + plo;
+        if (ge > i * boxb + phi) ge = i * boxb + phi;
+        if (gs >= ge) continue;
+        unsigned s = (unsigned)((b2_box_unrank(&a.box, (k - i * rpb) * a.box.run) + f0 - a.window) * ts + (gs - k * runb));
+        u8* out = a.dst + gs;
+        const int n = (int)(ge - gs);
+        if (!a.slot) {
+          for (int x = 0; x < n; x++) out[x] = a.src[s + x];
+        } else {
+          unsigned bend = 0;
+          const u8* base = a.src;
+          for (int x = 0; x < n; x++, s++) {
+            if (s >= bend) {
+              const unsigned blk = s / bs;
+              bend = (blk + 1) * bs;
+              base = a.src + (long long)a.slot[blk] * bs - (long long)blk * bs;
+            }
+            out[x] = base[s];
+          }
+        }
+      }
+    }
+  }
+}
+
+#ifdef SIMT_EMU
+/* The emulator's launchers of the batch kernels, as those of the box kernels: the check and the plan's two launches
+ * count as plan launches, the gather as a gather launch. */
+extern "C" int b2_launch_box_check(const BoxCheckArgs* a, b2_stream_t) {
+  if (a->nboxes <= 0) return 0;
+  BoxCheckArgs args = *a;
+  simt::launch(simt::Dim3(emu_range_ctas(a->nboxes)), simt::Dim3(PLAN_THREADS), 0, [&] { box_check_kernel(args); });
+  g_emu_plan_launches++;
+  return 0;
+}
+extern "C" int b2_launch_boxes_plan(const BoxesPlanArgs* a, b2_stream_t) {
+  if (a->plan.nblocks <= 0) return 0;
+  BoxesPlanArgs args = *a;
+  const long long nb = a->plan.nblocks;
+  simt::launch(simt::Dim3(emu_range_ctas(a->nboxes * a->per_box)), simt::Dim3(PLAN_THREADS), 0,
+               [&] { boxes_touch_kernel(args); });
+  simt::launch(simt::Dim3(emu_tiles(nb)), simt::Dim3(PLAN_THREADS), 0, [&] { plan_scan_kernel<PLAN_SLOT>(args.plan, nb); });
+  g_emu_plan_launches += 2;
+  return 0;
+}
+extern "C" int b2_launch_boxes_gather(const BoxesGatherArgs* a, b2_stream_t) {
+  if (a->total <= 0) return 0;
+  long long ctas = (a->total + (long long)GATHER_WARPS * GATHER_SPAN - 1) / ((long long)GATHER_WARPS * GATHER_SPAN);
+  if (ctas > 3) ctas = 3;
+  g_emu_gather_launches++;
+  BoxesGatherArgs args = *a;
+  simt::launch(simt::Dim3((unsigned)ctas), simt::Dim3(GATHER_WARPS * 32), 0, [&] { boxes_gather_kernel(args); });
   return 0;
 }
 #endif

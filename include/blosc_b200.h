@@ -176,6 +176,23 @@ long long blosc_b200_getitems(const void* src, int nranges, const int* starts, c
 long long blosc_b200_getslice(const void* src, int ndim, const int64_t* shape, const int64_t* start,
                               const int64_t* stop, void* dest);
 
+/* A batch of equal-sized boxes in one call: nboxes boxes of extents extent[0..ndim) (host memory), box i at the corner
+ * starts[i][0..ndim) (starts: nboxes x ndim int64, row-major), covering items [starts[i][k], starts[i][k] + extent[k])
+ * of each dimension k of the chunk's C-order array of `shape`.  Box i is written to dest + i * B, B = prod(extent) *
+ * typesize, as one contiguous C-order array, so dest is numpy's np.stack of the K slices.  Boxes may overlap, repeat
+ * and come in any order.  src / dest are host or device memory as in blosc_b200_getslice.  starts may be host memory
+ * (uploaded) or device memory on the call's device, chosen as blosc_b200_getitems chooses it (otherwise -1 with a
+ * message before anything is read).  The corners are checked and every box planned on the GPU: each touched block is
+ * decoded once, and the launches, read-backs and syncs do not grow with nboxes.  Returns the bytes written, nboxes * B;
+ * 0 when nboxes is 0 or an extent is 0, with nothing launched and starts never read.  -1 with a message on stderr,
+ * before anything is launched, when ndim is not in 1..8, a shape or extent entry is negative, extent[k] > shape[k],
+ * the shape's product overflows int64 or times the typesize is not the chunk's nbytes, nboxes < 0, or nboxes * B
+ * overflows int64.  A corner with starts[i][k] < 0 or > shape[k] - extent[k] returns -1 with one message naming the
+ * first such box, and nothing is decoded or written.  The chunk header is checked as blosc_getitem checks it, with its
+ * codes.  A touched block that fails to decode returns blosc_d's code and leaves dest untouched. */
+long long blosc_b200_getslices(const void* src, int ndim, const int64_t* shape, const int64_t* extent,
+                               long long nboxes, const int64_t* starts, void* dest);
+
 /* Frames: buffers larger than one chunk (a Blosc-1 chunk holds at most BLOSC_MAX_BUFFERSIZE
  * bytes, blosc.h:40).  The buffer is cut into `chunksize`-byte pieces (0 = 256 MiB; rounded down
  * to a multiple of typesize), each compressed exactly as blosc_compress_ctx() would with
@@ -208,6 +225,13 @@ long long blosc_b200_frame_getitems(const void* frame, size_t framesize, size_t 
  * nbytes. */
 long long blosc_b200_frame_getslice(const void* frame, size_t framesize, int ndim, const int64_t* shape,
                                     const int64_t* start, const int64_t* stop, void* dest);
+/* blosc_b200_getslices over a frame: the whole frame holds the C-order array, as in blosc_b200_frame_getslice, and a
+ * box may cross chunk boundaries.  The corners are checked once; the chunks that hold an item of some box are then
+ * read in ascending order, each decoding its touched blocks once for all boxes.  The first failure decides the result,
+ * as in blosc_b200_frame_getslice: on a failure a host dest is untouched; a device dest may hold parts of earlier
+ * chunks. */
+long long blosc_b200_frame_getslices(const void* frame, size_t framesize, int ndim, const int64_t* shape,
+                                     const int64_t* extent, long long nboxes, const int64_t* starts, void* dest);
 int       blosc_b200_frame_info(const void* frame, size_t framesize, size_t* nbytes, size_t* cbytes,
                                 size_t* chunksize, size_t* nchunks);
 long long blosc_b200_frame_chunk(const void* frame, size_t framesize, size_t i, size_t* chunk_cbytes);

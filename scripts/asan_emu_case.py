@@ -3,8 +3,8 @@
   LD_PRELOAD=$(gcc -print-file-name=libasan.so) ASAN_OPTIONS=detect_leaks=0 python scripts/asan_emu_case.py
 exact / fast / lz4hc / BloscLZ paths, exact-size buffers, damaged chunks, crafted and damaged zstd frames and zlib streams,
 crafted, random and damaged LZ4 and BloscLZ streams, the snappy encoder (serial and pool maxout rules), crafted,
-random and damaged snappy streams, and item ranges and boxes of whole and damaged chunks and frames, in host and in
-device memory."""
+random and damaged snappy streams, and item ranges, boxes and batches of boxes of whole and damaged chunks and frames,
+in host and in device memory."""
 import os, sys, ctypes as C, numpy as np
 sys.path.insert(0, os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), 'tests'))
 from datagen import gen, compress, decompress
@@ -142,14 +142,15 @@ for t in range(300):                        # crafted streams, then random damag
     assert (r==n)==(why is None) and (why is not None or out.tobytes()==got)
     cases+=1
 os.environ.pop('BLOSC_B200_SNAPPY', None)
-# item ranges and boxes of a chunk and of a frame: the host plan, the GPU plans and the box plan, each with the chunk or
+# item ranges, boxes and batches of boxes of a chunk and of a frame: the host plan, the GPU plans and the box plan, each with the chunk or
 # frame in host memory (the touched blocks staged, the block list read back) and then in device memory
 # (emu_set_all_device: lists and dest too); compressed, memcpyed and damaged chunks
 vp,sz,ll=C.c_void_p,C.c_size_t,C.c_longlong
 P=lambda a: a.ctypes.data_as(vp)
 for f,res,args in (("blosc_b200_getitems",ll,[vp,C.c_int,vp,vp,vp]),("blosc_b200_getslice",ll,[vp,C.c_int,vp,vp,vp,vp]),
                    ("blosc_b200_frame_bound",sz,[sz,sz,sz]),("blosc_b200_frame_compress",ll,[C.c_int,C.c_int,sz,sz,vp,vp,sz,C.c_char_p,sz,sz,C.c_int]),
-                   ("blosc_b200_frame_getitems",ll,[vp,sz,sz,vp,vp,vp]),("blosc_b200_frame_getslice",ll,[vp,sz,C.c_int,vp,vp,vp,vp])):
+                   ("blosc_b200_frame_getitems",ll,[vp,sz,sz,vp,vp,vp]),("blosc_b200_frame_getslice",ll,[vp,sz,C.c_int,vp,vp,vp,vp]),
+                   ("blosc_b200_getslices",ll,[vp,C.c_int,vp,vp,ll,vp,vp]),("blosc_b200_frame_getslices",ll,[vp,sz,C.c_int,vp,vp,ll,vp,vp])):
     getattr(emu,f).restype=res; getattr(emu,f).argtypes=args
 emu.emu_set_all_device.argtypes=[C.c_int]
 irng=np.random.default_rng(11)
@@ -162,6 +163,10 @@ st=np.array([r[0] for r in ranges],np.int32); nt=np.array([r[1] for r in ranges]
 want_items=b"".join(src[s*ts:(s+k)*ts].tobytes() for s,k in ranges)
 sh=np.array(shape,np.int64); b0=np.array(box[0],np.int64); b1=np.array(box[1],np.int64)
 fst=st.astype(np.uint64); fnt=nt.astype(np.uint64)
+ext=np.array([9,31],np.int64)                 # a batch of boxes, overlapping and on the array's edges, and a bad corner
+corners=np.array([[0,0],[291,219],[100,7],[100,7],[150,200]]+[[int(a),int(b)] for a,b in zip(irng.integers(0,292,40),irng.integers(0,220,40))],np.int64)
+want_boxes=b"".join(arr[a:a+9,b:b+31].tobytes() for a,b in corners)
+bad=corners.copy(); bad[30,1]=220
 for comp,shuf,cl in (("lz4",1,5),("blosclz",2,5),("lz4",1,0)):
     dest=np.zeros(n+16,np.uint8)
     r=emu.blosc_compress_ctx(C.c_int(cl),C.c_int(shuf),C.c_size_t(ts),C.c_size_t(n),P(src),P(dest),C.c_size_t(n+16),comp.encode(),C.c_size_t(4096),C.c_int(1))
@@ -182,7 +187,11 @@ for comp,shuf,cl in (("lz4",1,5),("blosclz",2,5),("lz4",1,0)):
                 out=np.zeros(len(want_box),np.uint8)
                 g=emu.blosc_b200_getslice(P(c),2,P(sh),P(b0),P(b1),P(out))
                 assert c is not chunk or (g==len(want_box) and out.tobytes()==want_box)
-                cases+=2
+                out=np.zeros(len(want_boxes),np.uint8)
+                g=emu.blosc_b200_getslices(P(c),2,P(sh),P(ext),len(corners),P(corners),P(out))
+                assert c is not chunk or (g==len(want_boxes) and out.tobytes()==want_boxes)
+                assert emu.blosc_b200_getslices(P(c),2,P(sh),P(ext),len(bad),P(bad),P(out))<0
+                cases+=4
             for f in [frame]+[frame.copy() for _ in range(2)]:
                 if f is not frame: pos=irng.integers(100,fb,6); f[pos]=irng.integers(0,256,6,dtype=np.uint8)
                 out=np.zeros(len(want_items),np.uint8)
@@ -191,7 +200,11 @@ for comp,shuf,cl in (("lz4",1,5),("blosclz",2,5),("lz4",1,0)):
                 out=np.zeros(len(want_box),np.uint8)
                 g=emu.blosc_b200_frame_getslice(P(f),fb,2,P(sh),P(b0),P(b1),P(out))
                 assert f is not frame or (g==len(want_box) and out.tobytes()==want_box)
-                cases+=2
+                out=np.zeros(len(want_boxes),np.uint8)
+                g=emu.blosc_b200_frame_getslices(P(f),fb,2,P(sh),P(ext),len(corners),P(corners),P(out))
+                assert f is not frame or (g==len(want_boxes) and out.tobytes()==want_boxes)
+                assert emu.blosc_b200_frame_getslices(P(f),fb,2,P(sh),P(ext),len(bad),P(bad),P(out))<0
+                cases+=4
         finally:
             emu.emu_set_all_device(0)
 print("asan workload ok, cases", cases)
