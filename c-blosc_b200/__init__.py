@@ -71,6 +71,10 @@ def _load(path: str) -> C.CDLL:
     lib.blosc_b200_getslice.argtypes = [vp, ci, vp, vp, vp, vp]
     lib.blosc_b200_frame_getslice.restype = ll
     lib.blosc_b200_frame_getslice.argtypes = [vp, sz, ci, vp, vp, vp, vp]
+    lib.blosc_b200_getslice_step.restype = ll
+    lib.blosc_b200_getslice_step.argtypes = [vp, ci, vp, vp, vp, vp, vp]
+    lib.blosc_b200_frame_getslice_step.restype = ll
+    lib.blosc_b200_frame_getslice_step.argtypes = [vp, sz, ci, vp, vp, vp, vp, vp]
     lib.blosc_b200_getslices.restype = ll
     lib.blosc_b200_getslices.argtypes = [vp, ci, vp, vp, ll, vp, vp]
     lib.blosc_b200_frame_getslices.restype = ll
@@ -163,12 +167,27 @@ def _box(shape, start, stop):
     return g
 
 
-def getslice(src, shape, start, stop, dest):
+def _step(sh, step):
+    """step as an int64 host array of the shape's length"""
+    import numpy as np
+    t = np.ascontiguousarray(step, dtype=np.int64).reshape(-1)
+    if t.size != sh.size:
+        raise ValueError(f"shape and step have {sh.size} and {t.size} entries")
+    return t
+
+
+def getslice(src, shape, start, stop, dest, step=None):
     """A box of the C-order array of `shape` that the chunk holds (blosc_b200_getslice): items [start[k], stop[k]) of
-    each dimension, written to `dest` as one contiguous C-order array.  Returns the bytes written, or a negative code
-    (dest is then untouched)."""
+    each dimension, written to `dest` as one contiguous C-order array.  With `step` (one positive int per dimension),
+    every step[k]-th of them (blosc_b200_getslice_step): numpy's a[start:stop:step], made contiguous.  Returns the bytes
+    written, or a negative code (dest is then untouched)."""
     sh, st, sp = _box(shape, start, stop)
-    return int(lib.blosc_b200_getslice(_ptr(src), sh.size, sh.ctypes.data, st.ctypes.data, sp.ctypes.data, _ptr(dest)))
+    if step is None:
+        return int(lib.blosc_b200_getslice(_ptr(src), sh.size, sh.ctypes.data, st.ctypes.data, sp.ctypes.data,
+                                           _ptr(dest)))
+    t = _step(sh, step)
+    return int(lib.blosc_b200_getslice_step(_ptr(src), sh.size, sh.ctypes.data, st.ctypes.data, sp.ctypes.data,
+                                            t.ctypes.data, _ptr(dest)))
 
 
 def _boxes(shape, extent, starts):
@@ -228,11 +247,16 @@ def frame_getitems(frame, framesize, starts, nitems, dest):
     return int(lib.blosc_b200_frame_getitems(_ptr(frame), framesize, st[2], st[1], n[1], _ptr(dest)))
 
 
-def frame_getslice(frame, framesize, shape, start, stop, dest):
-    """getslice over the array a frame holds (blosc_b200_frame_getslice); the box may cross chunk boundaries."""
+def frame_getslice(frame, framesize, shape, start, stop, dest, step=None):
+    """getslice over the array a frame holds (blosc_b200_frame_getslice, or blosc_b200_frame_getslice_step with
+    `step`); the box may cross chunk boundaries."""
     sh, st, sp = _box(shape, start, stop)
-    return int(lib.blosc_b200_frame_getslice(_ptr(frame), framesize, sh.size, sh.ctypes.data, st.ctypes.data,
-                                             sp.ctypes.data, _ptr(dest)))
+    if step is None:
+        return int(lib.blosc_b200_frame_getslice(_ptr(frame), framesize, sh.size, sh.ctypes.data, st.ctypes.data,
+                                                 sp.ctypes.data, _ptr(dest)))
+    t = _step(sh, step)
+    return int(lib.blosc_b200_frame_getslice_step(_ptr(frame), framesize, sh.size, sh.ctypes.data, st.ctypes.data,
+                                                  sp.ctypes.data, t.ctypes.data, _ptr(dest)))
 
 
 def frame_getslices(frame, framesize, shape, extent, starts, dest):

@@ -280,23 +280,29 @@ typedef struct FramePlanArgs {
 } FramePlanArgs;
 enum { FPLAN_DST = 3, FPLAN_COUNT = 4, FPLAN_BASE = 5, FPLAN_TOUCH = 6 };
 
-/* A box of an N-d C-order array (blosc_b200_getslice): items [start[k], stop[k]) of each dimension, none of them empty.
- * The host builds it after merging every dimension whose box covers its whole extent into the dimension before it, so
- * the innermost run of consecutive flat items is as long as the box allows.  Its arithmetic is the three functions
- * below, shared by the host (which touched chunks, where their output starts) and the kernels (which blocks a chunk's
- * part touches, where each output byte comes from).  Every loop runs over the fixed B2_BOX_MAXDIM with a guard, so the
- * kernels index the box with constants only. */
+/* A box of an N-d C-order array (blosc_b200_getslice): items start[k], start[k] + step[k], ... below stop[k] of each
+ * dimension, none of them empty.  The host builds it normalised (blosc_b200.c box_build): each stop is the last
+ * selected coordinate + 1, a dimension that selects one coordinate has step 1, and every dimension that the box covers
+ * whole with step 1 is merged into the dimension before it when that one's step is 1 too, so the innermost run of
+ * consecutive flat items is as long as the box allows.  A box whose steps are all 1 is then `stepped` 0.  Its
+ * arithmetic is the three functions below, shared by the host (which touched chunks, where their output starts) and
+ * the kernels (which blocks a chunk's part touches, where each output byte comes from).  Each takes `stepped`, which
+ * the kernels pass as a template constant: with 0 the step code folds away and step / ext are never read.  Every loop
+ * runs over the fixed B2_BOX_MAXDIM with a guard, so the kernels index the box with constants only. */
 #define B2_BOX_MAXDIM 8
 typedef struct B2Box {
   int ndim;                           /* dimensions after merging, 1..B2_BOX_MAXDIM */
-  int pad;
+  int stepped;                        /* some step[k] > 1 */
   long long start[B2_BOX_MAXDIM];
-  long long stop[B2_BOX_MAXDIM];
+  long long stop[B2_BOX_MAXDIM];      /* the last selected coordinate + 1 */
   long long stride[B2_BOX_MAXDIM];    /* flat items per step of dimension k: the product of the shape after k */
   long long inner[B2_BOX_MAXDIM];     /* box items per step of dimension k: the product of the extents after k */
-  long long run;                      /* items of one innermost run: the extent of the last dimension */
+  long long run;                      /* items of one innermost run: the extent of the last dimension, or 1 when its
+                                       * step is > 1 */
   long long nitems;                   /* items of the whole array: b2_box_next's end sentinel */
   long long count;                    /* items of the box */
+  long long step[B2_BOX_MAXDIM];      /* >= 1 */
+  long long ext[B2_BOX_MAXDIM];       /* selected coordinates of dimension k */
 } B2Box;
 
 /* a / b for a >= 0, b > 0.  On the device it makes no call to the 64-bit division routine, whose saved registers
@@ -316,9 +322,10 @@ static inline B2_HD long long b2_box_div(long long a, long long b) {
 #endif
 }
 
-/* The smallest flat index >= x (0 <= x <= nitems) that lies in the box; nitems when there is none */
-static inline B2_HD long long b2_box_next(const B2Box* b, long long x) {
-  long long c[B2_BOX_MAXDIM], r = x, v = 0;
+/* The smallest flat index >= x (0 <= x <= nitems) that lies in the box; nitems when there is none.  A coordinate
+ * inside [start, stop) but off its dimension's lattice moves up to the next lattice point, or carries past the last. */
+static inline B2_HD long long b2_box_next(const B2Box* b, long long x, int stepped) {
+  long long c[B2_BOX_MAXDIM], r = x, v = 0, lift = 0;
   int k, bad = -1, below = 0, p = -1;
 #pragma unroll
   for (k = 0; k < B2_BOX_MAXDIM; k++) {
@@ -327,17 +334,26 @@ static inline B2_HD long long b2_box_next(const B2Box* b, long long x) {
       c[k] = b2_box_div(r, b->stride[k]);
       r -= c[k] * b->stride[k];
       if (bad < 0 && (c[k] < b->start[k] || c[k] >= b->stop[k])) { bad = k; below = c[k] < b->start[k]; }
+      else if (stepped && bad < 0) {
+        const long long o = c[k] - b->start[k], q = b2_box_div(o, b->step[k]);
+        if (o != q * b->step[k]) {    /* off the lattice: up to the next point (>= 1) when it is below stop */
+          bad = k; lift = b->start[k] + (q + 1) * b->step[k]; below = lift < b->stop[k];
+        }
+      }
     }
   }
   if (bad < 0) return x;
-  if (below) {                      /* dimension `bad` moves up to its start, the ones after it to theirs */
+  if (below) {                      /* dimension `bad` moves up to its start (or lift), the ones after it to theirs */
     p = bad;
 #pragma unroll
     for (k = 0; k < B2_BOX_MAXDIM; k++) if (k == bad) v = b->start[k];
+    if (stepped && lift) v = lift;
   } else {                          /* past the box in `bad`: carry into the last dimension before it that has room */
 #pragma unroll
-    for (k = B2_BOX_MAXDIM - 1; k >= 0; k--)
-      if (p < 0 && k < bad && c[k] + 1 < b->stop[k]) { p = k; v = c[k] + 1; }
+    for (k = B2_BOX_MAXDIM - 1; k >= 0; k--) {
+      const long long s = stepped ? b->step[k] : 1;
+      if (p < 0 && k < bad && c[k] + s < b->stop[k]) { p = k; v = c[k] + s; }
+    }
     if (p < 0) return b->nitems;
   }
   r = 0;
@@ -348,7 +364,7 @@ static inline B2_HD long long b2_box_next(const B2Box* b, long long x) {
 }
 
 /* How many box items have a flat index < x (0 <= x <= nitems) */
-static inline B2_HD long long b2_box_rank(const B2Box* b, long long x) {
+static inline B2_HD long long b2_box_rank(const B2Box* b, long long x, int stepped) {
   long long r = x, rank = 0;
   int k;
 #pragma unroll
@@ -357,15 +373,23 @@ static inline B2_HD long long b2_box_rank(const B2Box* b, long long x) {
       const long long c = b2_box_div(r, b->stride[k]);
       r -= c * b->stride[k];
       if (c < b->start[k]) return rank;
-      if (c >= b->stop[k]) return rank + (b->stop[k] - b->start[k]) * b->inner[k];
-      rank += (c - b->start[k]) * b->inner[k];
+      if (stepped) {
+        long long o, q;
+        if (c >= b->stop[k]) return rank + b->ext[k] * b->inner[k];
+        o = c - b->start[k]; q = b2_box_div(o, b->step[k]);
+        rank += q * b->inner[k];
+        if (o != q * b->step[k]) return rank + b->inner[k];   /* off the lattice: lattice point q lies before x */
+      } else {
+        if (c >= b->stop[k]) return rank + (b->stop[k] - b->start[k]) * b->inner[k];
+        rank += (c - b->start[k]) * b->inner[k];
+      }
     }
   }
   return rank;
 }
 
 /* The flat index of box item p (0 <= p < count, C order inside the box) */
-static inline B2_HD long long b2_box_unrank(const B2Box* b, long long p) {
+static inline B2_HD long long b2_box_unrank(const B2Box* b, long long p, int stepped) {
   long long f = 0;
   int k;
 #pragma unroll
@@ -373,11 +397,11 @@ static inline B2_HD long long b2_box_unrank(const B2Box* b, long long p) {
     if (k < b->ndim) {
       long long q = p;
       if (k > 0) {
-        const long long e = b->stop[k] - b->start[k];
+        const long long e = stepped ? b->ext[k] : b->stop[k] - b->start[k];
         p = b2_box_div(p, e);
         q -= p * e;
       }
-      f += (b->start[k] + q) * b->stride[k];
+      f += (b->start[k] + (stepped ? q * b->step[k] : q)) * b->stride[k];
     }
   }
   return f;

@@ -435,14 +435,16 @@ extern "C" int b2_launch_fplan_scatter(const FramePlanArgs* a, b2_stream_t s) {
   return 0;
 }
 
-/* the box plan of getslice, counted as plan launches: box_touch_kernel, one thread per block, then the PLAN_SLOT scan of
- * the getitems plan over the blocks */
+/* the box plan of getslice, counted as plan launches: box_touch_kernel (its stepped instantiation for a stepped box),
+ * one thread per block, then the PLAN_SLOT scan of the getitems plan over the blocks */
 extern "C" int b2_launch_box_plan(const BoxPlanArgs* a, b2_stream_t s) {
   const long long nb = a->plan.nblocks;
   if (nb <= 0) return 0;
   {
     ProfScope ps(B2_K_PLAN, s->s);
-    box_touch_kernel<<<(unsigned)((nb + PLAN_THREADS - 1) / PLAN_THREADS), PLAN_THREADS, 0, s->s>>>(*a);
+    const unsigned ctas = (unsigned)((nb + PLAN_THREADS - 1) / PLAN_THREADS);
+    if (a->box.stepped) box_touch_kernel<true><<<ctas, PLAN_THREADS, 0, s->s>>>(*a);
+    else box_touch_kernel<false><<<ctas, PLAN_THREADS, 0, s->s>>>(*a);
     CK(cudaGetLastError());
   }
   ProfScope ps(B2_K_PLAN, s->s);
@@ -451,13 +453,14 @@ extern "C" int b2_launch_box_plan(const BoxPlanArgs* a, b2_stream_t s) {
   return 0;
 }
 
-/* the box gather of getslice, counted as a gather launch */
+/* the box gather of getslice (stepped or not, as the plan), counted as a gather launch */
 extern "C" int b2_launch_box_gather(const BoxGatherArgs* a, b2_stream_t s) {
   if (a->total <= 0) return 0;
   long long ctas = (a->total + (long long)GATHER_WARPS * GATHER_SPAN - 1) / ((long long)GATHER_WARPS * GATHER_SPAN);
   if (ctas > (long long)num_sms() * 8) ctas = (long long)num_sms() * 8;
   ProfScope ps(B2_K_GATHER, s->s);
-  box_gather_kernel<<<(unsigned)ctas, GATHER_WARPS * 32, 0, s->s>>>(*a);
+  if (a->box.stepped) box_gather_kernel<true><<<(unsigned)ctas, GATHER_WARPS * 32, 0, s->s>>>(*a);
+  else box_gather_kernel<false><<<(unsigned)ctas, GATHER_WARPS * 32, 0, s->s>>>(*a);
   CK(cudaGetLastError());
   return 0;
 }

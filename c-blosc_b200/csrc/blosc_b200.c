@@ -1463,29 +1463,48 @@ static int box_empty(int ndim, const int64_t* start, const int64_t* stop) {
   return 0;
 }
 
-/* The canonical box of a non-empty, checked one: every dimension that the box covers whole is merged into the one
- * before it, so the innermost run is as long as it can be. */
-static void box_build(int ndim, const int64_t* shape, const int64_t* start, const int64_t* stop, long long nitems,
-                      B2Box* b) {
+/* Every step >= 1 (step == NULL: all ones); -1 with a message naming the first dimension whose step is not */
+static int box_steps(int ndim, const int64_t* step) {
+  int k;
+  for (k = 0; step && k < ndim; k++)
+    if (step[k] < 1) {
+      fprintf(stderr, "blosc_b200: step[%d] = %lld is not >= 1\n", k, (long long)step[k]);
+      return -1;
+    }
+  return 0;
+}
+
+/* The canonical box of a non-empty, checked one with steps (NULL: all ones), normalised in this order: each stop
+ * becomes the last selected coordinate + 1; a dimension that selects one coordinate gets step 1; every dimension that
+ * the box covers whole with step 1 is merged into the one before it when that one's step is 1 too (merged into a
+ * stepped dimension, the selection would not be an arithmetic progression), so the innermost run is as long as it can
+ * be.  The innermost run is the last extent, or 1 item when the last step is > 1.  A box whose steps are all 1 is
+ * then exactly the step-less box, and `stepped` is 0. */
+static void box_build(int ndim, const int64_t* shape, const int64_t* start, const int64_t* stop, const int64_t* step,
+                      long long nitems, B2Box* b) {
   long long sh[B2_BOX_MAXDIM];
   int k, n = 0;
   memset(b, 0, sizeof *b);
   for (k = 0; k < ndim; k++) {
-    if (n > 0 && start[k] == 0 && stop[k] == shape[k]) {
+    const long long t = step ? step[k] : 1, e = (stop[k] - start[k] - 1) / t + 1;   /* e >= 1: no overflow */
+    const long long last = start[k] + (e - 1) * t, u = e == 1 ? 1 : t;
+    if (n > 0 && u == 1 && b->step[n - 1] == 1 && start[k] == 0 && last + 1 == shape[k]) {
       sh[n - 1] *= shape[k]; b->start[n - 1] *= shape[k]; b->stop[n - 1] *= shape[k];
     } else {
-      sh[n] = shape[k]; b->start[n] = start[k]; b->stop[n] = stop[k];
+      sh[n] = shape[k]; b->start[n] = start[k]; b->stop[n] = last + 1; b->step[n] = u;
+      b->stepped |= u > 1;
       n++;
     }
   }
   b->ndim = n;
+  for (k = 0; k < n; k++) b->ext[k] = (b->stop[k] - b->start[k] - 1) / b->step[k] + 1;
   b->stride[n - 1] = 1; b->inner[n - 1] = 1;
   for (k = n - 2; k >= 0; k--) {
     b->stride[k] = b->stride[k + 1] * sh[k + 1];
-    b->inner[k] = b->inner[k + 1] * (b->stop[k + 1] - b->start[k + 1]);
+    b->inner[k] = b->inner[k + 1] * b->ext[k + 1];
   }
-  b->run = b->stop[n - 1] - b->start[n - 1];
-  b->count = b->inner[0] * (b->stop[0] - b->start[0]);
+  b->run = b->step[n - 1] == 1 ? b->ext[n - 1] : 1;
+  b->count = b->inner[0] * b->ext[0];
   b->nitems = nitems;
 }
 
@@ -1494,8 +1513,8 @@ static void box_build(int ndim, const int64_t* shape, const int64_t* start, cons
  * code when a touched block fails to decode (nothing is written then), or -1. */
 static long long getslice_chunk(b2_ws* w, const void* src, int src_dev, const b2_hdr* h, int codec, const B2Box* box,
                                 long long window, uint8_t* d_dst) {
-  const long long ts = h->typesize, p0 = b2_box_rank(box, window);
-  const long long total = (b2_box_rank(box, window + h->nbytes / ts) - p0) * ts;
+  const long long ts = h->typesize, p0 = b2_box_rank(box, window, box->stepped);
+  const long long total = (b2_box_rank(box, window + h->nbytes / ts, box->stepped) - p0) * ts;
   GetitemsPlan rec = {0};
   BoxGatherArgs ga;
   int rc;
@@ -1517,21 +1536,21 @@ static long long getslice_chunk(b2_ws* w, const void* src, int src_dev, const b2
   return rc < 0 ? rc : total;
 }
 
-long long blosc_b200_getslice(const void* src, int ndim, const int64_t* shape, const int64_t* start,
-                              const int64_t* stop, void* dest) {
+long long blosc_b200_getslice_step(const void* src, int ndim, const int64_t* shape, const int64_t* start,
+                                   const int64_t* stop, const int64_t* step, void* dest) {
   b2_hdr h;
   B2Box box;
   b2_ws* w;
   uint8_t* d_dst;
   long long nitems = 0, result = -1;
   int src_dev, dest_dev, codec = 0, rc;
-  if (box_geometry(ndim, shape, start, stop, &nitems)) return -1;
+  if (box_geometry(ndim, shape, start, stop, &nitems) || box_steps(ndim, step)) return -1;
   src_dev = b2_ptr_is_device(src);
   rc = getitem_header(NULL, src, src_dev, -1, &h, &codec);
   if (rc) return rc;
   if (box_nbytes(nitems, h.typesize, (unsigned long long)h.nbytes)) return -1;
   if (box_empty(ndim, start, stop)) return 0;
-  box_build(ndim, shape, start, stop, nitems, &box);
+  box_build(ndim, shape, start, stop, step, nitems, &box);
   dest_dev = b2_ptr_is_device(dest);
   if (!(w = ws_acquire())) return -1;
   if ((d_dst = stage_dest(&w->slots, dest, dest_dev, (size_t)(box.count * h.typesize)))) {
@@ -1540,6 +1559,11 @@ long long blosc_b200_getslice(const void* src, int ndim, const int64_t* shape, c
   }
   ws_release(w);
   return result;
+}
+
+long long blosc_b200_getslice(const void* src, int ndim, const int64_t* shape, const int64_t* start,
+                              const int64_t* stop, void* dest) {
+  return blosc_b200_getslice_step(src, ndim, shape, start, stop, NULL, dest);
 }
 
 /* The checks of getslices that need no data: box_geometry on the box [0, extent), the count of boxes, and corners in
@@ -1575,10 +1599,10 @@ static int boxes_nbytes(long long nboxes, int ndim, long long count, long long t
 static void boxes_build(int ndim, const int64_t* shape, const int64_t* extent, long long nitems, long long nboxes,
                         B2Box* box, BoxCheckArgs* ck) {
   int k;
-  box_build(ndim, shape, g_box_origin, extent, nitems, box);
+  box_build(ndim, shape, g_box_origin, extent, NULL, nitems, box);
   memset(ck, 0, sizeof *ck);
   ck->box = *box; ck->nboxes = nboxes; ck->ndim = ndim;
-  ck->span = b2_box_unrank(box, box->count - 1) + 1;
+  ck->span = b2_box_unrank(box, box->count - 1, 0) + 1;
   ck->stride[ndim - 1] = 1;
   for (k = ndim - 2; k >= 0; k--) ck->stride[k] = ck->stride[k + 1] * shape[k + 1];
   for (k = 0; k < ndim; k++) ck->hi[k] = shape[k] - extent[k];
@@ -2172,8 +2196,8 @@ long long blosc_b200_frame_getitems(const void* frame, size_t framesize, size_t 
  * in dest follow from the box (b2_box_next, b2_box_rank on the chunks' item windows), and each touched chunk, in
  * ascending order, is read by the chunk path; the first failure decides the result.  A host dest is staged in device
  * memory and copied out once, so it is untouched on a failure. */
-long long blosc_b200_frame_getslice(const void* frame, size_t framesize, int ndim, const int64_t* shape,
-                                    const int64_t* start, const int64_t* stop, void* dest) {
+long long blosc_b200_frame_getslice_step(const void* frame, size_t framesize, int ndim, const int64_t* shape,
+                                         const int64_t* start, const int64_t* stop, const int64_t* step, void* dest) {
   size_t c;
   b2_frame f;
   long long nitems = 0, ts, ipc, sum = 0, got = 0, result = -1;
@@ -2182,7 +2206,7 @@ long long blosc_b200_frame_getslice(const void* frame, size_t framesize, int ndi
   b2_ws* w;
   uint8_t* d_dst;
   if (!backend_ready()) return -1;
-  if (box_geometry(ndim, shape, start, stop, &nitems)) return -1;
+  if (box_geometry(ndim, shape, start, stop, &nitems) || box_steps(ndim, step)) return -1;
   rc = frame_open_items(frame, framesize, &f);
   if (rc == -2)
     fprintf(stderr, "blosc_b200: chunk 0's typesize %lld does not divide the frame's chunksize\n", (long long)f.typesize);
@@ -2191,7 +2215,7 @@ long long blosc_b200_frame_getslice(const void* frame, size_t framesize, int ndi
   dest_dev = b2_ptr_is_device(dest);
   if (box_nbytes(nitems, ts, (unsigned long long)f.nbytes)) { free(f.off); return -1; }
   if (box_empty(ndim, start, stop)) { free(f.off); return 0; }
-  box_build(ndim, shape, start, stop, nitems, &box);
+  box_build(ndim, shape, start, stop, step, nitems, &box);
   if (!(w = ws_acquire())) { free(f.off); return -1; }
   do {
     if (!(d_dst = stage_dest(&w->fstage, dest, dest_dev, (size_t)(box.count * ts)))) break;
@@ -2199,7 +2223,7 @@ long long blosc_b200_frame_getslice(const void* frame, size_t framesize, int ndi
       const long long w0 = (long long)c * ipc, w1 = w0 + ipc < nitems ? w0 + ipc : nitems;
       b2_hdr h;
       int codec = 0;
-      if (b2_box_next(&box, w0) >= w1) continue;                          /* no box item in this chunk */
+      if (b2_box_next(&box, w0, box.stepped) >= w1) continue;             /* no box item in this chunk */
       got = frame_chunk_header(w, frame, &f, c, &h, &codec);
       if (got < 0) break;
       if (got || h.nbytes != (w1 - w0) * ts) {
@@ -2209,7 +2233,7 @@ long long blosc_b200_frame_getslice(const void* frame, size_t framesize, int ndi
         break;
       }
       got = getslice_chunk(w, (const uint8_t*)frame + f.off[c], f.dev, &h, codec, &box, w0,
-                           d_dst + b2_box_rank(&box, w0) * ts);
+                           d_dst + b2_box_rank(&box, w0, box.stepped) * ts);
       if (got < 0) break;
       sum += got;
     }
@@ -2221,6 +2245,11 @@ long long blosc_b200_frame_getslice(const void* frame, size_t framesize, int ndi
   ws_release(w);
   free(f.off);
   return result;
+}
+
+long long blosc_b200_frame_getslice(const void* frame, size_t framesize, int ndim, const int64_t* shape,
+                                    const int64_t* start, const int64_t* stop, void* dest) {
+  return blosc_b200_frame_getslice_step(frame, framesize, ndim, shape, start, stop, NULL, dest);
 }
 
 /* Boxes of the array a frame holds: one corner check over all of them, which also flags the chunks that hold an item

@@ -18,8 +18,9 @@
  *                   the same over a frame (blosc_b200_frame_getitems): the ranges cut into
  *                   one piece list per chunk, each read by the chunk plan
  *   box_touch_kernel, box_gather_kernel (+ plan_scan_kernel<PLAN_SLOT>)
- *                   a box of an N-d array (blosc_b200_getslice): the touched blocks and the
- *                   copy out of them, both from the box alone (B2Box, b2_args.h)
+ *                   a box of an N-d array, with a step per dimension or without
+ *                   (blosc_b200_getslice_step): the touched blocks and the copy out of them,
+ *                   both from the box alone (B2Box, b2_args.h)
  *   box_check_kernel, boxes_touch_kernel, boxes_gather_kernel (+ plan_scan_kernel<PLAN_SLOT>)
  *                   a batch of boxes of one extent (blosc_b200_getslices): the corners' check,
  *                   the blocks touched by any box and the copy out, from the origin box and one
@@ -1092,14 +1093,17 @@ extern "C" int b2_ptr_device(const void*) { return 0; }
 
 
 /* blosc_b200_getslice: a box of an N-d array (B2Box), planned and gathered from the box alone, with no per-run state.
- * box_touch_kernel, one thread per block of the chunk: the block is touched when some box item has a byte in it.  The
- * test is on bytes, so it holds when the blocksize is not a multiple of the typesize. */
+ * Both kernels come in two instantiations, STEPPED = the box's `stepped`: the step-1 one compiles the box arithmetic
+ * without its step code.  box_touch_kernel, one thread per block of the chunk: the block is touched when some box item
+ * has a byte in it.  The test is on bytes, so it holds when the blocksize is not a multiple of the typesize, and a step
+ * that jumps over whole blocks leaves them untouched. */
+template <bool STEPPED>
 __global__ void __launch_bounds__(PLAN_THREADS) box_touch_kernel(BoxPlanArgs a) {
   const long long ts = a.plan.typesize, bs = a.plan.blocksize;
   for (long long b = (long long)blockIdx.x * PLAN_THREADS + threadIdx.x; b < a.plan.nblocks;
        b += (long long)gridDim.x * PLAN_THREADS) {
     const long long lo = b * bs, hi = lo + bs < a.plan.nbytes ? lo + bs : a.plan.nbytes;
-    a.plan.cover[b] = b2_box_next(&a.box, a.window + b2_box_div(lo, ts)) < a.window + b2_box_div(hi + ts - 1, ts);
+    a.plan.cover[b] = b2_box_next(&a.box, a.window + b2_box_div(lo, ts), STEPPED) < a.window + b2_box_div(hi + ts - 1, ts);
   }
 }
 
@@ -1107,8 +1111,10 @@ __global__ void __launch_bounds__(PLAN_THREADS) box_touch_kernel(BoxPlanArgs a) 
  * GATHER_SPAN).  Runs of BOX_SHORT_RUN bytes or more are copied by the whole warp, one run piece at a time, each piece
  * cut at block edges.  Shorter runs are copied by one lane each: lane l takes every 32nd run that starts in the job's
  * bytes (the job of byte 0 also takes the run that the chunk's part starts inside), so no run is split between two
- * lanes.  Either way a run's source is the unrank of its first item. */
+ * lanes.  Either way a run's source is the unrank of its first item.  With a step in the innermost dimension every run
+ * is one item. */
 #define BOX_SHORT_RUN 64
+template <bool STEPPED>
 __global__ void __launch_bounds__(GATHER_WARPS * 32) box_gather_kernel(BoxGatherArgs a) {
   if (a.status && ld_cg_i32(a.status) < 0) return;       /* a stream failed to decode: dest stays untouched */
   const long long ts = a.typesize, runb = a.box.run * ts, g0 = a.p0 * ts, end = g0 + a.total;
@@ -1121,7 +1127,7 @@ __global__ void __launch_bounds__(GATHER_WARPS * 32) box_gather_kernel(BoxGather
     if (runb >= BOX_SHORT_RUN) {
       for (long long o = lo; o < hi;) {
         const long long g = g0 + o, k = b2_box_div(g, runb), u = g - k * runb;
-        unsigned s = (unsigned)((b2_box_unrank(&a.box, k * a.box.run) - a.window) * ts + u);
+        unsigned s = (unsigned)((b2_box_unrank(&a.box, k * a.box.run, STEPPED) - a.window) * ts + u);
         long long n = runb - u < hi - o ? runb - u : hi - o;
         while (n > 0) {
           int m = (int)n;
@@ -1139,7 +1145,7 @@ __global__ void __launch_bounds__(GATHER_WARPS * 32) box_gather_kernel(BoxGather
       const long long ka = b2_box_div(lo == 0 ? g0 : g0 + lo + runb - 1, runb), kb = b2_box_div(g0 + hi + runb - 1, runb);
       for (long long k = ka + lane; k < kb; k += 32) {
         const long long gs = k * runb > g0 ? k * runb : g0, ge = (k + 1) * runb < end ? (k + 1) * runb : end;
-        unsigned s = (unsigned)((b2_box_unrank(&a.box, k * a.box.run) - a.window) * ts + (gs - k * runb));
+        unsigned s = (unsigned)((b2_box_unrank(&a.box, k * a.box.run, STEPPED) - a.window) * ts + (gs - k * runb));
         u8* out = a.dst + (gs - g0);
         const int n = (int)(ge - gs);
         if (!a.slot) {
@@ -1168,7 +1174,9 @@ extern "C" int b2_launch_box_plan(const BoxPlanArgs* a, b2_stream_t) {
   if (a->plan.nblocks <= 0) return 0;
   BoxPlanArgs args = *a;
   const long long nb = a->plan.nblocks;
-  simt::launch(simt::Dim3(emu_range_ctas(nb)), simt::Dim3(PLAN_THREADS), 0, [&] { box_touch_kernel(args); });
+  simt::launch(simt::Dim3(emu_range_ctas(nb)), simt::Dim3(PLAN_THREADS), 0, [&] {
+    if (args.box.stepped) box_touch_kernel<true>(args); else box_touch_kernel<false>(args);
+  });
   simt::launch(simt::Dim3(emu_tiles(nb)), simt::Dim3(PLAN_THREADS), 0, [&] { plan_scan_kernel<PLAN_SLOT>(args.plan, nb); });
   g_emu_plan_launches += 2;
   return 0;
@@ -1179,7 +1187,9 @@ extern "C" int b2_launch_box_gather(const BoxGatherArgs* a, b2_stream_t) {
   if (ctas > 3) ctas = 3;
   g_emu_gather_launches++;
   BoxGatherArgs args = *a;
-  simt::launch(simt::Dim3((unsigned)ctas), simt::Dim3(GATHER_WARPS * 32), 0, [&] { box_gather_kernel(args); });
+  simt::launch(simt::Dim3((unsigned)ctas), simt::Dim3(GATHER_WARPS * 32), 0, [&] {
+    if (args.box.stepped) box_gather_kernel<true>(args); else box_gather_kernel<false>(args);
+  });
   return 0;
 }
 #endif
@@ -1188,7 +1198,7 @@ extern "C" int b2_launch_box_gather(const BoxGatherArgs* a, b2_stream_t) {
 /* blosc_b200_getslices: K boxes of one extent, box i the origin box moved by off[i] flat items.  The first flat index
  * >= x (0 <= x <= nitems) of box i, or nitems when there is none: the origin box's answer for x - off[i], moved back. */
 DEV long long box_next_at(const B2Box& b, long long off, long long x) {
-  const long long n = b2_box_next(&b, x > off ? x - off : 0);
+  const long long n = b2_box_next(&b, x > off ? x - off : 0, 0);
   return n < b.nitems ? n + off : b.nitems;
 }
 
@@ -1225,8 +1235,8 @@ __global__ void __launch_bounds__(PLAN_THREADS) boxes_touch_kernel(BoxesPlanArgs
     const long long i = b2_box_div(t, a.per_box), j = t - i * a.per_box, f0 = a.off[i];
     if (a.part && j == 0) {                      /* box i's items of flat index in [window, wend), as output bytes */
       const long long y0 = a.window > f0 ? a.window - f0 : 0, y1 = wend > f0 ? wend - f0 : 0;
-      a.part[2 * i] = b2_box_rank(&a.box, y0 < a.box.nitems ? y0 : a.box.nitems) * ts;
-      a.part[2 * i + 1] = b2_box_rank(&a.box, y1 < a.box.nitems ? y1 : a.box.nitems) * ts;
+      a.part[2 * i] = b2_box_rank(&a.box, y0 < a.box.nitems ? y0 : a.box.nitems, 0) * ts;
+      a.part[2 * i + 1] = b2_box_rank(&a.box, y1 < a.box.nitems ? y1 : a.box.nitems, 0) * ts;
     }
     const long long x0 = f0 > a.window ? f0 : a.window, x1 = f0 + a.span < wend ? f0 + a.span : wend;
     if (a.in_place || x0 >= x1) continue;
@@ -1266,7 +1276,7 @@ __global__ void __launch_bounds__(GATHER_WARPS * 32) boxes_gather_kernel(BoxesGa
         const long long gb = o - i * boxb;                 /* the byte's offset in its box */
         if (gb < plo) { o += plo - gb; continue; }
         if (gb >= phi) { o += boxb - gb; continue; }
-        unsigned s = (unsigned)((b2_box_unrank(&a.box, (k - i * rpb) * a.box.run) + f0 - a.window) * ts + u);
+        unsigned s = (unsigned)((b2_box_unrank(&a.box, (k - i * rpb) * a.box.run, 0) + f0 - a.window) * ts + u);
         long long n = runb - u < hi - o ? runb - u : hi - o;
         if (n > phi - gb) n = phi - gb;
         while (n > 0) {
@@ -1290,7 +1300,7 @@ __global__ void __launch_bounds__(GATHER_WARPS * 32) boxes_gather_kernel(BoxesGa
         if (gs < i * boxb + plo) gs = i * boxb + plo;
         if (ge > i * boxb + phi) ge = i * boxb + phi;
         if (gs >= ge) continue;
-        unsigned s = (unsigned)((b2_box_unrank(&a.box, (k - i * rpb) * a.box.run) + f0 - a.window) * ts + (gs - k * runb));
+        unsigned s = (unsigned)((b2_box_unrank(&a.box, (k - i * rpb) * a.box.run, 0) + f0 - a.window) * ts + (gs - k * runb));
         u8* out = a.dst + gs;
         const int n = (int)(ge - gs);
         if (!a.slot) {

@@ -176,6 +176,17 @@ long long blosc_b200_getitems(const void* src, int nranges, const int* starts, c
 long long blosc_b200_getslice(const void* src, int ndim, const int64_t* shape, const int64_t* start,
                               const int64_t* stop, void* dest);
 
+/* blosc_b200_getslice with a positive step per dimension: the items start[k], start[k] + step[k], ... below stop[k] of
+ * each dimension k, written to dest as one contiguous C-order array (numpy: a[start[0]:stop[0]:step[0], ...,
+ * start[ndim-1]:stop[ndim-1]:step[ndim-1]], made contiguous).  Dimension k selects n_k = ceil((stop[k] - start[k]) /
+ * step[k]) items.  step is host memory, ndim entries; step == NULL means all ones, which is blosc_b200_getslice.
+ * Returns the bytes written, prod(n_k) * typesize; 0 for an empty box, with nothing launched.  Every check of
+ * blosc_b200_getslice applies, and a step[k] < 1 also returns -1 with a message on stderr before anything is launched
+ * or written (negative steps are not supported).  Only the blocks that hold a byte of a selected item are decoded, so
+ * a step that jumps over whole blocks skips them, and the launches do not grow with the number of selected items. */
+long long blosc_b200_getslice_step(const void* src, int ndim, const int64_t* shape, const int64_t* start,
+                                   const int64_t* stop, const int64_t* step, void* dest);
+
 /* A batch of equal-sized boxes in one call: nboxes boxes of extents extent[0..ndim) (host memory), box i at the corner
  * starts[i][0..ndim) (starts: nboxes x ndim int64, row-major), covering items [starts[i][k], starts[i][k] + extent[k])
  * of each dimension k of the chunk's C-order array of `shape`.  Box i is written to dest + i * B, B = prod(extent) *
@@ -225,6 +236,10 @@ long long blosc_b200_frame_getitems(const void* frame, size_t framesize, size_t 
  * nbytes. */
 long long blosc_b200_frame_getslice(const void* frame, size_t framesize, int ndim, const int64_t* shape,
                                     const int64_t* start, const int64_t* stop, void* dest);
+/* blosc_b200_getslice_step over a frame, with the failures and ordering of blosc_b200_frame_getslice: chunks that
+ * hold no selected item are neither read nor decoded. */
+long long blosc_b200_frame_getslice_step(const void* frame, size_t framesize, int ndim, const int64_t* shape,
+                                         const int64_t* start, const int64_t* stop, const int64_t* step, void* dest);
 /* blosc_b200_getslices over a frame: the whole frame holds the C-order array, as in blosc_b200_frame_getslice, and a
  * box may cross chunk boundaries.  The corners are checked once; the chunks that hold an item of some box are then
  * read in ascending order, each decoding its touched blocks once for all boxes.  The first failure decides the result,

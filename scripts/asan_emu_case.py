@@ -150,7 +150,8 @@ P=lambda a: a.ctypes.data_as(vp)
 for f,res,args in (("blosc_b200_getitems",ll,[vp,C.c_int,vp,vp,vp]),("blosc_b200_getslice",ll,[vp,C.c_int,vp,vp,vp,vp]),
                    ("blosc_b200_frame_bound",sz,[sz,sz,sz]),("blosc_b200_frame_compress",ll,[C.c_int,C.c_int,sz,sz,vp,vp,sz,C.c_char_p,sz,sz,C.c_int]),
                    ("blosc_b200_frame_getitems",ll,[vp,sz,sz,vp,vp,vp]),("blosc_b200_frame_getslice",ll,[vp,sz,C.c_int,vp,vp,vp,vp]),
-                   ("blosc_b200_getslices",ll,[vp,C.c_int,vp,vp,ll,vp,vp]),("blosc_b200_frame_getslices",ll,[vp,sz,C.c_int,vp,vp,ll,vp,vp])):
+                   ("blosc_b200_getslices",ll,[vp,C.c_int,vp,vp,ll,vp,vp]),("blosc_b200_frame_getslices",ll,[vp,sz,C.c_int,vp,vp,ll,vp,vp]),
+                   ("blosc_b200_getslice_step",ll,[vp,C.c_int,vp,vp,vp,vp,vp]),("blosc_b200_frame_getslice_step",ll,[vp,sz,C.c_int,vp,vp,vp,vp,vp])):
     getattr(emu,f).restype=res; getattr(emu,f).argtypes=args
 emu.emu_set_all_device.argtypes=[C.c_int]
 irng=np.random.default_rng(11)
@@ -158,6 +159,7 @@ ts,shape=4,(300,250)
 n=ts*shape[0]*shape[1]
 src=gen("bench",n); arr=src.view(np.uint32).reshape(shape)
 box=([17,30],[123,200]); want_box=arr[17:123,30:200].tobytes()
+bstep=np.array([7,3],np.int64); want_step=arr[17:123:7,30:200:3].tobytes()
 ranges=[(int(s),int(k)) for s,k in zip(irng.integers(0,n//ts-600,40),irng.integers(0,600,40))]+[(5,0),(100,3),(101,900)]
 st=np.array([r[0] for r in ranges],np.int32); nt=np.array([r[1] for r in ranges],np.int32)
 want_items=b"".join(src[s*ts:(s+k)*ts].tobytes() for s,k in ranges)
@@ -187,11 +189,14 @@ for comp,shuf,cl in (("lz4",1,5),("blosclz",2,5),("lz4",1,0)):
                 out=np.zeros(len(want_box),np.uint8)
                 g=emu.blosc_b200_getslice(P(c),2,P(sh),P(b0),P(b1),P(out))
                 assert c is not chunk or (g==len(want_box) and out.tobytes()==want_box)
+                out=np.zeros(len(want_step),np.uint8)
+                g=emu.blosc_b200_getslice_step(P(c),2,P(sh),P(b0),P(b1),P(bstep),P(out))
+                assert c is not chunk or (g==len(want_step) and out.tobytes()==want_step)
                 out=np.zeros(len(want_boxes),np.uint8)
                 g=emu.blosc_b200_getslices(P(c),2,P(sh),P(ext),len(corners),P(corners),P(out))
                 assert c is not chunk or (g==len(want_boxes) and out.tobytes()==want_boxes)
                 assert emu.blosc_b200_getslices(P(c),2,P(sh),P(ext),len(bad),P(bad),P(out))<0
-                cases+=4
+                cases+=5
             for f in [frame]+[frame.copy() for _ in range(2)]:
                 if f is not frame: pos=irng.integers(100,fb,6); f[pos]=irng.integers(0,256,6,dtype=np.uint8)
                 out=np.zeros(len(want_items),np.uint8)
@@ -200,11 +205,14 @@ for comp,shuf,cl in (("lz4",1,5),("blosclz",2,5),("lz4",1,0)):
                 out=np.zeros(len(want_box),np.uint8)
                 g=emu.blosc_b200_frame_getslice(P(f),fb,2,P(sh),P(b0),P(b1),P(out))
                 assert f is not frame or (g==len(want_box) and out.tobytes()==want_box)
+                out=np.zeros(len(want_step),np.uint8)
+                g=emu.blosc_b200_frame_getslice_step(P(f),fb,2,P(sh),P(b0),P(b1),P(bstep),P(out))
+                assert f is not frame or (g==len(want_step) and out.tobytes()==want_step)
                 out=np.zeros(len(want_boxes),np.uint8)
                 g=emu.blosc_b200_frame_getslices(P(f),fb,2,P(sh),P(ext),len(corners),P(corners),P(out))
                 assert f is not frame or (g==len(want_boxes) and out.tobytes()==want_boxes)
                 assert emu.blosc_b200_frame_getslices(P(f),fb,2,P(sh),P(ext),len(bad),P(bad),P(out))<0
-                cases+=4
+                cases+=5
         finally:
             emu.emu_set_all_device(0)
 print("asan workload ok, cases", cases)
