@@ -79,6 +79,10 @@ def _load(path: str) -> C.CDLL:
     lib.blosc_b200_getslices.argtypes = [vp, ci, vp, vp, ll, vp, vp]
     lib.blosc_b200_frame_getslices.restype = ll
     lib.blosc_b200_frame_getslices.argtypes = [vp, sz, ci, vp, vp, ll, vp, vp]
+    lib.blosc_b200_getoindex.restype = ll
+    lib.blosc_b200_getoindex.argtypes = [vp, ci, vp, vp, vp, vp, vp, vp, vp]
+    lib.blosc_b200_frame_getoindex.restype = ll
+    lib.blosc_b200_frame_getoindex.argtypes = [vp, sz, ci, vp, vp, vp, vp, vp, vp, vp]
     lib.blosc_b200_frame_info.restype = ci
     lib.blosc_b200_frame_info.argtypes = [vp, sz, C.POINTER(sz), C.POINTER(sz), C.POINTER(sz), C.POINTER(sz)]
     lib.blosc_b200_frame_chunk.restype = ll
@@ -264,6 +268,90 @@ def frame_getslices(frame, framesize, shape, extent, starts, dest):
     sh, ex, st = _boxes(shape, extent, starts)
     return int(lib.blosc_b200_frame_getslices(_ptr(frame), framesize, sh.size, sh.ctypes.data, ex.ctypes.data, st[2],
                                               st[1], _ptr(dest)))
+
+
+def _selection(shape, selection):
+    """An orthogonal selection as the C call takes it: shape, start, stop and step as int64 host arrays (the slices,
+    list dimensions whole), the lists to keep alive, the index pointer array (None when no dimension is a list) and
+    the list lengths."""
+    import numpy as np
+    sh = np.ascontiguousarray(shape, dtype=np.int64).reshape(-1)
+    if len(selection) != sh.size:
+        raise ValueError(f"shape and selection have {sh.size} and {len(selection)} entries")
+    n = sh.size
+    st, sp, t, nidx = (np.zeros(n, np.int64) for _ in range(4))
+    ptrs, keep = (C.c_void_p * max(n, 1))(), []
+    for k, s in enumerate(selection):
+        st[k], sp[k], t[k] = 0, sh[k], 1
+        if isinstance(s, slice):
+            a, b, c = (0 if s.start is None else s.start), (sh[k] if s.stop is None else s.stop), \
+                (1 if s.step is None else s.step)
+            if a < 0 or b < 0 or c < 1:
+                raise ValueError(f"dimension {k}: negative slice fields and steps below 1 are not supported ({s})")
+            st[k] = min(a, sh[k])
+            sp[k] = min(max(b, st[k]), sh[k])
+            t[k] = c
+            continue
+        if isinstance(s, (int, np.integer)) and not isinstance(s, (bool, np.bool_)):
+            if s < 0:
+                raise ValueError(f"dimension {k}: negative index {s} is not supported")
+            st[k], sp[k] = s, s + 1
+            continue
+        if _is_cuda(s):
+            if s.dim() != 1:
+                raise ValueError(f"dimension {k}: an index list must be 1-d")
+            if str(s.dtype) == "torch.bool":
+                if s.numel() != sh[k]:
+                    raise ValueError(f"dimension {k}: a mask of {s.numel()} entries for an extent of {sh[k]}")
+                s = s.nonzero().reshape(-1)                 # syncs with the device
+            elif str(s.dtype) != "torch.int64":
+                raise TypeError(f"CUDA index lists must be torch.int64 or torch.bool, not {s.dtype}")
+            s = s.contiguous()
+            keep.append(s)
+            ptrs[k], nidx[k] = s.data_ptr(), s.numel()
+        else:
+            h = np.asarray(s.numpy() if hasattr(s, "numpy") else s)
+            if h.ndim != 1:
+                raise ValueError(f"dimension {k}: an index list must be 1-d")
+            if h.dtype == np.bool_:
+                if h.size != sh[k]:
+                    raise ValueError(f"dimension {k}: a mask of {h.size} entries for an extent of {sh[k]}")
+                h = np.flatnonzero(h)
+            elif h.size and h.dtype.kind not in "iu":
+                raise TypeError(f"dimension {k}: index lists must be integers, not {h.dtype}")
+            h = np.ascontiguousarray(h, dtype=np.int64)
+            keep.append(h)
+            ptrs[k], nidx[k] = h.ctypes.data, h.size
+        if not nidx[k]:                                     # an empty list, which is never read: any non-NULL address
+            ptrs[k] = sh.ctypes.data
+    return sh, st, sp, t, keep, (ptrs if keep else None), nidx
+
+
+def getoindex(src, shape, selection, dest):
+    """An orthogonal index selection of the C-order array of `shape` that the chunk holds (blosc_b200_getoindex):
+    numpy's a[np.ix_(...)] with slices kept as slices, made contiguous in C order (zarr's oindex).  `selection` has one
+    entry per dimension: a slice (positive fields; None takes numpy's default), an int (one coordinate, as numpy's
+    a[..., i, ...], which drops the dimension: the bytes are the same), a 1-d integer sequence or numpy array (uploaded
+    once), an int64 CUDA tensor on the device of the call (read in place; other CUDA dtypes raise TypeError), or a 1-d
+    bool mask of the dimension's length, turned into its indices with nonzero (on a CUDA mask that syncs with the
+    device).  Entries may be unsorted and repeat.  A selection with no list is getslice with its steps.  Returns the
+    bytes written, or a negative code (dest is then untouched)."""
+    sh, st, sp, t, keep, ptrs, nidx = _selection(shape, selection)
+    if ptrs is None:
+        return getslice(src, sh, st, sp, dest, step=t)
+    return int(lib.blosc_b200_getoindex(_ptr(src), sh.size, sh.ctypes.data, st.ctypes.data, sp.ctypes.data,
+                                        t.ctypes.data, C.cast(ptrs, C.c_void_p), nidx.ctypes.data, _ptr(dest)))
+
+
+def frame_getoindex(frame, framesize, shape, selection, dest):
+    """getoindex over the array a frame holds (blosc_b200_frame_getoindex); the selection may cross chunk
+    boundaries, and chunks that hold no selected item are not read."""
+    sh, st, sp, t, keep, ptrs, nidx = _selection(shape, selection)
+    if ptrs is None:
+        return frame_getslice(frame, framesize, sh, st, sp, dest, step=t)
+    return int(lib.blosc_b200_frame_getoindex(_ptr(frame), framesize, sh.size, sh.ctypes.data, st.ctypes.data,
+                                              sp.ctypes.data, t.ctypes.data, C.cast(ptrs, C.c_void_p),
+                                              nidx.ctypes.data, _ptr(dest)))
 
 
 def frame_info(frame, framesize):

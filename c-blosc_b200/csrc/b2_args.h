@@ -482,6 +482,84 @@ typedef struct BoxesGatherArgs {
   const int* status;
 } BoxesGatherArgs;
 
+/* An orthogonal index selection of an N-d C-order array (blosc_b200_getoindex): numpy's a[np.ix_(...)], where each
+ * dimension is either a slice (start, step, ext coordinates) or a list of coordinates in device memory, in any order
+ * and with repeats.  The host builds it (blosc_b200.c osel_build) with B2Box's merging of the slice dimensions: a whole
+ * step-1 slice merges into the dimension before it when that one is a step-1 slice too; a list never merges.  The run
+ * is the innermost extent when the innermost dimension is a step-1 slice, else one item.  Position q of dimension k is
+ * the coordinate list[k][q], or start[k] + q * step[k]. */
+typedef struct B2OSel {
+  int ndim;                           /* dimensions after merging, 1..B2_BOX_MAXDIM */
+  int kdim[B2_BOX_MAXDIM];            /* the caller's dimension of each list, for the bad-entry key */
+  long long start[B2_BOX_MAXDIM];
+  long long step[B2_BOX_MAXDIM];
+  long long ext[B2_BOX_MAXDIM];       /* positions of dimension k: n_k */
+  long long shape[B2_BOX_MAXDIM];     /* the dimension's extent in the array: a list entry must lie in [0, shape) */
+  long long stride[B2_BOX_MAXDIM];    /* flat items per coordinate of dimension k */
+  const long long* list[B2_BOX_MAXDIM];   /* NULL for a slice */
+  long long lbase[B2_BOX_MAXDIM];     /* entries of the lists before list k, in the check's numbering */
+  long long run;                      /* items of one run */
+  long long slab;                     /* items of the selection per position of dimension 0 */
+  long long count;                    /* items of the selection */
+  long long nruns;                    /* count / run */
+  long long nentries;                 /* entries of all lists */
+} B2OSel;
+
+/* The flat index of selection item p (0 <= p < count), or -1 when a list entry it reads lies outside its dimension
+ * (the check reports those; the plan must not index with them).  Only the kernels call it: the lists are device
+ * memory. */
+static inline B2_HD long long b2_osel_unrank(const B2OSel* s, long long p) {
+  long long f = 0;
+  int k, bad = 0;
+#pragma unroll
+  for (k = B2_BOX_MAXDIM - 1; k >= 0; k--) {
+    if (k < s->ndim) {
+      long long q = p, c;
+      if (k > 0) {
+        p = b2_box_div(p, s->ext[k]);
+        q -= p * s->ext[k];
+      }
+      c = s->list[k] ? s->list[k][q] : s->start[k] + q * s->step[k];
+      bad |= c < 0 || c >= s->shape[k];
+      f += c * s->stride[k];
+    }
+  }
+  return bad ? -1 : f;
+}
+
+/* oindex_touch_kernel over work items [0, (check ? nentries : 0) + r1 - r0).  The first nentries check the list
+ * entries: an entry outside its dimension puts the key (caller's dimension << 56 | position) to *bad by atomicMin, so
+ * the first bad entry wins.  The rest take one run each, the runs [r0, r1) (a frame's chunk: those of the output
+ * bytes its gather walks).  touched != NULL (a frame): the run flags every
+ * chunk, of ipc items, that holds one of its items.  Else the run marks in plan.cover every block of the chunk, which
+ * holds the array's flat items [window, window + nbytes / typesize), that holds a byte of it (it only stores 1s; cover
+ * starts zeroed), and the PLAN_SLOT scan lists them. */
+typedef struct OIndexPlanArgs {
+  B2OSel sel;
+  long long window;
+  int check, pad;
+  long long r0, r1;
+  unsigned long long* bad;
+  int* touched;
+  long long ipc;
+  PlanArgs plan;
+} OIndexPlanArgs;
+
+/* oindex_gather_kernel: the output bytes [g0, g1) of the selection (each a multiple of the run's bytes), at dst + byte.
+ * clip (a frame): only the items inside the chunk's window [window, wend) are written; a position of dimension 0
+ * whose coordinate's flat span misses the window is skipped whole.  slot / src / status as in BoxGatherArgs. */
+typedef struct OIndexGatherArgs {
+  B2OSel sel;
+  long long window, wend;
+  long long g0, g1;
+  int typesize, blocksize;
+  int clip, pad;
+  const int* slot;
+  const uint8_t* src;
+  uint8_t* dst;
+  const int* status;
+} OIndexGatherArgs;
+
 #ifdef __cplusplus
 }
 #endif

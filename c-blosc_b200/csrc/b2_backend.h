@@ -66,6 +66,10 @@ int  b2_launch_box_check(const BoxCheckArgs* a, b2_stream_t s);        /* box_ch
 int  b2_launch_boxes_plan(const BoxesPlanArgs* a, b2_stream_t s);      /* boxes_touch_kernel + plan_scan_kernel<PLAN_SLOT>:
                                                                         * the blocks a chunk's part of a batch touches */
 int  b2_launch_boxes_gather(const BoxesGatherArgs* a, b2_stream_t s);  /* boxes_gather_kernel (getslices) */
+int  b2_launch_oindex_plan(const OIndexPlanArgs* a, b2_stream_t s);    /* oindex_touch_kernel (+ plan_scan_kernel<PLAN_SLOT>
+                                                                        * when it marks blocks): getoindex's list check and
+                                                                        * touched blocks, or a frame's touched chunks */
+int  b2_launch_oindex_gather(const OIndexGatherArgs* a, b2_stream_t s);   /* oindex_gather_kernel (getoindex) */
 
 /* profiling: per-kernel-kind CUDA-event timing (off by default) */
 enum { B2_K_FILTER = 0, B2_K_ENCODE, B2_K_SCAN, B2_K_COMPACT, B2_K_DECODE, B2_K_UNFILTER, B2_K_INDEX, B2_K_PARSE, B2_K_ZENC, B2_K_DENC, B2_K_SENC, B2_K_GATHER, B2_K_PLAN, B2_K_COUNT };

@@ -499,3 +499,31 @@ extern "C" int b2_launch_boxes_gather(const BoxesGatherArgs* a, b2_stream_t s) {
   CK(cudaGetLastError());
   return 0;
 }
+
+/* the index selection of getoindex: oindex_touch_kernel over the list entries and the runs (on a frame, once, to flag
+ * the touched chunks), then, when it marked blocks, the PLAN_SLOT scan, all counted as plan launches; the gather as a
+ * gather launch */
+extern "C" int b2_launch_oindex_plan(const OIndexPlanArgs* a, b2_stream_t s) {
+  const long long n = (a->check ? a->sel.nentries : 0) + a->r1 - a->r0, nb = a->plan.nblocks;
+  if (n > 0) {
+    ProfScope ps(B2_K_PLAN, s->s);
+    oindex_touch_kernel<<<range_ctas(n), PLAN_THREADS, 0, s->s>>>(*a);
+    CK(cudaGetLastError());
+  }
+  if (a->touched || a->r1 <= a->r0 || nb <= 0) return 0;
+  ProfScope ps(B2_K_PLAN, s->s);
+  plan_scan_kernel<PLAN_SLOT><<<(unsigned)((nb + PLAN_TILE - 1) / PLAN_TILE), PLAN_THREADS, 0, s->s>>>(a->plan, nb);
+  CK(cudaGetLastError());
+  return 0;
+}
+
+extern "C" int b2_launch_oindex_gather(const OIndexGatherArgs* a, b2_stream_t s) {
+  const long long total = a->g1 - a->g0;
+  if (total <= 0) return 0;
+  long long ctas = (total + (long long)GATHER_WARPS * GATHER_SPAN - 1) / ((long long)GATHER_WARPS * GATHER_SPAN);
+  if (ctas > (long long)num_sms() * 8) ctas = (long long)num_sms() * 8;
+  ProfScope ps(B2_K_GATHER, s->s);
+  oindex_gather_kernel<<<(unsigned)ctas, GATHER_WARPS * 32, 0, s->s>>>(*a);
+  CK(cudaGetLastError());
+  return 0;
+}

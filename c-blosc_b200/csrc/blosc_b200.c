@@ -1711,6 +1711,181 @@ long long blosc_b200_getslices(const void* src, int ndim, const int64_t* shape, 
 }
 
 /* ------------------------------------------------------------------------- */
+/* orthogonal index selections (blosc_b200_getoindex, _frame_getoindex)       */
+/* ------------------------------------------------------------------------- */
+/* numpy's a[np.ix_(...)]: some dimensions select a list of coordinates, the others a slice.  The selection (B2OSel,
+ * b2_args.h) holds the lists as device pointers, so neither the plan nor the gather keeps per-run state:
+ * oindex_touch_kernel checks the entries and marks the touched blocks in one launch, the PLAN_SLOT scan lists them,
+ * they are decoded as for a box, and oindex_gather_kernel writes the output.  A frame runs the check once over all its
+ * chunks, which also flags the touched ones. */
+
+/* whether some dimension is a list (ndim already checked) */
+static int osel_any(int ndim, const int64_t* const* index) {
+  int k;
+  for (k = 0; index && k < ndim; k++) if (index[k]) return 1;
+  return 0;
+}
+
+/* The checks of an index selection that need no data, with getslice_step's messages on the slice dimensions: its
+ * slices with the list dimensions made whole (st, sp, t), the array's items, the output's items, and device lists on
+ * the device the call runs on (that of data or dest when either is device memory).  -1 with a message when one fails. */
+static int osel_geometry(int ndim, const int64_t* shape, const int64_t* start, const int64_t* stop, const int64_t* step,
+                         const int64_t* const* index, const int64_t* nindex, const void* data, const void* dest,
+                         int64_t* st, int64_t* sp, int64_t* t, long long* nitems, long long* count) {
+  long long prod = 1;
+  int k, dev, zero = 0;
+  for (k = 0; k < ndim; k++) {
+    st[k] = index[k] ? 0 : start[k]; sp[k] = index[k] ? shape[k] : stop[k]; t[k] = index[k] || !step ? 1 : step[k];
+  }
+  if (box_geometry(ndim, shape, st, sp, nitems) || box_steps(ndim, t)) return -1;
+  for (k = 0; k < ndim; k++) {
+    const long long n = index[k] ? nindex[k] : st[k] == sp[k] ? 0 : (sp[k] - st[k] - 1) / t[k] + 1;
+    if (n < 0) { fprintf(stderr, "blosc_b200: nindex[%d] = %lld is negative\n", k, n); return -1; }
+    zero |= n == 0;
+    if (!zero && ((index[k] && n > (1LL << 56)) || prod > LLONG_MAX / n)) {   /* the check's key holds 56 bits */
+      fprintf(stderr, "blosc_b200: the selection's item count overflows int64\n");
+      return -1;
+    }
+    if (!zero) prod *= n;
+  }
+  *count = zero ? 0 : prod;
+  dev = b2_ptr_is_device(data) ? b2_ptr_device(data) : b2_ptr_is_device(dest) ? b2_ptr_device(dest) : b2_get_device();
+  for (k = 0; k < ndim; k++)
+    if (index[k] && b2_ptr_is_device(index[k]) && b2_ptr_device(index[k]) != dev) {
+      fprintf(stderr, "blosc_b200: index[%d] is not on device %d, where the call runs\n", k, dev);
+      return -1;
+    }
+  return 0;
+}
+
+/* the output's bytes: -1 with a message when they overflow int64 */
+static int osel_nbytes(long long count, long long typesize) {
+  if (count > LLONG_MAX / typesize) {
+    fprintf(stderr, "blosc_b200: the selection's %lld items of %lld bytes overflow int64\n", count, typesize);
+    return -1;
+  }
+  return 0;
+}
+
+/* The selection of a checked, non-empty one: the lists as the kernels read them, in device memory (host lists are
+ * uploaded into w->segs, one copy each), and the slice dimensions merged as box_build merges them, a list never.
+ * Returns 0, or -1 when an upload fails. */
+static int osel_build(b2_ws* w, int ndim, const int64_t* shape, const int64_t* st, const int64_t* sp, const int64_t* t,
+                      const int64_t* const* index, const int64_t* nindex, B2OSel* s) {
+  long long sh[B2_BOX_MAXDIM], up = 0, at = 0;
+  int k, n = 0;
+  memset(s, 0, sizeof *s);
+  for (k = 0; k < ndim; k++) if (index[k] && !b2_ptr_is_device(index[k])) up += nindex[k];
+  if (up && buf_ensure(&w->segs, 8 * (size_t)up + 64)) return -1;
+  for (k = 0; k < ndim; k++) {
+    if (index[k]) {
+      const long long* l = (const long long*)index[k];
+      if (!b2_ptr_is_device(l)) {
+        l = (const long long*)w->segs.p + at;
+        if (h2d_any(w, (void*)l, index[k], 8 * (size_t)nindex[k])) return -1;
+        at += nindex[k];
+      }
+      sh[n] = shape[k]; s->list[n] = l; s->ext[n] = nindex[k]; s->step[n] = 1; s->kdim[n] = k;
+      s->lbase[n] = s->nentries; s->nentries += nindex[k];
+      n++;
+    } else {
+      const long long e = (sp[k] - st[k] - 1) / t[k] + 1, u = e == 1 ? 1 : t[k];
+      if (n > 0 && !s->list[n - 1] && s->step[n - 1] == 1 && u == 1 && st[k] == 0 && e == shape[k]) {
+        sh[n - 1] *= shape[k]; s->start[n - 1] *= shape[k]; s->ext[n - 1] *= shape[k];
+      } else {
+        sh[n] = shape[k]; s->start[n] = st[k]; s->step[n] = u; s->ext[n] = e;
+        n++;
+      }
+    }
+  }
+  s->ndim = n;
+  s->stride[n - 1] = 1;
+  for (k = n - 2; k >= 0; k--) s->stride[k] = s->stride[k + 1] * sh[k + 1];
+  s->count = 1;
+  for (k = 0; k < n; k++) { s->shape[k] = sh[k]; s->count *= s->ext[k]; }
+  s->run = !s->list[n - 1] && s->step[n - 1] == 1 ? s->ext[n - 1] : 1;
+  s->slab = s->count / s->ext[0];
+  s->nruns = s->count / s->run;
+  return 0;
+}
+
+/* A bad list entry, from the check's key (the caller's dimension << 56 | position): the entry is read back from the
+ * device list and named.  Returns -1. */
+static int osel_bad_entry(b2_ws* w, const B2OSel* s, unsigned long long key) {
+  const int kd = (int)(key >> 56);
+  const long long q = (long long)(key & ((1ull << 56) - 1));
+  long long c = 0;
+  int k;
+  for (k = 0; k < s->ndim; k++)
+    if (s->list[k] && s->kdim[k] == kd && !copy_any(&c, 0, s->list[k] + q, 1, 8, w->stream))
+      fprintf(stderr, "blosc_b200: index[%d][%lld] = %lld is not in [0, %lld)\n", kd, q, c, s->shape[k]);
+  return -1;
+}
+
+/* One chunk's part of a selection: the chunk (header h, checked) holds the array's flat items [window, window + nbytes
+ * / typesize), and the output bytes [g0, g1) are written at d_dst + byte (device memory).  A chunk call (frame 0)
+ * checks the list entries with the touch, and a memcpyed device chunk is then read in place after the check alone; a
+ * frame's chunk (frame 1, checked already) writes only the items inside it.  Returns 0, blosc_d's code when a touched
+ * block fails to decode (nothing is written then), or -1. */
+static int oindex_chunk(b2_ws* w, const void* src, int src_dev, const b2_hdr* h, int codec, const B2OSel* sel, int frame,
+                        long long window, long long g0, long long g1, uint8_t* d_dst) {
+  const int in_place = (h->flags & BLOSC_MEMCPYED) && src_dev;
+  GetitemsPlan rec = {0};
+  OIndexGatherArgs ga;
+  int rc;
+  memset(&ga, 0, sizeof ga);
+  ga.sel = *sel; ga.window = window; ga.wend = window + h->nbytes / h->typesize; ga.g0 = g0; ga.g1 = g1;
+  ga.typesize = h->typesize; ga.blocksize = h->blocksize; ga.clip = frame; ga.dst = d_dst;
+  if (!in_place || !frame) {
+    OIndexPlanArgs pa;
+    memset(&pa, 0, sizeof pa);
+    pa.sel = *sel; pa.window = window; pa.check = !frame;
+    if (!in_place) { pa.r0 = g0 / (sel->run * h->typesize); pa.r1 = g1 / (sel->run * h->typesize); }
+    if (!plan_scratch(w, h, 0, 0, &pa.plan)) return -1;
+    pa.bad = &pa.plan.rec->bad_box;
+    if (b2_memset_dev(pa.bad, 0xff, 8, w->stream) || b2_launch_oindex_plan(&pa, w->stream) ||
+        read_plan(w, pa.plan.rec, &rec, sizeof rec))
+      return -1;
+    if (rec.bad_box != ~0ull) return osel_bad_entry(w, sel, rec.bad_box);
+    if (!in_place) ga.slot = pa.plan.slot;
+  }
+  if (touched_source(w, src, src_dev, h, codec, rec.nlisted, rec.has_left, &ga.src, &ga.status)) return -1;
+  if (b2_launch_oindex_gather(&ga, w->stream)) { ws_reset_counters(w); return -1; }
+  rc = read_verdict(w, ga.status);
+  return rc < 0 ? rc : 0;
+}
+
+long long blosc_b200_getoindex(const void* src, int ndim, const int64_t* shape, const int64_t* start,
+                               const int64_t* stop, const int64_t* step, const int64_t* const* index,
+                               const int64_t* nindex, void* dest) {
+  int64_t st[B2_BOX_MAXDIM], sp[B2_BOX_MAXDIM], t[B2_BOX_MAXDIM];
+  b2_hdr h;
+  B2OSel sel;
+  b2_ws* w;
+  uint8_t* d_dst;
+  long long nitems = 0, count = 0, result = -1;
+  int src_dev, dest_dev, codec = 0, rc;
+  if (ndim < 1 || ndim > B2_BOX_MAXDIM || !osel_any(ndim, index))      /* no list: getslice_step (which checks ndim) */
+    return blosc_b200_getslice_step(src, ndim, shape, start, stop, step, dest);
+  if (osel_geometry(ndim, shape, start, stop, step, index, nindex, src, dest, st, sp, t, &nitems, &count)) return -1;
+  src_dev = b2_ptr_is_device(src);
+  rc = getitem_header(NULL, src, src_dev, -1, &h, &codec);
+  if (rc) return rc;
+  if (box_nbytes(nitems, h.typesize, (unsigned long long)h.nbytes) || osel_nbytes(count, h.typesize)) return -1;
+  if (count == 0) return 0;
+  dest_dev = b2_ptr_is_device(dest);
+  if (!(w = ws_acquire())) return -1;
+  if ((d_dst = stage_dest(&w->slots, dest, dest_dev, (size_t)(count * h.typesize))) &&
+      !osel_build(w, ndim, shape, st, sp, t, index, nindex, &sel) &&
+      (result = oindex_chunk(w, src, src_dev, &h, codec, &sel, 0, 0, 0, count * h.typesize, d_dst)) == 0) {
+    result = count * h.typesize;
+    if (!dest_dev && d2h_any(w, dest, d_dst, (size_t)result)) result = -1;
+  }
+  ws_release(w);
+  return result;
+}
+
+/* ------------------------------------------------------------------------- */
 /* frames: buffers larger than one chunk (SURVEY.md section 8, row f3)           */
 /* ------------------------------------------------------------------------- */
 /* A Blosc-1 chunk holds at most INT_MAX-16 bytes (blosc.h:40) and a single call leaves most of
@@ -2301,6 +2476,93 @@ long long blosc_b200_frame_getslices(const void* frame, size_t framesize, int nd
         break;
       }
       got = boxes_read(w, (const uint8_t*)frame + f.off[c], f.dev, &h, codec, &ck, 0, w0, part, nbytes, d_dst);
+      if (got < 0) break;
+    }
+    if (c < f.nchunks) { result = got; break; }
+    if (!dest_dev && d2h_any(w, dest, d_dst, (size_t)nbytes)) break;
+    result = nbytes;
+  } while (0);
+  ws_release(w);
+  free(head);
+  free(f.off);
+  return result;
+}
+
+/* The output bytes [*g0, *g1) that a frame chunk of items [w0, w1) can write: those of the positions of dimension 0
+ * whose coordinate's rows meet the chunk.  A slice's coordinates ascend, so they are one interval; a list's are not,
+ * and the gather then walks all of them, skipping the positions that miss the chunk. */
+static void osel_slabs(const B2OSel* s, long long w0, long long w1, long long ts, long long* g0, long long* g1) {
+  long long jlo = 0, jhi = s->ext[0];
+  if (!s->list[0]) {                     /* rows [clo, chi) meet the chunk */
+    const long long clo = w0 / s->stride[0], chi = (w1 + s->stride[0] - 1) / s->stride[0];
+    jlo = clo <= s->start[0] ? 0 : (clo - s->start[0] + s->step[0] - 1) / s->step[0];
+    jhi = chi <= s->start[0] ? 0 : (chi - s->start[0] + s->step[0] - 1) / s->step[0];
+    if (jhi > s->ext[0]) jhi = s->ext[0];
+    if (jlo > jhi) jlo = jhi;
+  }
+  *g0 = jlo * s->slab * ts; *g1 = jhi * s->slab * ts;
+}
+
+/* An index selection of the array a frame holds, in items of chunk 0's typesize: one launch checks the list entries
+ * and flags the chunks that hold a selected item, read back with one sync; then each flagged chunk, in ascending
+ * order, writes the selected items it holds by the chunk path, and the first failure decides the result.  A host dest
+ * is staged in device memory and copied out once. */
+long long blosc_b200_frame_getoindex(const void* frame, size_t framesize, int ndim, const int64_t* shape,
+                                     const int64_t* start, const int64_t* stop, const int64_t* step,
+                                     const int64_t* const* index, const int64_t* nindex, void* dest) {
+  int64_t st[B2_BOX_MAXDIM], sp[B2_BOX_MAXDIM], t[B2_BOX_MAXDIM];
+  size_t c;
+  b2_frame f;
+  long long nitems = 0, count = 0, ts, ipc, nbytes, got = 0, result = -1;
+  int dest_dev, rc;
+  B2OSel sel;
+  b2_ws* w;
+  uint8_t *d_dst, *head = NULL;
+  if (ndim < 1 || ndim > B2_BOX_MAXDIM || !osel_any(ndim, index))
+    return blosc_b200_frame_getslice_step(frame, framesize, ndim, shape, start, stop, step, dest);
+  if (!backend_ready()) return -1;
+  if (osel_geometry(ndim, shape, start, stop, step, index, nindex, frame, dest, st, sp, t, &nitems, &count)) return -1;
+  rc = frame_open_items(frame, framesize, &f);
+  if (rc == -2)
+    fprintf(stderr, "blosc_b200: chunk 0's typesize %lld does not divide the frame's chunksize\n", (long long)f.typesize);
+  if (rc) return -1;
+  ts = (long long)f.typesize; ipc = (long long)f.ipc;
+  dest_dev = b2_ptr_is_device(dest);
+  if (box_nbytes(nitems, ts, (unsigned long long)f.nbytes) || osel_nbytes(count, ts)) { free(f.off); return -1; }
+  if (count == 0) { free(f.off); return 0; }
+  nbytes = count * ts;
+  if (!(w = ws_acquire())) { free(f.off); return -1; }
+  do {
+    OIndexPlanArgs fa;
+    if (!(d_dst = stage_dest(&w->fstage, dest, dest_dev, (size_t)nbytes))) break;
+    if (osel_build(w, ndim, shape, st, sp, t, index, nindex, &sel)) break;
+    /* the scratch in w->fplan, which the chunk plans leave alone: the first bad entry (all ones), then the chunks' flags
+     * (zeroed) */
+    if (buf_ensure(&w->fplan, 16 + 4 * f.nchunks) || b2_memset_dev(w->fplan.p, 0, 16 + 4 * f.nchunks, w->stream) ||
+        b2_memset_dev(w->fplan.p, 0xff, 8, w->stream))
+      break;
+    memset(&fa, 0, sizeof fa);
+    fa.sel = sel; fa.check = 1; fa.r1 = sel.nruns; fa.ipc = ipc;
+    fa.bad = (unsigned long long*)w->fplan.p; fa.touched = (int*)((uint8_t*)w->fplan.p + 16);
+    if (b2_launch_oindex_plan(&fa, w->stream)) break;
+    if (!(head = (uint8_t*)malloc(16 + 4 * f.nchunks)) || d2h_any(w, head, w->fplan.p, 16 + 4 * f.nchunks)) break;
+    if (*(unsigned long long*)head != ~0ull) { osel_bad_entry(w, &sel, *(unsigned long long*)head); break; }
+    for (c = 0; c < f.nchunks; c++) {
+      const long long w0 = (long long)c * ipc, w1 = w0 + ipc < nitems ? w0 + ipc : nitems;
+      long long g0, g1;
+      b2_hdr h;
+      int codec = 0;
+      if (!((int*)(head + 16))[c]) continue;                               /* no selected item in this chunk */
+      got = frame_chunk_header(w, frame, &f, c, &h, &codec);
+      if (got < 0) break;
+      if (got || h.nbytes != (w1 - w0) * ts) {
+        fprintf(stderr, "blosc_b200: chunk %zu holds %d items of %d bytes, not the frame's %lld of %lld\n", c,
+                h.nbytes / h.typesize, h.typesize, w1 - w0, ts);
+        got = -1;
+        break;
+      }
+      osel_slabs(&sel, w0, w1, ts, &g0, &g1);
+      got = oindex_chunk(w, (const uint8_t*)frame + f.off[c], f.dev, &h, codec, &sel, 1, w0, g0, g1, d_dst);
       if (got < 0) break;
     }
     if (c < f.nchunks) { result = got; break; }

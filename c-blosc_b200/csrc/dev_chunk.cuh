@@ -1354,6 +1354,148 @@ extern "C" int b2_launch_boxes_gather(const BoxesGatherArgs* a, b2_stream_t) {
 #endif
 
 
+/* blosc_b200_getoindex: an orthogonal index selection (B2OSel).  The lists need not be sorted, so there is no closed
+ * form for "the next selected item >= x" and the touched blocks are planned forward: oindex_touch_kernel takes the
+ * selection's runs, grid-stride, and marks the blocks (or, on a frame, the chunks) each run's source span overlaps, with
+ * box_touch_kernel's byte test.  Its first work items check the list entries, so the check costs no launch of its own.
+ * The work is proportional to the runs and the list entries, never to the shape. */
+__global__ void __launch_bounds__(PLAN_THREADS) oindex_touch_kernel(OIndexPlanArgs a) {
+  const long long ts = a.plan.typesize, bs = a.plan.blocksize, nb = a.plan.nbytes;
+  const long long ne = a.check ? a.sel.nentries : 0, n = ne + a.r1 - a.r0;
+  const long long wend = a.window + (a.touched ? 0 : b2_box_div(nb, ts));
+  for (long long t = (long long)blockIdx.x * PLAN_THREADS + threadIdx.x; t < n; t += (long long)gridDim.x * PLAN_THREADS) {
+    if (t < ne) {                                /* entry t: list d's position t - lbase[d] */
+      int d = 0;
+#pragma unroll
+      for (int k = 0; k < B2_BOX_MAXDIM; k++)
+        if (k < a.sel.ndim && a.sel.list[k] && t >= a.sel.lbase[k]) d = k;
+      const long long q = t - a.sel.lbase[d], c = a.sel.list[d][q];
+      if (c < 0 || c >= a.sel.shape[d]) atomicMin(a.bad, ((unsigned long long)a.sel.kdim[d] << 56) | (unsigned long long)q);
+      continue;
+    }
+    const long long f = b2_osel_unrank(&a.sel, (a.r0 + t - ne) * a.sel.run);
+    if (f < 0) continue;                         /* a bad entry: the check reports it */
+    if (a.touched) {
+      for (long long c = b2_box_div(f, a.ipc), last = b2_box_div(f + a.sel.run - 1, a.ipc); c <= last; c++)
+        a.touched[c] = 1;
+      continue;
+    }
+    const long long x0 = f > a.window ? f : a.window, x1 = f + a.sel.run < wend ? f + a.sel.run : wend;
+    if (x0 >= x1) continue;
+    for (long long b = b2_box_div((x0 - a.window) * ts, bs), e = (x1 - a.window) * ts; b * bs < e; b++)
+      a.plan.cover[b] = 1;
+  }
+}
+
+/* oindex_gather_kernel: box_gather_kernel's walk over the output bytes [g0, g1), one warp job per GATHER_SPAN bytes,
+ * whole-warp copies for runs of BOX_SHORT_RUN bytes or more and one run per lane below that.  A run's source is the
+ * unrank of its first item, list dimensions reading their entry; repeated and unsorted entries need nothing more.  On
+ * a frame (clip) a run is first tested by its position of dimension 0 alone, one list lookup, and skipped with the
+ * rest of that slab when the coordinate's rows miss the chunk; a run that crosses the window's edge is cut at it. */
+__global__ void __launch_bounds__(GATHER_WARPS * 32) oindex_gather_kernel(OIndexGatherArgs a) {
+  if (a.status && ld_cg_i32(a.status) < 0) return;       /* a stream failed to decode: dest stays untouched */
+  const long long ts = a.typesize, run = a.sel.run, runb = run * ts, slabb = a.sel.slab * ts, total = a.g1 - a.g0;
+  const unsigned bs = (unsigned)a.blocksize;              /* chunk offsets are below 2^31 */
+  const int lane = lane_id();
+  const long long warps = (long long)gridDim.x * GATHER_WARPS;
+  /* whether slab i (a position of dimension 0) has rows inside the window */
+  auto slab_in = [&](long long i) {
+    const long long c = a.sel.list[0] ? a.sel.list[0][i] : a.sel.start[0] + i * a.sel.step[0];
+    return c * a.sel.stride[0] < a.wend && (c + 1) * a.sel.stride[0] > a.window;
+  };
+  for (long long lo = ((long long)blockIdx.x * GATHER_WARPS + (threadIdx.x >> 5)) * GATHER_SPAN; lo < total;
+       lo += warps * GATHER_SPAN) {
+    const long long hi = lo + GATHER_SPAN < total ? lo + GATHER_SPAN : total;
+    if (runb >= BOX_SHORT_RUN) {
+      for (long long o = lo; o < hi;) {
+        const long long g = a.g0 + o, k = b2_box_div(g, runb);
+        long long u = g - k * runb, n = runb - u < hi - o ? runb - u : hi - o;
+        if (a.clip) {
+          const long long i = b2_box_div(g, slabb);
+          if (!slab_in(i)) { o = (i + 1) * slabb - a.g0 < hi ? (i + 1) * slabb - a.g0 : hi; continue; }
+        }
+        const long long f = b2_osel_unrank(&a.sel, k * run);
+        if (a.clip) {                            /* the run's bytes [alo, ahi) whose items lie in the window */
+          const long long alo = (f < a.window ? a.window - f : 0) * ts;
+          const long long ahi = (f + run > a.wend ? a.wend - f : run) * ts;
+          if (u < alo) { o += alo - u < n ? alo - u : n; continue; }
+          if (u >= ahi) { o += n; continue; }
+          if (n > ahi - u) n = ahi - u;
+        }
+        unsigned s = (unsigned)((f - a.window) * ts + u);
+        while (n > 0) {
+          int m = (int)n;
+          const u8* from = a.src + s;
+          if (a.slot) {
+            const unsigned blk = s / bs, left = (blk + 1) * bs - s;
+            if ((unsigned)m > left) m = (int)left;
+            from = a.src + (long long)a.slot[blk] * bs + (s - blk * bs);
+          }
+          warp_copy_vec(a.dst + a.g0 + o, from, m);
+          o += m; s += (unsigned)m; n -= m;
+        }
+      }
+    } else {
+      const long long ka = b2_box_div(a.g0 + lo + runb - 1, runb), kb = b2_box_div(a.g0 + hi + runb - 1, runb);
+      for (long long k = ka + lane; k < kb; k += 32) {
+        if (a.clip && !slab_in(b2_box_div(k * run, a.sel.slab))) continue;
+        const long long f = b2_osel_unrank(&a.sel, k * run);
+        long long x0 = 0, x1 = run;              /* the run's items inside the window */
+        if (a.clip) {
+          if (f < a.window) x0 = a.window - f;
+          if (f + run > a.wend) x1 = a.wend - f;
+        }
+        unsigned s = (unsigned)((f + x0 - a.window) * ts);
+        u8* out = a.dst + (k * run + x0) * ts;
+        const int n = (int)((x1 - x0) * ts);
+        if (!a.slot) {
+          for (int x = 0; x < n; x++) out[x] = a.src[s + x];
+        } else {
+          unsigned bend = 0;
+          const u8* base = a.src;
+          for (int x = 0; x < n; x++, s++) {
+            if (s >= bend) {
+              const unsigned blk = s / bs;
+              bend = (blk + 1) * bs;
+              base = a.src + (long long)a.slot[blk] * bs - (long long)blk * bs;
+            }
+            out[x] = base[s];
+          }
+        }
+      }
+    }
+  }
+}
+
+#ifdef SIMT_EMU
+/* The emulator's launchers of the index-selection kernels, as those of the box kernels: the touch (and, on a chunk
+ * that is not read in place, the slot scan) count as plan launches, the gather as a gather launch. */
+extern "C" int b2_launch_oindex_plan(const OIndexPlanArgs* a, b2_stream_t) {
+  const long long n = (a->check ? a->sel.nentries : 0) + a->r1 - a->r0, nb = a->plan.nblocks;
+  OIndexPlanArgs args = *a;
+  if (n > 0) {
+    simt::launch(simt::Dim3(emu_range_ctas(n)), simt::Dim3(PLAN_THREADS), 0, [&] { oindex_touch_kernel(args); });
+    g_emu_plan_launches++;
+  }
+  if (!a->touched && a->r1 > a->r0 && nb > 0) {
+    simt::launch(simt::Dim3(emu_tiles(nb)), simt::Dim3(PLAN_THREADS), 0, [&] { plan_scan_kernel<PLAN_SLOT>(args.plan, nb); });
+    g_emu_plan_launches++;
+  }
+  return 0;
+}
+extern "C" int b2_launch_oindex_gather(const OIndexGatherArgs* a, b2_stream_t) {
+  const long long total = a->g1 - a->g0;
+  if (total <= 0) return 0;
+  long long ctas = (total + (long long)GATHER_WARPS * GATHER_SPAN - 1) / ((long long)GATHER_WARPS * GATHER_SPAN);
+  if (ctas > 3) ctas = 3;
+  g_emu_gather_launches++;
+  OIndexGatherArgs args = *a;
+  simt::launch(simt::Dim3((unsigned)ctas), simt::Dim3(GATHER_WARPS * 32), 0, [&] { oindex_gather_kernel(args); });
+  return 0;
+}
+#endif
+
+
 /* LZ4 chunks: one CTA of two warps per stream -- a parser that walks the tokens and a copier that owns the output
  * (dev_lz4dpair.cuh).  The parser warp alone draws tickets, checks the size prefixes, counts finished streams and
  * publishes the verdict, exactly as a warp of decode_kernel does. */

@@ -204,6 +204,26 @@ long long blosc_b200_getslice_step(const void* src, int ndim, const int64_t* sha
 long long blosc_b200_getslices(const void* src, int ndim, const int64_t* shape, const int64_t* extent,
                                long long nboxes, const int64_t* starts, void* dest);
 
+/* An orthogonal index selection (numpy: a[np.ix_(...)] with slices kept as slices, made contiguous in C order; zarr's
+ * oindex): dimension k is a list when index != NULL and index[k] != NULL, selecting the coordinates index[k][0 ..
+ * nindex[k]), in any order and with repeats; start[k] / stop[k] / step[k] are then not read.  Every other dimension is
+ * a slice, as in blosc_b200_getslice_step (step == NULL: all ones).  Dimension k contributes n_k = nindex[k] entries for
+ * a list, ceil((stop[k] - start[k]) / step[k]) for a slice, and the result is written to dest as one contiguous C-order
+ * array.  shape, start, stop, step, nindex and the index pointer array are host memory; each list may be host memory
+ * (uploaded once) or device memory on the call's device, chosen as blosc_b200_getitems chooses it, and a device list is
+ * never copied to the host.  src / dest are host or device memory as in blosc_b200_getslice.  With no list (index ==
+ * NULL or all NULL) this is blosc_b200_getslice_step.  Returns the bytes written, prod(n_k) * typesize; 0 when some n_k
+ * is 0, with nothing launched and no list read.  -1 with a message on stderr, before anything is launched, on every
+ * failing check of blosc_b200_getslice_step on the shape and the slice dimensions, nindex[k] < 0, an output size that
+ * overflows int64, or a device list on another device.  The list entries are checked on the GPU by the planning
+ * launch: an entry < 0 or >= shape[k] returns -1 with one message naming the first bad entry (lowest k, then lowest
+ * position), and nothing is decoded or written (negative indices are not wrapped).  The header codes and decode
+ * failures are those of blosc_b200_getslice.  Only the blocks that hold a byte of a selected item are decoded, and the
+ * launches, read-backs and syncs do not grow with the list lengths. */
+long long blosc_b200_getoindex(const void* src, int ndim, const int64_t* shape, const int64_t* start,
+                               const int64_t* stop, const int64_t* step, const int64_t* const* index,
+                               const int64_t* nindex, void* dest);
+
 /* Frames: buffers larger than one chunk (a Blosc-1 chunk holds at most BLOSC_MAX_BUFFERSIZE
  * bytes, blosc.h:40).  The buffer is cut into `chunksize`-byte pieces (0 = 256 MiB; rounded down
  * to a multiple of typesize), each compressed exactly as blosc_compress_ctx() would with
@@ -247,6 +267,12 @@ long long blosc_b200_frame_getslice_step(const void* frame, size_t framesize, in
  * chunks. */
 long long blosc_b200_frame_getslices(const void* frame, size_t framesize, int ndim, const int64_t* shape,
                                      const int64_t* extent, long long nboxes, const int64_t* starts, void* dest);
+/* blosc_b200_getoindex over a frame, with the failures and ordering of blosc_b200_frame_getslice_step: the list
+ * entries are checked once, by one launch that also flags the chunks holding a selected item; chunks that hold none
+ * are neither read nor decoded. */
+long long blosc_b200_frame_getoindex(const void* frame, size_t framesize, int ndim, const int64_t* shape,
+                                     const int64_t* start, const int64_t* stop, const int64_t* step,
+                                     const int64_t* const* index, const int64_t* nindex, void* dest);
 int       blosc_b200_frame_info(const void* frame, size_t framesize, size_t* nbytes, size_t* cbytes,
                                 size_t* chunksize, size_t* nchunks);
 long long blosc_b200_frame_chunk(const void* frame, size_t framesize, size_t i, size_t* chunk_cbytes);
