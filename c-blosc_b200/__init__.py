@@ -83,6 +83,8 @@ def _load(path: str) -> C.CDLL:
     lib.blosc_b200_getoindex.argtypes = [vp, ci, vp, vp, vp, vp, vp, vp, vp]
     lib.blosc_b200_frame_getoindex.restype = ll
     lib.blosc_b200_frame_getoindex.argtypes = [vp, sz, ci, vp, vp, vp, vp, vp, vp, vp]
+    lib.blosc_b200_grid_getslice.restype = ll
+    lib.blosc_b200_grid_getslice.argtypes = [ci, vp, vp, sz, vp, vp, vp, vp, vp, vp]
     lib.blosc_b200_frame_info.restype = ci
     lib.blosc_b200_frame_info.argtypes = [vp, sz, C.POINTER(sz), C.POINTER(sz), C.POINTER(sz), C.POINTER(sz)]
     lib.blosc_b200_frame_chunk.restype = ll
@@ -217,6 +219,38 @@ def getslices(src, shape, extent, starts, dest):
     or a sequence.  Returns the bytes written, or a negative code (dest is then untouched)."""
     sh, ex, st = _boxes(shape, extent, starts)
     return int(lib.blosc_b200_getslices(_ptr(src), sh.size, sh.ctypes.data, ex.ctypes.data, st[2], st[1], _ptr(dest)))
+
+
+def grid_getslice(chunks, shape, chunkshape, itemsize, start, stop, dest, step=None, fill=None):
+    """A box, with steps, of the C-order array of `shape` stored as a regular grid of chunks (zarr v2, HDF5 blosc,
+    PyTables; blosc_b200_grid_getslice): `chunks` lists the ceil(shape[k] / chunkshape[k]) chunks per dimension in C
+    order of the grid, each a Blosc-1 chunk of its sub-array at full chunk shape (bytes, bytearray, a numpy array or a
+    torch tensor on the host or on CUDA), or None for a missing chunk, whose items are `fill` (itemsize bytes, or a
+    numpy scalar of that size; None: zeros).  Items are `itemsize` bytes whatever the chunks' header typesize.  Writes
+    numpy's a[start:stop:step] to `dest` as one contiguous C-order array, as getslice does.  Returns the bytes written,
+    or a negative code (a host dest is then untouched)."""
+    import numpy as np
+    sh, st, sp = _box(shape, start, stop)
+    cs = np.ascontiguousarray(chunkshape, dtype=np.int64).reshape(-1)
+    if cs.size != sh.size:
+        raise ValueError(f"shape and chunkshape have {sh.size} and {cs.size} entries")
+    if (cs >= 1).all() and (sh >= 0).all():                # else the library rejects the geometry
+        nchunks = 1
+        for s, c in zip(sh.tolist(), cs.tolist()):
+            nchunks *= -(-s // c)
+        if len(chunks) != nchunks:
+            raise ValueError(f"{len(chunks)} chunks, but the grid has {nchunks}")
+    table = (C.c_void_p * max(len(chunks), 1))(*[_ptr(c) for c in chunks])
+    f = None
+    if fill is not None:
+        f = np.frombuffer(bytes(fill), np.uint8) if isinstance(fill, (bytes, bytearray)) else \
+            np.ascontiguousarray(fill).reshape(-1).view(np.uint8)
+        if f.size != itemsize:
+            raise ValueError(f"fill has {f.size} bytes, not the itemsize {itemsize}")
+    t = None if step is None else _step(sh, step)
+    return int(lib.blosc_b200_grid_getslice(sh.size, sh.ctypes.data, cs.ctypes.data, itemsize, table,
+                                            None if f is None else f.ctypes.data, st.ctypes.data, sp.ctypes.data,
+                                            None if t is None else t.ctypes.data, _ptr(dest)))
 
 
 def _name(compressor):

@@ -560,6 +560,27 @@ typedef struct OIndexGatherArgs {
   const int* status;
 } OIndexGatherArgs;
 
+/* One touched chunk of a chunk grid (blosc_b200_grid_getslice) and its part of the selection, as two boxes with the
+ * same extents: `box` in the chunk's own coordinates (over the chunk shape, with the selection's steps) and `out` in
+ * the output array's (step 1), so box item p of the one is box item p of the other.  placed_gather_kernel copies run q
+ * of `run` items from box's unrank of q * run in the chunk to out's unrank of q * run in dst; `run` is the shorter of
+ * the two boxes' runs (each is a product of trailing extents, so it divides the longer).  placed_fill_kernel (a missing
+ * chunk; box, slot, src and status unused) writes the itemsize-byte pattern `fill`, or zeros when it is NULL, over out
+ * instead.  slot / src / status as in BoxGatherArgs. */
+typedef struct PlacedGatherArgs {
+  B2Box box;
+  B2Box out;
+  long long run;
+  long long total;            /* bytes of the part: out.count * itemsize */
+  long long itemsize;
+  int blocksize, pad;
+  const int* slot;
+  const uint8_t* src;
+  const uint8_t* fill;        /* device memory */
+  uint8_t* dst;
+  const int* status;
+} PlacedGatherArgs;
+
 #ifdef __cplusplus
 }
 #endif

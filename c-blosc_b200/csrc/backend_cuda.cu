@@ -527,3 +527,27 @@ extern "C" int b2_launch_oindex_gather(const OIndexGatherArgs* a, b2_stream_t s)
   CK(cudaGetLastError());
   return 0;
 }
+
+/* the placed gather and fill of grid_getslice (stepped or not, as the chunk's box), counted as gather launches */
+static unsigned gather_ctas(long long total) {
+  long long ctas = (total + (long long)GATHER_WARPS * GATHER_SPAN - 1) / ((long long)GATHER_WARPS * GATHER_SPAN);
+  if (ctas > (long long)num_sms() * 8) ctas = (long long)num_sms() * 8;
+  return (unsigned)ctas;
+}
+
+extern "C" int b2_launch_placed_gather(const PlacedGatherArgs* a, b2_stream_t s) {
+  if (a->total <= 0) return 0;
+  ProfScope ps(B2_K_GATHER, s->s);
+  if (a->box.stepped) placed_gather_kernel<true><<<gather_ctas(a->total), GATHER_WARPS * 32, 0, s->s>>>(*a);
+  else placed_gather_kernel<false><<<gather_ctas(a->total), GATHER_WARPS * 32, 0, s->s>>>(*a);
+  CK(cudaGetLastError());
+  return 0;
+}
+
+extern "C" int b2_launch_placed_fill(const PlacedGatherArgs* a, b2_stream_t s) {
+  if (a->total <= 0) return 0;
+  ProfScope ps(B2_K_GATHER, s->s);
+  placed_fill_kernel<<<gather_ctas(a->total), GATHER_WARPS * 32, 0, s->s>>>(*a);
+  CK(cudaGetLastError());
+  return 0;
+}

@@ -215,8 +215,9 @@ static void ws_release(b2_ws* w) {
 /* A workspace = one stream + scratch on one device.  The reference's _ctx calls have no limit on the
  * number of concurrent callers (each allocates its own context, blosc.c:1287-1309); here the 17th
  * concurrent call WAITS for a slot instead of failing, and an idle slot that was made on another
- * device is rebuilt for the caller's device when no matching or unused slot is left. */
-static b2_ws* ws_acquire(void) {
+ * device is rebuilt for the caller's device when no matching or unused slot is left.  wait 0: NULL at once instead of
+ * waiting (a helper thread of a call that already holds a slot, which must not wait for the slot it holds). */
+static b2_ws* ws_acquire_if(int wait) {
   b2_ws* w = NULL;
   int i, dev, rebuild = 0;
   if (!backend_ready()) return NULL;
@@ -230,9 +231,11 @@ static b2_ws* ws_acquire(void) {
     for (i = 0; i < B2_MAX_WS && !w; i++)
       if (!g_ws[i].in_use) { w = &g_ws[i]; rebuild = 1; }
     if (w) { w->in_use = 1; break; }
+    if (!wait) break;
     pthread_cond_wait(&g_ws_cv, &g_ws_mutex);
   }
   pthread_mutex_unlock(&g_ws_mutex);
+  if (!w) return NULL;
   if (rebuild) ws_teardown(w);
   if (!w->ready) {
     void* p = NULL;
@@ -254,6 +257,8 @@ static b2_ws* ws_acquire(void) {
   }
   return w;
 }
+
+static b2_ws* ws_acquire(void) { return ws_acquire_if(1); }
 
 static int buf_ensure(b2_buf* b, size_t need) {
   if (need <= b->cap) return 0;
@@ -2572,6 +2577,286 @@ long long blosc_b200_frame_getoindex(const void* frame, size_t framesize, int nd
   ws_release(w);
   free(head);
   free(f.off);
+  return result;
+}
+
+/* ------------------------------------------------------------------------- */
+/* boxes of arrays stored as a grid of chunks (blosc_b200_grid_getslice)      */
+/* ------------------------------------------------------------------------- */
+/* zarr v2, the HDF5 blosc filter and PyTables store an N-d array as a regular grid of equally shaped chunks, each one
+ * Blosc-1 buffer holding its sub-array in C order (edge chunks at full shape, their padding never read).  The chunks a
+ * selection touches follow from the geometry alone: per dimension, the chunk indices that hold a selected coordinate,
+ * and their product in C order.  A touched chunk's part is two boxes with the same extents (PlacedGatherArgs): one in
+ * the chunk's coordinates, which plans and decodes the chunk as getslice_step does, and one in the output's, where the
+ * placed gather writes the part directly.  A missing chunk is one placed fill.  Touched chunks are taken in ascending
+ * order by up to BLOSC_B200_FRAME_WORKERS threads, each with its own workspace and stream; the parts are disjoint in
+ * dest, so they are written without ordering. */
+typedef struct {
+  pthread_mutex_t mu;
+  int ndim, dev, failed, err;
+  long long next, ntouched, failed_at;     /* the next touched chunk to take; the lowest failing one */
+  const int64_t *chunkshape, *start, *step;
+  int64_t shape[B2_BOX_MAXDIM], n[B2_BOX_MAXDIM];  /* the array's shape and the output's */
+  long long itemsize, chunk_items, out_items;
+  long long* list[B2_BOX_MAXDIM];          /* the chunk indices of dimension k that hold a selected coordinate */
+  long long nlist[B2_BOX_MAXDIM];
+  const void** src;                        /* [ntouched] the touched chunks' table entries, in grid C order */
+  uint8_t* src_dev;                        /* [ntouched] which of them are device memory */
+  const uint8_t* fill;                     /* the fill pattern in device memory, or NULL for zeros */
+  uint8_t* d_dst;
+} b2_grid_job;
+
+/* The checks of grid_getslice that need no chunk: getslice_step's on the shape, the chunk shape, the item size and a
+ * chunk's bytes (*chunk_items: the items of one chunk).  -1 with a message when one fails. */
+static int grid_geometry(int ndim, const int64_t* shape, const int64_t* chunkshape, size_t itemsize,
+                         const int64_t* start, const int64_t* stop, const int64_t* step, long long* chunk_items) {
+  long long nitems = 0, items = 1;
+  int k;
+  if (box_geometry(ndim, shape, start, stop, &nitems) || box_steps(ndim, step)) return -1;
+  if (itemsize < 1) { fprintf(stderr, "blosc_b200: itemsize is 0\n"); return -1; }
+  for (k = 0; k < ndim; k++)
+    if (chunkshape[k] < 1) {
+      fprintf(stderr, "blosc_b200: chunkshape[%d] = %lld is not >= 1\n", k, (long long)chunkshape[k]);
+      return -1;
+    }
+  for (k = 0; k < ndim && items <= BLOSC_MAX_BUFFERSIZE; k++)
+    items = chunkshape[k] > BLOSC_MAX_BUFFERSIZE ? (long long)BLOSC_MAX_BUFFERSIZE + 1 : items * chunkshape[k];
+  if (items > BLOSC_MAX_BUFFERSIZE || itemsize > (size_t)(BLOSC_MAX_BUFFERSIZE / items)) {
+    fprintf(stderr, "blosc_b200: a chunk of the chunk shape and %zu-byte items is larger than %d bytes\n", itemsize,
+            BLOSC_MAX_BUFFERSIZE);
+    return -1;
+  }
+  *chunk_items = items;
+  return 0;
+}
+
+/* The first selected coordinate of dimension k at or after `org` and below `lim`, or -1 when there is none */
+static long long grid_first(const b2_grid_job* j, int k, long long org, long long lim) {
+  const long long s = j->start[k], t = j->step[k], d = org - s;
+  const long long q = d <= 0 ? 0 : d / t + (d % t != 0);
+  return q < j->n[k] && s + q * t < lim ? s + q * t : -1;      /* q < n: s + q * t is a selected coordinate */
+}
+
+/* The per-dimension lists of touched chunk indices, ascending: the chunks of the selected coordinates, or the chunks of
+ * the selection's span that hold one, whichever is fewer to walk.  Returns the number of touched chunks, or -1. */
+static long long grid_lists(b2_grid_job* j) {
+  long long total = 1;
+  int k;
+  for (k = 0; k < j->ndim; k++) {
+    const long long cs = j->chunkshape[k], t = j->step[k], first = j->start[k], last = first + (j->n[k] - 1) * t;
+    const long long c0 = first / cs, c1 = last / cs;
+    long long i, c, m = 0;
+    if (!(j->list[k] = (long long*)malloc(8 * (size_t)(j->n[k] < c1 - c0 + 1 ? j->n[k] : c1 - c0 + 1)))) return -1;
+    if (j->n[k] < c1 - c0 + 1) {
+      for (i = 0; i < j->n[k]; i++)
+        if (m == 0 || j->list[k][m - 1] != (first + i * t) / cs) j->list[k][m++] = (first + i * t) / cs;
+    } else {
+      for (c = c0; c <= c1; c++) {
+        const long long org = c * cs, lim = cs < j->shape[k] - org ? org + cs : j->shape[k];
+        if (grid_first(j, k, org, lim) >= 0) j->list[k][m++] = c;
+      }
+    }
+    j->nlist[k] = m;
+    total *= m;                          /* at most the grid's chunks, which the caller's table holds */
+  }
+  return total;
+}
+
+/* The grid coordinates of touched chunk `t` (its position in C order of the lists' product), and its index in the
+ * chunk table */
+static long long grid_coords(const b2_grid_job* j, long long t, long long* c) {
+  long long g = 0, gs = 1;
+  int k;
+  for (k = j->ndim - 1; k >= 0; k--) {
+    c[k] = j->list[k][t % j->nlist[k]];
+    t /= j->nlist[k];
+    g += c[k] * gs;
+    gs *= (j->shape[k] - 1) / j->chunkshape[k] + 1;
+  }
+  return g;
+}
+
+/* The part of the chunk at grid coordinates c, as the box in the chunk's coordinates and the box in the output's */
+static void grid_part(const b2_grid_job* j, const long long* c, B2Box* box, B2Box* out) {
+  int64_t lst[B2_BOX_MAXDIM], lsp[B2_BOX_MAXDIM], ost[B2_BOX_MAXDIM], osp[B2_BOX_MAXDIM];
+  int k;
+  for (k = 0; k < j->ndim; k++) {
+    const long long cs = j->chunkshape[k], t = j->step[k], org = c[k] * cs;
+    const long long lim = cs < j->shape[k] - org ? org + cs : j->shape[k];
+    const long long last = j->start[k] + (j->n[k] - 1) * t, hi = last < lim - 1 ? last : lim - 1;
+    const long long f = grid_first(j, k, org, lim), l = f + (hi - f) / t * t;
+    lst[k] = f - org; lsp[k] = l - org + 1;
+    ost[k] = (f - j->start[k]) / t; osp[k] = ost[k] + (l - f) / t + 1;
+  }
+  box_build(j->ndim, j->chunkshape, lst, lsp, j->step, j->chunk_items, box);
+  box_build(j->ndim, j->n, ost, osp, NULL, j->out_items, out);
+}
+
+static long long grid_take(b2_grid_job* j) {
+  long long t;
+  pthread_mutex_lock(&j->mu);
+  t = !j->failed && j->next < j->ntouched ? j->next++ : -1;
+  pthread_mutex_unlock(&j->mu);
+  return t;
+}
+
+/* Touched chunk t failed with rc: the lowest failing chunk decides the result.  Chunks are taken in ascending order,
+ * so every chunk below t was taken already and finishes; none above it is taken from now on. */
+static void grid_fail(b2_grid_job* j, long long t, int rc) {
+  pthread_mutex_lock(&j->mu);
+  if (t < j->failed_at) { j->failed_at = t; j->err = rc; }
+  j->failed = 1;
+  pthread_mutex_unlock(&j->mu);
+}
+
+/* Touched chunk t, present at grid coordinates c: its header checked with blosc_getitem's codes and its bytes against
+ * the chunk shape, its touched blocks planned at the caller's item size (the header's typesize only unshuffles) and
+ * decoded, and its part gathered into place.  Returns 0, blosc_getitem's or blosc_d's code, or -1. */
+static int grid_chunk(const b2_grid_job* j, b2_ws* w, long long t, const long long* c, const B2Box* box,
+                      const B2Box* out) {
+  const void* src = j->src[t];
+  const int src_dev = j->src_dev[t];
+  GetitemsPlan rec = {0};
+  PlacedGatherArgs ga;
+  b2_hdr h;
+  int codec = 0, rc, k;
+  if ((rc = getitem_header(w, src, src_dev, -1, &h, &codec))) return rc;
+  if ((long long)h.nbytes != j->chunk_items * j->itemsize) {
+    char at[B2_BOX_MAXDIM * 24];
+    size_t o = 0;
+    for (k = 0; k < j->ndim; k++) o += (size_t)snprintf(at + o, sizeof at - o, k ? ", %lld" : "%lld", c[k]);
+    fprintf(stderr, "blosc_b200: chunk (%s) holds %d bytes, not the %lld of its shape\n", at, h.nbytes,
+            j->chunk_items * j->itemsize);
+    return -1;
+  }
+  memset(&ga, 0, sizeof ga);
+  ga.box = *box; ga.out = *out; ga.run = box->run < out->run ? box->run : out->run;
+  ga.total = out->count * j->itemsize; ga.itemsize = j->itemsize; ga.blocksize = h.blocksize; ga.dst = j->d_dst;
+  if (!((h.flags & BLOSC_MEMCPYED) && src_dev)) {            /* a memcpyed device chunk is read in place: no plan */
+    BoxPlanArgs bp;
+    bp.box = *box; bp.window = 0;
+    if (!plan_scratch(w, &h, 0, 0, &bp.plan)) return -1;
+    bp.plan.typesize = (int)j->itemsize;
+    if (b2_launch_box_plan(&bp, w->stream) || read_plan(w, bp.plan.rec, &rec, sizeof rec)) return -1;
+    ga.slot = bp.plan.slot;
+  }
+  if (touched_source(w, src, src_dev, &h, codec, rec.nlisted, rec.has_left, &ga.src, &ga.status)) return -1;
+  if (b2_launch_placed_gather(&ga, w->stream)) { ws_reset_counters(w); return -1; }
+  return read_verdict(w, ga.status);
+}
+
+/* A worker: takes touched chunks until none is left or one has failed.  A missing chunk is one fill launch, with no
+ * sync; the worker's stream is drained once at the end. */
+static void grid_work(b2_grid_job* j, b2_ws* w) {
+  long long t, c[B2_BOX_MAXDIM];
+  B2Box box, out;
+  while ((t = grid_take(j)) >= 0) {
+    int rc = 0;
+    grid_coords(j, t, c);
+    grid_part(j, c, &box, &out);
+    if (j->src[t]) rc = grid_chunk(j, w, t, c, &box, &out);
+    else {
+      PlacedGatherArgs fa;
+      memset(&fa, 0, sizeof fa);
+      fa.out = out; fa.run = out.run; fa.total = out.count * j->itemsize; fa.itemsize = j->itemsize;
+      fa.fill = j->fill; fa.dst = j->d_dst;
+      if (b2_launch_placed_fill(&fa, w->stream)) rc = -1;
+    }
+    if (rc < 0) grid_fail(j, t, rc);
+  }
+  if (b2_stream_sync(w->stream)) grid_fail(j, j->ntouched, -1);
+}
+
+/* A worker thread beside the caller's: on the call's device, with a workspace of its own when one is free (else the
+ * other workers take its share) */
+static void* grid_helper(void* arg) {
+  b2_grid_job* j = (b2_grid_job*)arg;
+  b2_ws* w;
+  b2_set_device(j->dev);
+  if (!(w = ws_acquire_if(0))) return NULL;
+  grid_work(j, w);
+  ws_release(w);
+  return NULL;
+}
+
+long long blosc_b200_grid_getslice(int ndim, const int64_t* shape, const int64_t* chunkshape, size_t itemsize,
+                                   const void* const* chunks, const void* fill, const int64_t* start,
+                                   const int64_t* stop, const int64_t* step, void* dest) {
+  static const int64_t ones[B2_BOX_MAXDIM] = {1, 1, 1, 1, 1, 1, 1, 1};
+  pthread_t th[B2_FRAME_MAX_WORKERS];
+  b2_grid_job j;
+  b2_ws* w = NULL;
+  long long t, c[B2_BOX_MAXDIM], chunk_items = 0, nbytes = 0, result = -1;
+  int k, dest_dev, dev, old_dev = 0, started = 0, missing = 0, workers;
+  if (grid_geometry(ndim, shape, chunkshape, itemsize, start, stop, step, &chunk_items)) return -1;
+  if (box_empty(ndim, start, stop)) return 0;
+  memset(&j, 0, sizeof j);
+  j.chunk_items = chunk_items; j.ndim = ndim; j.chunkshape = chunkshape; j.start = start; j.step = step ? step : ones;
+  j.itemsize = (long long)itemsize; j.out_items = 1;
+  for (k = 0; k < ndim; k++) {
+    j.shape[k] = shape[k];
+    j.n[k] = (stop[k] - start[k] - 1) / j.step[k] + 1;
+    j.out_items *= j.n[k];                 /* at most the array's items */
+  }
+  if (j.out_items > LLONG_MAX / j.itemsize) {
+    fprintf(stderr, "blosc_b200: the output of %lld items of %zu bytes overflows int64\n", j.out_items, itemsize);
+    return -1;
+  }
+  nbytes = j.out_items * j.itemsize;
+  if (!chunks) { fprintf(stderr, "blosc_b200: chunks is NULL\n"); return -1; }
+  do {
+    if ((j.ntouched = grid_lists(&j)) < 0) break;
+    j.src = (const void**)malloc(sizeof(void*) * (size_t)j.ntouched);
+    j.src_dev = (uint8_t*)malloc((size_t)j.ntouched);
+    if (!j.src || !j.src_dev) break;
+    for (t = 0; t < j.ntouched; t++) {                 /* the table entries of touched chunks, and no other */
+      j.src[t] = chunks[grid_coords(&j, t, c)];
+      j.src_dev[t] = j.src[t] && b2_ptr_is_device(j.src[t]);
+      missing |= !j.src[t];
+    }
+    /* the call runs on dest's device, else on the first device chunk's, else on the current one */
+    dest_dev = b2_ptr_is_device(dest);
+    dev = dest_dev ? b2_ptr_device(dest) : -1;
+    for (t = 0; t < j.ntouched && dev < 0; t++) if (j.src_dev[t]) dev = b2_ptr_device(j.src[t]);
+    if (dev < 0) dev = b2_get_device();
+    for (t = 0; t < j.ntouched; t++)
+      if (j.src_dev[t] && b2_ptr_device(j.src[t]) != dev) break;
+    if (t < j.ntouched) {
+      fprintf(stderr, "blosc_b200: chunk %lld of the table is on device %d, not on device %d where the call runs\n",
+              grid_coords(&j, t, c), b2_ptr_device(j.src[t]), dev);
+      break;
+    }
+    if (!backend_ready()) break;
+    old_dev = b2_get_device();
+    if (dev != old_dev && b2_set_device(dev)) break;
+    if ((w = ws_acquire())) {
+      do {
+        if (!(j.d_dst = stage_dest(&w->fstage, dest, dest_dev, (size_t)nbytes))) break;
+        if (missing && fill) {
+          if (buf_ensure(&w->fplan, itemsize) || copy_any(w->fplan.p, 1, fill, b2_ptr_is_device(fill), itemsize, w->stream))
+            break;
+          j.fill = (const uint8_t*)w->fplan.p;
+        }
+        pthread_mutex_init(&j.mu, NULL);
+        j.dev = dev; j.failed_at = LLONG_MAX;
+        workers = frame_workers(j.ntouched < B2_FRAME_MAX_WORKERS ? (int)j.ntouched : B2_FRAME_MAX_WORKERS);
+        for (k = 1; k < workers; k++) {
+          if (pthread_create(&th[started], NULL, grid_helper, &j) != 0) break;
+          started++;
+        }
+        grid_work(&j, w);                              /* the calling thread is a worker too */
+        for (k = 0; k < started; k++) pthread_join(th[k], NULL);
+        pthread_mutex_destroy(&j.mu);
+        if (j.failed) { result = j.err; break; }
+        if (!dest_dev && d2h_any(w, dest, j.d_dst, (size_t)nbytes)) break;
+        result = nbytes;
+      } while (0);
+      ws_release(w);
+    }
+    if (dev != old_dev) b2_set_device(old_dev);
+  } while (0);
+  for (k = 0; k < ndim; k++) free(j.list[k]);
+  free(j.src); free(j.src_dev);
   return result;
 }
 

@@ -25,6 +25,10 @@
  *                   a batch of boxes of one extent (blosc_b200_getslices): the corners' check,
  *                   the blocks touched by any box and the copy out, from the origin box and one
  *                   flat offset per box
+ *   placed_gather_kernel, placed_fill_kernel
+ *                   one chunk's part of a box of an array stored as a grid of chunks
+ *                   (blosc_b200_grid_getslice), written straight into its place in the output,
+ *                   or the fill value over the part of a missing chunk
  */
 #pragma once
 #include "b2_args.h"
@@ -1491,6 +1495,110 @@ extern "C" int b2_launch_oindex_gather(const OIndexGatherArgs* a, b2_stream_t) {
   g_emu_gather_launches++;
   OIndexGatherArgs args = *a;
   simt::launch(simt::Dim3((unsigned)ctas), simt::Dim3(GATHER_WARPS * 32), 0, [&] { oindex_gather_kernel(args); });
+  return 0;
+}
+#endif
+
+
+/* blosc_b200_grid_getslice: a touched chunk's part written straight into its place in the output (PlacedGatherArgs).
+ * The walk is box_gather_kernel's over the part's bytes [0, total), one warp job per GATHER_SPAN bytes, with the run's
+ * source the chunk box's unrank and its destination the output box's.  The part starts at a run edge and holds whole
+ * runs, so a lane-per-run job takes exactly the runs that start in its bytes.  STEPPED = the chunk box's `stepped`;
+ * the output box has step 1.  A kernel of its own, so that the box kernels' code and registers stay as they are. */
+template <bool STEPPED>
+__global__ void __launch_bounds__(GATHER_WARPS * 32) placed_gather_kernel(PlacedGatherArgs a) {
+  if (a.status && ld_cg_i32(a.status) < 0) return;       /* a stream failed to decode: dest stays untouched */
+  const long long ts = a.itemsize, runb = a.run * ts;
+  const unsigned bs = (unsigned)a.blocksize;              /* chunk offsets are below 2^31 */
+  const int lane = lane_id();
+  const long long warps = (long long)gridDim.x * GATHER_WARPS;
+  for (long long lo = ((long long)blockIdx.x * GATHER_WARPS + (threadIdx.x >> 5)) * GATHER_SPAN; lo < a.total;
+       lo += warps * GATHER_SPAN) {
+    const long long hi = lo + GATHER_SPAN < a.total ? lo + GATHER_SPAN : a.total;
+    if (runb >= BOX_SHORT_RUN) {
+      for (long long o = lo; o < hi;) {
+        const long long k = b2_box_div(o, runb), u = o - k * runb;
+        u8* out = a.dst + b2_box_unrank(&a.out, k * a.run, 0) * ts + u;
+        unsigned s = (unsigned)(b2_box_unrank(&a.box, k * a.run, STEPPED) * ts + u);
+        long long n = runb - u < hi - o ? runb - u : hi - o;
+        while (n > 0) {
+          int m = (int)n;
+          const u8* from = a.src + s;
+          if (a.slot) {
+            const unsigned blk = s / bs, left = (blk + 1) * bs - s;
+            if ((unsigned)m > left) m = (int)left;
+            from = a.src + (long long)a.slot[blk] * bs + (s - blk * bs);
+          }
+          warp_copy_vec(out, from, m);
+          out += m; o += m; s += (unsigned)m; n -= m;
+        }
+      }
+    } else {
+      const long long ka = b2_box_div(lo + runb - 1, runb), kb = b2_box_div(hi + runb - 1, runb);
+      for (long long k = ka + lane; k < kb; k += 32) {
+        unsigned s = (unsigned)(b2_box_unrank(&a.box, k * a.run, STEPPED) * ts);
+        u8* out = a.dst + b2_box_unrank(&a.out, k * a.run, 0) * ts;
+        const int n = (int)runb;
+        if (!a.slot) {
+          for (int x = 0; x < n; x++) out[x] = a.src[s + x];
+        } else {
+          unsigned bend = 0;
+          const u8* base = a.src;
+          for (int x = 0; x < n; x++, s++) {
+            if (s >= bend) {
+              const unsigned blk = s / bs;
+              bend = (blk + 1) * bs;
+              base = a.src + (long long)a.slot[blk] * bs - (long long)blk * bs;
+            }
+            out[x] = base[s];
+          }
+        }
+      }
+    }
+  }
+}
+
+/* placed_fill_kernel: a missing chunk's part of the output, the output box `out`, filled with the item pattern.  Warp
+ * job k covers the part's bytes [k * GATHER_SPAN, (k + 1) * GATHER_SPAN), cut at run edges; the lanes store each
+ * piece's consecutive bytes.  A run starts at an item edge, so byte u of a run is byte u % itemsize of the pattern. */
+__global__ void __launch_bounds__(GATHER_WARPS * 32) placed_fill_kernel(PlacedGatherArgs a) {
+  const long long runb = a.run * a.itemsize;
+  const unsigned ts = (unsigned)a.itemsize;               /* a part's bytes are below 2^31 */
+  const int lane = lane_id();
+  const long long warps = (long long)gridDim.x * GATHER_WARPS;
+  for (long long lo = ((long long)blockIdx.x * GATHER_WARPS + (threadIdx.x >> 5)) * GATHER_SPAN; lo < a.total;
+       lo += warps * GATHER_SPAN) {
+    const long long hi = lo + GATHER_SPAN < a.total ? lo + GATHER_SPAN : a.total;
+    for (long long o = lo; o < hi;) {
+      const long long k = b2_box_div(o, runb), u = o - k * runb;
+      u8* out = a.dst + b2_box_unrank(&a.out, k * a.run, 0) * a.itemsize + u;
+      const int n = (int)(runb - u < hi - o ? runb - u : hi - o);
+      for (int x = lane; x < n; x += 32) out[x] = a.fill ? a.fill[((unsigned)u + (unsigned)x) % ts] : 0;
+      o += n;
+    }
+  }
+}
+
+#ifdef SIMT_EMU
+/* The emulator's launchers of the placed kernels, as those of the box kernels; both count as gather launches */
+static unsigned emu_gather_ctas(long long total) {
+  const long long ctas = (total + (long long)GATHER_WARPS * GATHER_SPAN - 1) / ((long long)GATHER_WARPS * GATHER_SPAN);
+  return (unsigned)(ctas > 3 ? 3 : ctas);
+}
+extern "C" int b2_launch_placed_gather(const PlacedGatherArgs* a, b2_stream_t) {
+  if (a->total <= 0) return 0;
+  g_emu_gather_launches++;
+  PlacedGatherArgs args = *a;
+  simt::launch(simt::Dim3(emu_gather_ctas(a->total)), simt::Dim3(GATHER_WARPS * 32), 0, [&] {
+    if (args.box.stepped) placed_gather_kernel<true>(args); else placed_gather_kernel<false>(args);
+  });
+  return 0;
+}
+extern "C" int b2_launch_placed_fill(const PlacedGatherArgs* a, b2_stream_t) {
+  if (a->total <= 0) return 0;
+  g_emu_gather_launches++;
+  PlacedGatherArgs args = *a;
+  simt::launch(simt::Dim3(emu_gather_ctas(a->total)), simt::Dim3(GATHER_WARPS * 32), 0, [&] { placed_fill_kernel(args); });
   return 0;
 }
 #endif

@@ -277,6 +277,30 @@ int       blosc_b200_frame_info(const void* frame, size_t framesize, size_t* nby
                                 size_t* chunksize, size_t* nchunks);
 long long blosc_b200_frame_chunk(const void* frame, size_t framesize, size_t i, size_t* chunk_cbytes);
 
+/* blosc_b200_getslice_step over an N-d array stored as a regular grid of chunks (zarr v2, the HDF5 blosc filter,
+ * PyTables): the C-order array of `shape`, items of `itemsize` bytes, is cut into grid[k] = ceil(shape[k] /
+ * chunkshape[k]) chunks per dimension.  chunks is a host array of prod(grid) pointers in C order of the grid, each a
+ * Blosc-1 chunk in host or device memory holding its sub-array of prod(chunkshape) * itemsize bytes in C order (edge
+ * chunks at full shape; their padding is never read), or NULL for a missing chunk, whose items are the itemsize bytes
+ * at `fill` (host memory; NULL: zero bytes).  The selection is blosc_b200_getslice_step's, written to dest (host or
+ * device memory) as one contiguous C-order array.  Only the table entries of touched chunks (those holding a selected
+ * item) are read, and in a touched chunk only the blocks holding a byte of a selected item are decoded.  The item size
+ * is the caller's: a chunk's header typesize may differ (it is used for unshuffling alone), and chunks may differ in
+ * codec, filter and typesize; only the header's nbytes must be prod(chunkshape) * itemsize.  Each touched chunk's part
+ * is gathered straight into its place in dest, and touched chunks are read by up to BLOSC_B200_FRAME_WORKERS threads
+ * (default 4) at once.  Returns the bytes written, prod(n_k) * itemsize; 0 for an empty selection, with nothing launched
+ * or read (chunks may then be NULL).  -1 with a message on stderr, before anything is launched or read, on every
+ * failing check of blosc_b200_getslice_step against `shape`, chunkshape[k] < 1, itemsize < 1, a chunk larger than
+ * BLOSC_MAX_BUFFERSIZE bytes, an output size that overflows int64, chunks == NULL, or a touched device chunk on another
+ * device than the call's: dest's when dest is device memory, else the first touched device chunk's, else the one
+ * chosen with blosc_b200_set_device.  A touched chunk's header failure returns blosc_getitem's code, an nbytes other
+ * than prod(chunkshape) * itemsize returns -1 with a message naming its grid coordinates, and a touched block that
+ * fails to decode returns blosc_d's code; when several touched chunks fail, the lowest in grid C order decides, whatever
+ * the number of workers.  On a failure a host dest is untouched; a device dest may hold the parts of other chunks. */
+long long blosc_b200_grid_getslice(int ndim, const int64_t* shape, const int64_t* chunkshape, size_t itemsize,
+                                   const void* const* chunks, const void* fill, const int64_t* start,
+                                   const int64_t* stop, const int64_t* step, void* dest);
+
 /* Select the CUDA device used by the calling thread's subsequent calls with HOST pointers
  * (device pointers carry their device).  Multi-GPU callers run one process (or thread) per GPU. */
 int blosc_b200_set_device(int dev);
