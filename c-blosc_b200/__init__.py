@@ -85,6 +85,10 @@ def _load(path: str) -> C.CDLL:
     lib.blosc_b200_frame_getoindex.argtypes = [vp, sz, ci, vp, vp, vp, vp, vp, vp, vp]
     lib.blosc_b200_grid_getslice.restype = ll
     lib.blosc_b200_grid_getslice.argtypes = [ci, vp, vp, sz, vp, vp, vp, vp, vp, vp]
+    lib.blosc_b200_grid_bound.restype = sz
+    lib.blosc_b200_grid_bound.argtypes = [ci, vp, vp, sz]
+    lib.blosc_b200_grid_compress.restype = ll
+    lib.blosc_b200_grid_compress.argtypes = [ci, ci, sz, C.c_char_p, sz, ci, ci, vp, vp, sz, vp, vp, ci, vp, sz, vp]
     lib.blosc_b200_frame_info.restype = ci
     lib.blosc_b200_frame_info.argtypes = [vp, sz, C.POINTER(sz), C.POINTER(sz), C.POINTER(sz), C.POINTER(sz)]
     lib.blosc_b200_frame_chunk.restype = ll
@@ -221,6 +225,77 @@ def getslices(src, shape, extent, starts, dest):
     return int(lib.blosc_b200_getslices(_ptr(src), sh.size, sh.ctypes.data, ex.ctypes.data, st[2], st[1], _ptr(dest)))
 
 
+def _fill(fill, itemsize):
+    """a grid's fill value as itemsize bytes in a numpy array (bytes, or a numpy scalar of that size), or None"""
+    import numpy as np
+    if fill is None:
+        return None
+    f = np.frombuffer(bytes(fill), np.uint8) if isinstance(fill, (bytes, bytearray)) else \
+        np.ascontiguousarray(fill).reshape(-1).view(np.uint8)
+    if f.size != itemsize:
+        raise ValueError(f"fill has {f.size} bytes, not the itemsize {itemsize}")
+    return f
+
+
+def _grid_shapes(shape, chunkshape):
+    import numpy as np
+    sh = np.ascontiguousarray(shape, dtype=np.int64).reshape(-1)
+    cs = np.ascontiguousarray(chunkshape, dtype=np.int64).reshape(-1)
+    if cs.size != sh.size:
+        raise ValueError(f"shape and chunkshape have {sh.size} and {cs.size} entries")
+    return sh, cs
+
+
+def _nbytes(buf):
+    if hasattr(buf, "untyped_storage"):     # torch.Tensor
+        return buf.numel() * buf.element_size()
+    return buf.nbytes if hasattr(buf, "nbytes") else len(buf)
+
+
+def grid_bound(shape, chunkshape, itemsize) -> int:
+    """Bytes that always hold grid_compress's chunks (blosc_b200_grid_bound); 0 on overflow"""
+    sh, cs = _grid_shapes(shape, chunkshape)
+    return int(lib.blosc_b200_grid_bound(sh.size, sh.ctypes.data, cs.ctypes.data, itemsize))
+
+
+def grid_compress(src, shape, chunkshape, itemsize, clevel, doshuffle, compressor, dest, destsize=None, typesize=None,
+                  blocksize=0, fill=None, skip_fill=False, numinternalthreads=1):
+    """The C-order array `src` of `shape` (itemsize-byte items; a numpy array or a torch tensor, host or CUDA) written
+    as the regular grid of Blosc-1 chunks that grid_getslice reads (zarr v2, HDF5 blosc; blosc_b200_grid_compress): each
+    chunk is compress_ctx of its sub-array at full chunk shape, edge padding `fill` (as in grid_getslice; None: zeros),
+    header typesize `typesize` (default itemsize).  The chunks go back to back into `dest` (host or CUDA; destsize
+    default: all of it) in grid C order.  skip_fill: a chunk that holds only `fill` is not written.  Returns (nbytes,
+    offsets): the bytes written, or 0 when they do not fit, or a negative code, and the nchunks + 1 int64 offsets of the
+    chunks in dest (grid_chunks cuts them out)."""
+    import numpy as np
+    sh, cs = _grid_shapes(shape, chunkshape)
+    nchunks = 1
+    if (cs >= 1).all() and (sh >= 0).all():               # else the library rejects the geometry
+        for s, c in zip(sh.tolist(), cs.tolist()):
+            nchunks *= -(-s // c)
+    offsets = np.zeros(nchunks + 1, np.int64)
+    f = _fill(fill, itemsize)
+    n = lib.blosc_b200_grid_compress(clevel, doshuffle, itemsize if typesize is None else typesize, _name(compressor),
+                                     blocksize, numinternalthreads, sh.size, sh.ctypes.data, cs.ctypes.data, itemsize,
+                                     _ptr(src), None if f is None else f.ctypes.data, int(bool(skip_fill)), _ptr(dest),
+                                     _nbytes(dest) if destsize is None else destsize, offsets.ctypes.data)
+    return int(n), offsets
+
+
+def grid_chunks(dest, offsets):
+    """The chunks grid_compress wrote into `dest`, in grid C order, as views of it (None for a chunk skip_fill left
+    out), ready to pass as grid_getslice's `chunks`"""
+    d = dest.reshape(-1)
+    if hasattr(d, "untyped_storage"):
+        import torch
+        d = d.view(torch.uint8)
+    elif hasattr(d, "view"):
+        import numpy as np
+        d = d.view(np.uint8)
+    o = [int(x) for x in offsets]
+    return [d[a:b] if b > a else None for a, b in zip(o[:-1], o[1:])]
+
+
 def grid_getslice(chunks, shape, chunkshape, itemsize, start, stop, dest, step=None, fill=None):
     """A box, with steps, of the C-order array of `shape` stored as a regular grid of chunks (zarr v2, HDF5 blosc,
     PyTables; blosc_b200_grid_getslice): `chunks` lists the ceil(shape[k] / chunkshape[k]) chunks per dimension in C
@@ -241,12 +316,7 @@ def grid_getslice(chunks, shape, chunkshape, itemsize, start, stop, dest, step=N
         if len(chunks) != nchunks:
             raise ValueError(f"{len(chunks)} chunks, but the grid has {nchunks}")
     table = (C.c_void_p * max(len(chunks), 1))(*[_ptr(c) for c in chunks])
-    f = None
-    if fill is not None:
-        f = np.frombuffer(bytes(fill), np.uint8) if isinstance(fill, (bytes, bytearray)) else \
-            np.ascontiguousarray(fill).reshape(-1).view(np.uint8)
-        if f.size != itemsize:
-            raise ValueError(f"fill has {f.size} bytes, not the itemsize {itemsize}")
+    f = _fill(fill, itemsize)
     t = None if step is None else _step(sh, step)
     return int(lib.blosc_b200_grid_getslice(sh.size, sh.ctypes.data, cs.ctypes.data, itemsize, table,
                                             None if f is None else f.ctypes.data, st.ctypes.data, sp.ctypes.data,

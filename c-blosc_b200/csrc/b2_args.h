@@ -34,7 +34,9 @@ typedef struct StreamMap {
 
 /* the per-workspace int32 words behind `result` / `queue` / `done` / `status` (zero between calls: the
  * last warp of every encode / decode launch puts the counters back) */
-enum { B2_R_CBYTES = 0, B2_R_FITS = 1, B2_R_STATUS = 2, B2_R_QUEUE = 3, B2_R_DONE = 4, B2_R_STATUS_OUT = 5, B2_R_WORDS = 16 };
+enum { B2_R_CBYTES = 0, B2_R_FITS = 1, B2_R_STATUS = 2, B2_R_QUEUE = 3, B2_R_DONE = 4, B2_R_STATUS_OUT = 5,
+       B2_R_DIFF = 6,      /* grid_pack_kernel: some packed byte differs from the fill pattern (cleared before use) */
+       B2_R_WORDS = 16 };
 #define B2_FOLD_SCAN_MAX_BLOCKS 65536   /* above this the 1024-thread scan_kernel is launched instead of the in-kernel scan */
 
 typedef struct ScanArgs {
@@ -580,6 +582,24 @@ typedef struct PlacedGatherArgs {
   uint8_t* dst;
   const int* status;
 } PlacedGatherArgs;
+
+/* One chunk of a chunk grid being written (blosc_b200_grid_compress): its sub-array as two step-1 boxes with the same
+ * extents, `box` in the array's coordinates and `out` in the chunk's, as in PlacedGatherArgs with the roles swapped.
+ * grid_pack_kernel copies run q of `run` items from box's unrank of q * run in `src` (the whole array, which may be far
+ * larger than 4 GiB: 64-bit offsets) to out's unrank of q * run in `dst` (the chunk's input, below 2^31 bytes).  `diff`
+ * NULL: a plain copy.  Otherwise a lane that stores a byte other than the itemsize-byte pattern `fill` (NULL: zeros)
+ * sets *diff to 1. */
+typedef struct GridPackArgs {
+  B2Box box;
+  B2Box out;
+  long long run;
+  long long total;            /* bytes of the part: box.count * itemsize */
+  long long itemsize;
+  const uint8_t* src;
+  const uint8_t* fill;        /* device memory */
+  uint8_t* dst;
+  int* diff;
+} GridPackArgs;
 
 #ifdef __cplusplus
 }

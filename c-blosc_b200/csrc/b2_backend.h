@@ -72,6 +72,7 @@ int  b2_launch_oindex_plan(const OIndexPlanArgs* a, b2_stream_t s);    /* oindex
 int  b2_launch_oindex_gather(const OIndexGatherArgs* a, b2_stream_t s);   /* oindex_gather_kernel (getoindex) */
 int  b2_launch_placed_gather(const PlacedGatherArgs* a, b2_stream_t s);   /* placed_gather_kernel (grid_getslice) */
 int  b2_launch_placed_fill(const PlacedGatherArgs* a, b2_stream_t s);     /* placed_fill_kernel (grid_getslice) */
+int  b2_launch_grid_pack(const GridPackArgs* a, b2_stream_t s);          /* grid_pack_kernel (grid_compress) */
 
 /* profiling: per-kernel-kind CUDA-event timing (off by default) */
 enum { B2_K_FILTER = 0, B2_K_ENCODE, B2_K_SCAN, B2_K_COMPACT, B2_K_DECODE, B2_K_UNFILTER, B2_K_INDEX, B2_K_PARSE, B2_K_ZENC, B2_K_DENC, B2_K_SENC, B2_K_GATHER, B2_K_PLAN, B2_K_COUNT };

@@ -551,3 +551,13 @@ extern "C" int b2_launch_placed_fill(const PlacedGatherArgs* a, b2_stream_t s) {
   CK(cudaGetLastError());
   return 0;
 }
+
+/* the pack of grid_compress, with or without the fill compare, counted as a gather launch */
+extern "C" int b2_launch_grid_pack(const GridPackArgs* a, b2_stream_t s) {
+  if (a->total <= 0) return 0;
+  ProfScope ps(B2_K_GATHER, s->s);
+  if (a->diff) grid_pack_kernel<true><<<gather_ctas(a->total), GATHER_WARPS * 32, 0, s->s>>>(*a);
+  else grid_pack_kernel<false><<<gather_ctas(a->total), GATHER_WARPS * 32, 0, s->s>>>(*a);
+  CK(cudaGetLastError());
+  return 0;
+}

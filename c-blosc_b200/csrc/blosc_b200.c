@@ -610,12 +610,51 @@ static int emit_memcpyed(const uint8_t* hdr, const void* src, int src_dev, void*
   return nbytes + 16;
 }
 
+/* header + raw payload from device memory, inside a held workspace (no second one is taken) */
+static int emit_memcpyed_ws(b2_ws* w, const uint8_t* hdr, const void* d_src, void* dest, int dest_dev, int32_t nbytes) {
+  if (copy_any(dest, dest_dev, hdr, 0, 16, w->stream)) return -1;
+  if (dest_dev ? copy_any((uint8_t*)dest + 16, 1, d_src, 1, (size_t)nbytes, w->stream)
+               : d2h_any(w, (uint8_t*)dest + 16, d_src, (size_t)nbytes))
+    return -1;
+  return nbytes + 16;
+}
+
+/* A chunk of a grid being written (blosc_b200_grid_compress) whose input compress_impl packs out of a device array into
+ * its own workspace: `pack` (dst and diff unset) and, for an edge chunk, `pad` (total > 0; dst unset), the fill over the
+ * whole chunk that goes first.  skip: the pack compares with the fill pattern, and a chunk that holds nothing else is
+ * `skipped`, with nothing written. */
+typedef struct {
+  GridPackArgs pack;
+  PlacedGatherArgs pad;
+  int skip, skipped;
+} b2_pack;
+
+/* The chunk's input made in w->in (room for it ensured) on w's stream; with skip, one read-back and sync of the
+ * compare flag */
+static int grid_pack(b2_ws* w, b2_pack* pk) {
+  pk->pack.dst = (uint8_t*)w->in.p;
+  pk->pack.diff = pk->skip ? w->d_result + B2_R_DIFF : NULL;
+  if (pk->pad.total > 0) {
+    pk->pad.dst = (uint8_t*)w->in.p;
+    if (b2_launch_placed_fill(&pk->pad, w->stream)) return -1;
+  }
+  if (pk->skip && b2_memset_dev(pk->pack.diff, 0, 4, w->stream)) return -1;
+  if (b2_launch_grid_pack(&pk->pack, w->stream)) return -1;
+  if (pk->skip) {
+    if (b2_copy_d2h(w->h_result + B2_R_DIFF, pk->pack.diff, 4, w->stream) || b2_stream_sync(w->stream)) return -1;
+    pk->skipped = !w->h_result[B2_R_DIFF];
+  }
+  return 0;
+}
+
 /* ------------------------------------------------------------------------- */
 /* compression                                                                */
 /* ------------------------------------------------------------------------- */
+/* pk NULL: the input is `src`.  Otherwise the input is packed into the workspace (grid_pack) and src is unused; every
+ * exit, the MEMCPYED ones included, is then served from the packed bytes while the workspace is held. */
 static int compress_impl(int clevel, int doshuffle, size_t typesize, size_t nbytes, const void* src, void* dest,
                          size_t destsize, const char* compressor, size_t blocksize, int numinternalthreads,
-                         b2_place* pl, int pl_dest_dev) {
+                         b2_place* pl, int pl_dest_dev, b2_pack* pk) {
   const int compcode = blosc_compname_to_compcode(compressor);
   int32_t ts, nb, bs, nblocks, leftover, dsz;
   int flags = 0, compformat, dont_split, src_dev, dest_dev, dofilter, fmode = 0, nsplits, result = -1, launched = 0;
@@ -658,13 +697,13 @@ static int compress_impl(int clevel, int doshuffle, size_t typesize, size_t nbyt
   flags |= dont_split << 4;
   flags |= compformat << 5;
 
-  src_dev = (nb > 0) ? b2_ptr_is_device(src) : 0;
+  src_dev = pk ? 1 : (nb > 0) ? b2_ptr_is_device(src) : 0;
   dest_dev = pl ? pl_dest_dev : b2_ptr_is_device(dest);
 
   /* blosc_compress_context, blosc.c:1250-1279 */
   if ((flags & BLOSC_MEMCPYED) && nb + BLOSC_MAX_OVERHEAD > dsz) return 0;
   if (check_threads(numinternalthreads, nb, bs) < 0) return -1;
-  if (flags & BLOSC_MEMCPYED) {
+  if ((flags & BLOSC_MEMCPYED) && !pk) {
     make_header(hdr, 1, flags, ts, nb, bs, nb + 16);
     if (pl && !(dest = frame_place(pl, nb + 16))) return 0;
     return emit_memcpyed(hdr, src, src_dev, dest, dest_dev, nb);
@@ -678,6 +717,13 @@ static int compress_impl(int clevel, int doshuffle, size_t typesize, size_t nbyt
     ScanArgs sa;
     CompactArgs ca;
     const int32_t nfull = nb / bs;
+    if (pk) {                                  /* the input packed in place of the staging copy below */
+      launched = 1;
+      if (buf_ensure(&w->in, (size_t)nb + 64) || grid_pack(w, pk)) break;
+      src = w->in.p;
+      if (pk->skipped) { result = 0; break; }
+      if (flags & BLOSC_MEMCPYED) { result = -2; break; }
+    }
     /* stage the input on the device if it lives in host memory */
     if (src_dev) d_src = (const uint8_t*)src;
     else {
@@ -769,6 +815,7 @@ static int compress_impl(int clevel, int doshuffle, size_t typesize, size_t nbyt
         /* the records need 256 bytes per segment; whichever of the staging / filter buffers does not hold the
          * codec input is free for them */
         b2_buf* recs = d_codec_in == (const uint8_t*)w->in.p ? &w->filt : &w->in;
+        if (recs == &w->in && pk) recs = &w->plan;         /* w->in holds the packed input the redo below reads */
         if (buf_ensure(recs, (size_t)nsegs * B2_FAST_SEG + 64)) break;
         if (buf_ensure(&w->segs, (size_t)nsegs * 4 + 64)) break;
         fx.recs = (uint32_t*)recs->p; fx.nrec = (uint32_t*)w->segs.p;
@@ -805,6 +852,11 @@ static int compress_impl(int clevel, int doshuffle, size_t typesize, size_t nbyt
     }
   } while (0);
   if (result == -1 && launched) ws_reset_counters(w);                      /* a failed call must not leave the counters dirty */
+  if (result == -2 && pk) {                  /* MEMCPYED, from the packed bytes before another call may reuse w->in */
+    flags |= BLOSC_MEMCPYED;
+    make_header(hdr, 1, flags, ts, nb, bs, nb + 16);
+    result = pl && !(dest = frame_place(pl, nb + 16)) ? 0 : emit_memcpyed_ws(w, hdr, w->in.p, dest, dest_dev, nb);
+  }
   ws_release(w);
   if (result == -2) {
     flags |= BLOSC_MEMCPYED;
@@ -818,7 +870,7 @@ static int compress_impl(int clevel, int doshuffle, size_t typesize, size_t nbyt
 int blosc_compress_ctx(int clevel, int doshuffle, size_t typesize, size_t nbytes, const void* src, void* dest,
                        size_t destsize, const char* compressor, size_t blocksize, int numinternalthreads) {
   return compress_impl(clevel, doshuffle, typesize, nbytes, src, dest, destsize, compressor, blocksize,
-                       numinternalthreads, NULL, 0);
+                       numinternalthreads, NULL, 0, NULL);
 }
 
 /* ------------------------------------------------------------------------- */
@@ -1925,6 +1977,11 @@ struct b2_frame_job {
   uint64_t* offsets;
   /* decompression */
   const uint8_t* frame;
+  /* a chunk grid (blosc_b200_grid_compress): src is the array */
+  int ndim, src_dev, skip_fill;
+  long long itemsize, nitems, chunk_items;
+  int64_t shape[B2_BOX_MAXDIM], chunkshape[B2_BOX_MAXDIM];
+  const uint8_t* fill;      /* the fill pattern where the pack reads it (device memory for a device src); NULL: zeros */
 };
 
 static void wr_u64(uint8_t* p, uint64_t v) { int i; for (i = 0; i < 8; i++) p[i] = (uint8_t)(v >> (8 * i)); }
@@ -1987,7 +2044,7 @@ static void* frame_compress_worker(void* arg) {
     pl.job = j; pl.index = i; pl.placed = 0; pl.many = j->workers > 1;
     if (!failed)
       rc = compress_impl(j->clevel, j->doshuffle, j->typesize, n, j->src + off, NULL, n + BLOSC_MAX_OVERHEAD,
-                         j->compressor, j->blocksize, j->nthreads, &pl, j->dest_dev);
+                         j->compressor, j->blocksize, j->nthreads, &pl, j->dest_dev, NULL);
     if (!pl.placed) frame_place(&pl, -1);
     if (rc <= 0 && !failed) frame_fail(j, rc);
   }
@@ -2858,6 +2915,194 @@ long long blosc_b200_grid_getslice(int ndim, const int64_t* shape, const int64_t
   for (k = 0; k < ndim; k++) free(j.list[k]);
   free(j.src); free(j.src_dev);
   return result;
+}
+
+/* ------------------------------------------------------------------------- */
+/* writing arrays as a grid of chunks (blosc_b200_grid_compress)              */
+/* ------------------------------------------------------------------------- */
+/* The write side of the grid above: every chunk of the array's grid is compressed by the frame's machinery -- workers
+ * from BLOSC_B200_FRAME_WORKERS take chunks in order, each through compress_impl on its own workspace and stream, and
+ * frame_place lays them out back to back in grid C order whatever the worker count.  A chunk's input is its sub-array
+ * at full chunk shape: two step-1 boxes with the same extents, one in the array's coordinates and one in the chunk's.
+ * From a device array, compress_impl packs it into its workspace with grid_pack_kernel (after one placed_fill_kernel
+ * over an edge chunk), so the array is never copied whole; from a host array, the worker gathers it run by run into
+ * a pinned buffer of its own, which compress_impl stages as any host input. */
+
+size_t blosc_b200_grid_bound(int ndim, const int64_t* shape, const int64_t* chunkshape, size_t itemsize) {
+  size_t n = 1, items = 1;
+  int k;
+  if (ndim < 1 || ndim > B2_BOX_MAXDIM || itemsize < 1) return 0;
+  for (k = 0; k < ndim; k++) {
+    size_t g;
+    if (shape[k] < 0 || chunkshape[k] < 1) return 0;
+    g = (size_t)(shape[k] / chunkshape[k] + (shape[k] % chunkshape[k] != 0));
+    if ((g && n > SIZE_MAX / g) || items > SIZE_MAX / (size_t)chunkshape[k]) return 0;
+    n *= g;
+    items *= (size_t)chunkshape[k];
+  }
+  if (items > (SIZE_MAX - BLOSC_MAX_OVERHEAD) / itemsize) return 0;
+  items = items * itemsize + BLOSC_MAX_OVERHEAD;
+  return n && items > SIZE_MAX / n ? 0 : n * items;
+}
+
+/* Chunk g of the grid: its sub-array as the box in the array's coordinates and the box in the chunk's.  Returns 1 for
+ * an edge chunk, which holds padding. */
+static int grid_chunk_boxes(const b2_frame_job* j, long long g, B2Box* box, B2Box* out) {
+  int64_t org[B2_BOX_MAXDIM], lim[B2_BOX_MAXDIM], ext[B2_BOX_MAXDIM];
+  int k, edge = 0;
+  for (k = j->ndim - 1; k >= 0; k--) {
+    const long long cs = j->chunkshape[k], n = (j->shape[k] - 1) / cs + 1;
+    org[k] = g % n * cs;
+    lim[k] = cs < j->shape[k] - org[k] ? org[k] + cs : j->shape[k];
+    ext[k] = lim[k] - org[k];
+    edge |= ext[k] < cs;
+    g /= n;
+  }
+  box_build(j->ndim, j->shape, org, lim, NULL, j->nitems, box);
+  box_build(j->ndim, j->chunkshape, g_box_origin, ext, NULL, j->chunk_items, out);
+  return edge;
+}
+
+/* n bytes of whole items, each the itemsize-byte pattern fill (NULL: zeros) */
+static void pattern_fill(uint8_t* p, size_t n, const uint8_t* fill, size_t ts) {
+  size_t have = ts < n ? ts : n;
+  if (!fill) { memset(p, 0, n); return; }
+  memcpy(p, fill, have);
+  for (; have < n; have *= 2) memcpy(p + have, p, have < n - have ? have : n - have);
+}
+
+/* n bytes of whole items all equal to the pattern fill (NULL: zeros) */
+static int pattern_equal(const uint8_t* p, size_t n, const uint8_t* fill, size_t ts) {
+  size_t x;
+  uint8_t d = 0;
+  if (!fill) { for (x = 0; x < n; x++) d |= p[x]; return d == 0; }
+  for (x = 0; x < n; x += ts) if (memcmp(p + x, fill, ts)) return 0;
+  return 1;
+}
+
+/* A host array: chunk a's sub-array gathered run by run into `host`, over the fill pattern in an edge chunk.  Returns
+ * 1 when skip_fill is asked and every gathered byte is the fill pattern (the chunk is then not written), else 0. */
+static int grid_gather_host(const b2_frame_job* j, const GridPackArgs* a, int edge, uint8_t* host) {
+  const long long ts = j->itemsize, runb = a->run * ts;
+  long long q;
+  int same = j->skip_fill;
+  if (edge) pattern_fill(host, (size_t)(j->chunk_items * ts), j->fill, (size_t)ts);
+  for (q = 0; q < a->box.count; q += a->run) {
+    const uint8_t* from = j->src + b2_box_unrank(&a->box, q, 0) * ts;
+    memcpy(host + b2_box_unrank(&a->out, q, 0) * ts, from, (size_t)runb);
+    if (same) same = pattern_equal(from, (size_t)runb, j->fill, (size_t)ts);
+  }
+  return same;
+}
+
+static void* grid_compress_worker(void* arg) {
+  b2_frame_job* j = (b2_frame_job*)arg;
+  const long long cb = j->chunk_items * j->itemsize;
+  const int64_t items = j->chunk_items;
+  B2Box whole;                               /* the whole chunk, which an edge chunk's fill covers */
+  uint8_t* host = NULL;
+  int i, failed;
+  b2_set_device(j->dev);
+  box_build(1, &items, g_box_origin, &items, NULL, items, &whole);
+  if (!j->src_dev) {
+    void* p = NULL;
+    if (b2_pinned_alloc(&p, (size_t)cb) == 0) host = (uint8_t*)p;
+  }
+  while ((i = frame_take(j, &failed)) >= 0) {
+    b2_place pl;
+    b2_pack pk;
+    int rc = -1, edge;
+    pl.job = j; pl.index = i; pl.placed = 0; pl.many = j->workers > 1;
+    memset(&pk, 0, sizeof pk);
+    if (!failed && (j->src_dev || host)) {
+      edge = grid_chunk_boxes(j, i, &pk.pack.box, &pk.pack.out);
+      pk.pack.run = pk.pack.box.run < pk.pack.out.run ? pk.pack.box.run : pk.pack.out.run;
+      pk.pack.total = pk.pack.box.count * j->itemsize; pk.pack.itemsize = j->itemsize;
+      pk.pack.src = j->src; pk.pack.fill = j->fill;
+      pk.skip = j->skip_fill;
+      if (j->src_dev) {
+        if (edge) {
+          pk.pad.out = whole; pk.pad.run = whole.run; pk.pad.total = cb; pk.pad.itemsize = j->itemsize;
+          pk.pad.fill = j->fill;
+        }
+        rc = compress_impl(j->clevel, j->doshuffle, j->typesize, (size_t)cb, NULL, NULL, (size_t)cb + BLOSC_MAX_OVERHEAD,
+                           j->compressor, j->blocksize, j->nthreads, &pl, j->dest_dev, &pk);
+      } else if (!(pk.skipped = grid_gather_host(j, &pk.pack, edge, host)))
+        rc = compress_impl(j->clevel, j->doshuffle, j->typesize, (size_t)cb, host, NULL, (size_t)cb + BLOSC_MAX_OVERHEAD,
+                           j->compressor, j->blocksize, j->nthreads, &pl, j->dest_dev, NULL);
+      if (pk.skipped) {                      /* its turn in the ordered commit, with no bytes: not "does not fit" */
+        frame_place(&pl, 0);
+        rc = 1;
+      }
+    }
+    if (!pl.placed) frame_place(&pl, -1);
+    if (rc <= 0 && !failed) frame_fail(j, rc);
+  }
+  if (host) b2_pinned_free(host);
+  return NULL;
+}
+
+long long blosc_b200_grid_compress(int clevel, int doshuffle, size_t typesize, const char* compressor, size_t blocksize,
+                                   int numinternalthreads, int ndim, const int64_t* shape, const int64_t* chunkshape,
+                                   size_t itemsize, const void* src, const void* fill, int skip_fill, void* dest,
+                                   size_t destsize, int64_t* offsets) {
+  b2_frame_job j;
+  void* d_fill = NULL;
+  long long chunk_items = 0, nchunks = 1, nitems = 1;
+  int k, rc, src_dev, dest_dev, dev, old_dev;
+  if (clevel < 0 || clevel > 9) return -10;                       /* the chunk API's codes */
+  if (doshuffle != 0 && doshuffle != 1 && doshuffle != 2) return -10;
+  if (typesize == 0) return -10;
+  if (!compressor || blosc_compname_to_compcode(compressor) < 0) return -5;
+  if (grid_geometry(ndim, shape, chunkshape, itemsize, g_box_origin, shape, NULL, &chunk_items)) return -1;
+  for (k = 0; k < ndim; k++) {
+    const long long g = shape[k] / chunkshape[k] + (shape[k] % chunkshape[k] != 0);
+    nitems *= shape[k];                                           /* box_geometry checked the product */
+    if (g == 0) nchunks = 0;
+    else if (nchunks > 0) nchunks = nchunks > (INT_MAX / 2) / g ? (long long)INT_MAX : nchunks * g;
+  }
+  if (nchunks > INT_MAX / 2) {
+    fprintf(stderr, "blosc_b200: the grid has more than %d chunks\n", INT_MAX / 2);
+    return -1;
+  }
+  if (nchunks == 0) {
+    if (offsets) offsets[0] = 0;
+    return 0;
+  }
+  if (!src || !offsets) { fprintf(stderr, "blosc_b200: %s is NULL\n", src ? "offsets" : "src"); return -1; }
+  /* the call runs on dest's device when dest is device memory, else on src's, else on the current one */
+  src_dev = b2_ptr_is_device(src);
+  dest_dev = b2_ptr_is_device(dest);
+  dev = dest_dev ? b2_ptr_device(dest) : src_dev ? b2_ptr_device(src) : b2_get_device();
+  if (src_dev && b2_ptr_device(src) != dev) {
+    fprintf(stderr, "blosc_b200: src is on device %d, not on device %d where the call runs\n", b2_ptr_device(src), dev);
+    return -1;
+  }
+  if (!backend_ready()) return -1;
+  old_dev = b2_get_device();
+  if (dev != old_dev && b2_set_device(dev)) return -1;
+  memset(&j, 0, sizeof j);
+  j.nchunks = (int)nchunks; j.workers = frame_workers((int)nchunks); j.dest_dev = dest_dev;
+  j.clevel = clevel; j.doshuffle = doshuffle; j.nthreads = numinternalthreads;
+  j.typesize = typesize; j.blocksize = blocksize; j.compressor = compressor;
+  j.destsize = destsize; j.cursor = 0; j.src = (const uint8_t*)src; j.dest = (uint8_t*)dest;
+  j.offsets = (uint64_t*)offsets;
+  j.ndim = ndim; j.src_dev = src_dev; j.skip_fill = skip_fill != 0;
+  j.itemsize = (long long)itemsize; j.nitems = nitems; j.chunk_items = chunk_items;
+  for (k = 0; k < ndim; k++) { j.shape[k] = shape[k]; j.chunkshape[k] = chunkshape[k]; }
+  j.fill = (const uint8_t*)fill;
+  rc = 0;
+  if (src_dev && fill) {                     /* the pack reads the pattern on the device */
+    if (b2_dev_alloc(&d_fill, itemsize) || copy_some(d_fill, 1, fill, 0, itemsize)) rc = -1;
+    j.fill = (const uint8_t*)d_fill;
+  }
+  if (rc == 0) rc = frame_run(&j, grid_compress_worker);
+  else j.err = -1;
+  if (d_fill) b2_dev_free(d_fill);
+  if (dev != old_dev) b2_set_device(old_dev);
+  if (rc) return j.err ? j.err : (j.failed ? 0 : -1);            /* 0: does not fit in destsize, as frame_compress */
+  offsets[nchunks] = (int64_t)j.cursor;
+  return (long long)j.cursor;
 }
 
 /* ------------------------------------------------------------------------- */

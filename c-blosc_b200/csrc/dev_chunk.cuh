@@ -29,6 +29,9 @@
  *                   one chunk's part of a box of an array stored as a grid of chunks
  *                   (blosc_b200_grid_getslice), written straight into its place in the output,
  *                   or the fill value over the part of a missing chunk
+ *   grid_pack_kernel
+ *                   one chunk's sub-array packed out of an N-d array into the chunk's input
+ *                   (blosc_b200_grid_compress), compared with the fill value on request
  */
 #pragma once
 #include "b2_args.h"
@@ -1579,6 +1582,76 @@ __global__ void __launch_bounds__(GATHER_WARPS * 32) placed_fill_kernel(PlacedGa
   }
 }
 
+/* warp_copy_vec that also compares: byte x of the piece is held against byte (u0 + x) % ts of the pattern `fill`
+ * (zeros when NULL).  Returns nonzero in a lane that copied a byte other than the pattern's. */
+DEV unsigned warp_copy_cmp(u8* __restrict__ dst, const u8* __restrict__ src, int n, const u8* fill, unsigned ts,
+                           unsigned u0) {
+  const int lane = lane_id();
+  unsigned d = 0;
+  int i = lane;
+  if ((((uintptr_t)dst ^ (uintptr_t)src) & 15u) == 0 && n >= 32) {
+    const int head = (int)((16u - ((uintptr_t)dst & 15u)) & 15u);
+    const int nv = (n - head) >> 4;
+    const uint4* s4 = (const uint4*)(src + head);
+    uint4* d4 = (uint4*)(dst + head);
+    if (lane < head) { const u8 v = src[lane]; dst[lane] = v; d |= v ^ (fill ? fill[(u0 + lane) % ts] : 0); }
+    for (int q = lane; q < nv; q += 32) {
+      const uint4 v = s4[q];
+      d4[q] = v;
+      if (!fill) d |= v.x | v.y | v.z | v.w;
+      else {
+        const unsigned w[4] = {v.x, v.y, v.z, v.w}, at = u0 + (unsigned)head + 16u * (unsigned)q;
+#pragma unroll
+        for (int b = 0; b < 16; b++) d |= ((w[b >> 2] >> (8 * (b & 3))) & 0xffu) ^ fill[(at + b) % ts];
+      }
+    }
+    i = head + (nv << 4) + lane;
+  }
+  for (; i < n; i += 32) { const u8 v = src[i]; dst[i] = v; d |= v ^ (fill ? fill[(u0 + i) % ts] : 0); }
+  return d;
+}
+
+/* blosc_b200_grid_compress: one chunk's sub-array packed out of the array into the chunk's input (GridPackArgs).  The
+ * walk is placed_gather_kernel's over the part's bytes [0, total), with the run's source the array box's unrank and its
+ * destination the chunk box's; both boxes have step 1.  Source offsets are 64-bit: the array may exceed 4 GiB.  CMP =
+ * a.diff != NULL: each lane compares the bytes it stores with the fill pattern and sets *diff once at the end; without
+ * it the kernel only copies.  A kernel of its own, so that the placed kernels keep their code and registers. */
+template <bool CMP>
+__global__ void __launch_bounds__(GATHER_WARPS * 32) grid_pack_kernel(GridPackArgs a) {
+  const long long ts = a.itemsize, runb = a.run * ts;
+  const unsigned its = (unsigned)a.itemsize;              /* a chunk's bytes are below 2^31 */
+  const int lane = lane_id();
+  const long long warps = (long long)gridDim.x * GATHER_WARPS;
+  unsigned d = 0;
+  for (long long lo = ((long long)blockIdx.x * GATHER_WARPS + (threadIdx.x >> 5)) * GATHER_SPAN; lo < a.total;
+       lo += warps * GATHER_SPAN) {
+    const long long hi = lo + GATHER_SPAN < a.total ? lo + GATHER_SPAN : a.total;
+    if (runb >= BOX_SHORT_RUN) {
+      for (long long o = lo; o < hi;) {
+        const long long k = b2_box_div(o, runb), u = o - k * runb;
+        const u8* from = a.src + b2_box_unrank(&a.box, k * a.run, 0) * ts + u;
+        u8* out = a.dst + b2_box_unrank(&a.out, k * a.run, 0) * ts + u;
+        const int n = (int)(runb - u < hi - o ? runb - u : hi - o);
+        if (CMP) d |= warp_copy_cmp(out, from, n, a.fill, its, (unsigned)u);
+        else warp_copy_vec(out, from, n);
+        o += n;
+      }
+    } else {
+      const long long ka = b2_box_div(lo + runb - 1, runb), kb = b2_box_div(hi + runb - 1, runb);
+      for (long long k = ka + lane; k < kb; k += 32) {
+        const u8* from = a.src + b2_box_unrank(&a.box, k * a.run, 0) * ts;
+        u8* out = a.dst + b2_box_unrank(&a.out, k * a.run, 0) * ts;
+        for (int x = 0; x < (int)runb; x++) {
+          const u8 v = from[x];
+          out[x] = v;
+          if (CMP) d |= v ^ (a.fill ? a.fill[(unsigned)x % its] : 0);
+        }
+      }
+    }
+  }
+  if (CMP && d) *a.diff = 1;
+}
+
 #ifdef SIMT_EMU
 /* The emulator's launchers of the placed kernels, as those of the box kernels; both count as gather launches */
 static unsigned emu_gather_ctas(long long total) {
@@ -1599,6 +1672,15 @@ extern "C" int b2_launch_placed_fill(const PlacedGatherArgs* a, b2_stream_t) {
   g_emu_gather_launches++;
   PlacedGatherArgs args = *a;
   simt::launch(simt::Dim3(emu_gather_ctas(a->total)), simt::Dim3(GATHER_WARPS * 32), 0, [&] { placed_fill_kernel(args); });
+  return 0;
+}
+extern "C" int b2_launch_grid_pack(const GridPackArgs* a, b2_stream_t) {
+  if (a->total <= 0) return 0;
+  g_emu_gather_launches++;
+  GridPackArgs args = *a;
+  simt::launch(simt::Dim3(emu_gather_ctas(a->total)), simt::Dim3(GATHER_WARPS * 32), 0, [&] {
+    if (args.diff) grid_pack_kernel<true>(args); else grid_pack_kernel<false>(args);
+  });
   return 0;
 }
 #endif

@@ -301,6 +301,35 @@ long long blosc_b200_grid_getslice(int ndim, const int64_t* shape, const int64_t
                                    const void* const* chunks, const void* fill, const int64_t* start,
                                    const int64_t* stop, const int64_t* step, void* dest);
 
+/* The size that always holds blosc_b200_grid_compress's chunks: nchunks * (prod(chunkshape) * itemsize + 16), nchunks =
+ * prod(ceil(shape[k] / chunkshape[k])).  0 when that overflows size_t or the geometry is invalid. */
+size_t    blosc_b200_grid_bound(int ndim, const int64_t* shape, const int64_t* chunkshape, size_t itemsize);
+
+/* Writes the C-order array of `shape` (items of itemsize bytes, src in host or device memory) as the regular grid of
+ * chunks that blosc_b200_grid_getslice reads: grid[k] = ceil(shape[k] / chunkshape[k]) chunks per dimension, chunk g (in
+ * grid C order) holding its sub-array at full chunk shape in C order, with the padding of edge chunks the itemsize-byte
+ * pattern at `fill` (host memory; NULL: zero bytes), as zarr v2 writes it.  Each chunk is byte-identical to
+ * blosc_compress_ctx(clevel, doshuffle, typesize, chunk_bytes, <that padded sub-array>, d, chunk_bytes + 16, compressor,
+ * blocksize, numinternalthreads), chunk_bytes = prod(chunkshape) * itemsize; typesize is the header's and the shuffle's
+ * (above 255: 1), itemsize the geometry's.  The chunks are written back to back into dest (host or device memory) in
+ * grid C order from offset 0, with nothing else; offsets (host memory, nchunks + 1 entries) receives chunk g's place,
+ * dest[offsets[g], offsets[g + 1]).  The layout does not depend on BLOSC_B200_FRAME_WORKERS, the number of chunks
+ * compressed at once (default 4).  A device src is packed chunk by chunk on the device, never copied whole.
+ * skip_fill != 0 (zarr's write_empty_chunks=False): a chunk whose items inside the array all equal the fill pattern is
+ * not written, offsets[g] == offsets[g + 1].  Returns the bytes written, offsets[nchunks]; 0 when the chunks do not fit
+ * in destsize (blosc_b200_grid_bound always fits), and 0 with offsets[0] = 0 for a grid with no chunk (some shape[k] ==
+ * 0); -10 / -5 for a bad clevel, doshuffle or typesize or an unknown compressor, as blosc_compress_ctx.  -1 with a
+ * message on stderr, before anything is launched or read, for ndim outside 1..8, a negative shape, chunkshape[k] < 1,
+ * itemsize < 1, a chunk larger than BLOSC_MAX_BUFFERSIZE bytes, more than INT_MAX / 2 chunks, src or offsets NULL for a
+ * non-empty grid, or a device src on another device than the call's (dest's when dest is device memory, else src's).
+ * A chunk that fails returns its code (-1 or blosc_compress_ctx's); the contents of dest and offsets are then
+ * unspecified. */
+long long blosc_b200_grid_compress(int clevel, int doshuffle, size_t typesize, const char* compressor,
+                                   size_t blocksize, int numinternalthreads,
+                                   int ndim, const int64_t* shape, const int64_t* chunkshape, size_t itemsize,
+                                   const void* src, const void* fill, int skip_fill,
+                                   void* dest, size_t destsize, int64_t* offsets);
+
 /* Select the CUDA device used by the calling thread's subsequent calls with HOST pointers
  * (device pointers carry their device).  Multi-GPU callers run one process (or thread) per GPU. */
 int blosc_b200_set_device(int dev);
