@@ -355,12 +355,32 @@ extern "C" int b2_launch_decode(const DecodeArgs* a, b2_stream_t s) {
   return 0;
 }
 
+/* The grids of the grid-stride kernels: one warp job per GATHER_SPAN bytes (gather kinds) or one thread per item
+ * (per-range checks and touches), at most 8 CTAs per SM */
+static unsigned gather_ctas(long long total) {
+  long long ctas = (total + (long long)GATHER_WARPS * GATHER_SPAN - 1) / ((long long)GATHER_WARPS * GATHER_SPAN);
+  if (ctas > (long long)num_sms() * 8) ctas = (long long)num_sms() * 8;
+  return (unsigned)ctas;
+}
+
+static unsigned range_ctas(long long n) {
+  long long ctas = (n + PLAN_THREADS - 1) / PLAN_THREADS;
+  if (ctas > (long long)num_sms() * 8) ctas = (long long)num_sms() * 8;
+  return (unsigned)ctas;
+}
+
 extern "C" int b2_launch_gather(const GatherArgs* a, b2_stream_t s) {
   if (a->total <= 0) return 0;
-  long long ctas = (a->total + (long long)GATHER_WARPS * GATHER_SPAN - 1) / ((long long)GATHER_WARPS * GATHER_SPAN);
-  if (ctas > (long long)num_sms() * 8) ctas = (long long)num_sms() * 8;
   ProfScope ps(B2_K_GATHER, s->s);
-  gather_kernel<<<(unsigned)ctas, GATHER_WARPS * 32, 0, s->s>>>(*a);
+  gather_kernel<<<gather_ctas(a->total), GATHER_WARPS * 32, 0, s->s>>>(*a);
+  CK(cudaGetLastError());
+  return 0;
+}
+
+/* the PLAN_SLOT scan over a chunk plan's blocks, a plan launch: it numbers and lists the touched blocks */
+static int launch_slot_scan(const PlanArgs& p, b2_stream_t s) {
+  ProfScope ps(B2_K_PLAN, s->s);
+  plan_scan_kernel<PLAN_SLOT><<<(unsigned)((p.nblocks + PLAN_TILE - 1) / PLAN_TILE), PLAN_THREADS, 0, s->s>>>(p, p.nblocks);
   CK(cudaGetLastError());
   return 0;
 }
@@ -369,25 +389,18 @@ extern "C" int b2_launch_gather(const GatherArgs* a, b2_stream_t s) {
 extern "C" int b2_launch_plan(const PlanArgs* a, b2_stream_t s) {
   if (a->nranges <= 0) return 0;
   {
-    long long ctas = ((long long)a->nranges + PLAN_THREADS - 1) / PLAN_THREADS;
-    if (ctas > (long long)num_sms() * 8) ctas = (long long)num_sms() * 8;
     ProfScope ps(B2_K_PLAN, s->s);
-    plan_check_kernel<<<(unsigned)ctas, PLAN_THREADS, 0, s->s>>>(*a);
+    plan_check_kernel<<<range_ctas(a->nranges), PLAN_THREADS, 0, s->s>>>(*a);
     CK(cudaGetLastError());
   }
   if (!a->in_place) {
     const long long nb = a->nblocks;
-    const unsigned tiles = (unsigned)((nb + PLAN_TILE - 1) / PLAN_TILE);
     {
       ProfScope ps(B2_K_PLAN, s->s);
-      plan_scan_kernel<PLAN_COVER><<<tiles, PLAN_THREADS, 0, s->s>>>(*a, nb);
+      plan_scan_kernel<PLAN_COVER><<<(unsigned)((nb + PLAN_TILE - 1) / PLAN_TILE), PLAN_THREADS, 0, s->s>>>(*a, nb);
       CK(cudaGetLastError());
     }
-    {
-      ProfScope ps(B2_K_PLAN, s->s);
-      plan_scan_kernel<PLAN_SLOT><<<tiles, PLAN_THREADS, 0, s->s>>>(*a, nb);
-      CK(cudaGetLastError());
-    }
+    if (launch_slot_scan(*a, s)) return -1;
   }
   const long long nr = a->nranges;
   ProfScope ps(B2_K_PLAN, s->s);
@@ -398,12 +411,6 @@ extern "C" int b2_launch_plan(const PlanArgs* a, b2_stream_t s) {
 
 /* the frame plan, counted as plan launches: the per-range check and the range scan, then the three chunk scans (none
  * for a frame without chunks); the scatter is a launch of its own, made once the host has sized the piece lists */
-static unsigned range_ctas(long long n) {
-  long long ctas = (n + PLAN_THREADS - 1) / PLAN_THREADS;
-  if (ctas > (long long)num_sms() * 8) ctas = (long long)num_sms() * 8;
-  return (unsigned)ctas;
-}
-
 template <int MODE>
 static int launch_fplan_scan(const FramePlanArgs* a, long long n, b2_stream_t s) {
   ProfScope ps(B2_K_PLAN, s->s);
@@ -447,20 +454,15 @@ extern "C" int b2_launch_box_plan(const BoxPlanArgs* a, b2_stream_t s) {
     else box_touch_kernel<false><<<ctas, PLAN_THREADS, 0, s->s>>>(*a);
     CK(cudaGetLastError());
   }
-  ProfScope ps(B2_K_PLAN, s->s);
-  plan_scan_kernel<PLAN_SLOT><<<(unsigned)((nb + PLAN_TILE - 1) / PLAN_TILE), PLAN_THREADS, 0, s->s>>>(a->plan, nb);
-  CK(cudaGetLastError());
-  return 0;
+  return launch_slot_scan(a->plan, s);
 }
 
 /* the box gather of getslice (stepped or not, as the plan), counted as a gather launch */
 extern "C" int b2_launch_box_gather(const BoxGatherArgs* a, b2_stream_t s) {
   if (a->total <= 0) return 0;
-  long long ctas = (a->total + (long long)GATHER_WARPS * GATHER_SPAN - 1) / ((long long)GATHER_WARPS * GATHER_SPAN);
-  if (ctas > (long long)num_sms() * 8) ctas = (long long)num_sms() * 8;
   ProfScope ps(B2_K_GATHER, s->s);
-  if (a->box.stepped) box_gather_kernel<true><<<(unsigned)ctas, GATHER_WARPS * 32, 0, s->s>>>(*a);
-  else box_gather_kernel<false><<<(unsigned)ctas, GATHER_WARPS * 32, 0, s->s>>>(*a);
+  if (a->box.stepped) box_gather_kernel<true><<<gather_ctas(a->total), GATHER_WARPS * 32, 0, s->s>>>(*a);
+  else box_gather_kernel<false><<<gather_ctas(a->total), GATHER_WARPS * 32, 0, s->s>>>(*a);
   CK(cudaGetLastError());
   return 0;
 }
@@ -484,18 +486,13 @@ extern "C" int b2_launch_boxes_plan(const BoxesPlanArgs* a, b2_stream_t s) {
     boxes_touch_kernel<<<range_ctas(a->nboxes * a->per_box), PLAN_THREADS, 0, s->s>>>(*a);
     CK(cudaGetLastError());
   }
-  ProfScope ps(B2_K_PLAN, s->s);
-  plan_scan_kernel<PLAN_SLOT><<<(unsigned)((nb + PLAN_TILE - 1) / PLAN_TILE), PLAN_THREADS, 0, s->s>>>(a->plan, nb);
-  CK(cudaGetLastError());
-  return 0;
+  return launch_slot_scan(a->plan, s);
 }
 
 extern "C" int b2_launch_boxes_gather(const BoxesGatherArgs* a, b2_stream_t s) {
   if (a->total <= 0) return 0;
-  long long ctas = (a->total + (long long)GATHER_WARPS * GATHER_SPAN - 1) / ((long long)GATHER_WARPS * GATHER_SPAN);
-  if (ctas > (long long)num_sms() * 8) ctas = (long long)num_sms() * 8;
   ProfScope ps(B2_K_GATHER, s->s);
-  boxes_gather_kernel<<<(unsigned)ctas, GATHER_WARPS * 32, 0, s->s>>>(*a);
+  boxes_gather_kernel<<<gather_ctas(a->total), GATHER_WARPS * 32, 0, s->s>>>(*a);
   CK(cudaGetLastError());
   return 0;
 }
@@ -511,30 +508,19 @@ extern "C" int b2_launch_oindex_plan(const OIndexPlanArgs* a, b2_stream_t s) {
     CK(cudaGetLastError());
   }
   if (a->touched || a->r1 <= a->r0 || nb <= 0) return 0;
-  ProfScope ps(B2_K_PLAN, s->s);
-  plan_scan_kernel<PLAN_SLOT><<<(unsigned)((nb + PLAN_TILE - 1) / PLAN_TILE), PLAN_THREADS, 0, s->s>>>(a->plan, nb);
-  CK(cudaGetLastError());
-  return 0;
+  return launch_slot_scan(a->plan, s);
 }
 
 extern "C" int b2_launch_oindex_gather(const OIndexGatherArgs* a, b2_stream_t s) {
   const long long total = a->g1 - a->g0;
   if (total <= 0) return 0;
-  long long ctas = (total + (long long)GATHER_WARPS * GATHER_SPAN - 1) / ((long long)GATHER_WARPS * GATHER_SPAN);
-  if (ctas > (long long)num_sms() * 8) ctas = (long long)num_sms() * 8;
   ProfScope ps(B2_K_GATHER, s->s);
-  oindex_gather_kernel<<<(unsigned)ctas, GATHER_WARPS * 32, 0, s->s>>>(*a);
+  oindex_gather_kernel<<<gather_ctas(total), GATHER_WARPS * 32, 0, s->s>>>(*a);
   CK(cudaGetLastError());
   return 0;
 }
 
 /* the placed gather and fill of grid_getslice (stepped or not, as the chunk's box), counted as gather launches */
-static unsigned gather_ctas(long long total) {
-  long long ctas = (total + (long long)GATHER_WARPS * GATHER_SPAN - 1) / ((long long)GATHER_WARPS * GATHER_SPAN);
-  if (ctas > (long long)num_sms() * 8) ctas = (long long)num_sms() * 8;
-  return (unsigned)ctas;
-}
-
 extern "C" int b2_launch_placed_gather(const PlacedGatherArgs* a, b2_stream_t s) {
   if (a->total <= 0) return 0;
   ProfScope ps(B2_K_GATHER, s->s);

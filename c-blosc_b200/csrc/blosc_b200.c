@@ -2205,6 +2205,39 @@ static int frame_chunk_header(b2_ws* w, const void* frame, const b2_frame* f, si
   return (size_t)h->typesize != f->typesize;
 }
 
+/* frame_open_items for an N-d read of the frame's nitems items: 0, or -1 with a message when chunk 0's typesize does
+ * not divide the chunksize or nitems of it are not the frame's bytes; f->off is freed on a failure. */
+static int frame_open_nd(const void* frame, size_t framesize, long long nitems, b2_frame* f) {
+  const int rc = frame_open_items(frame, framesize, f);
+  if (rc == -2)
+    fprintf(stderr, "blosc_b200: chunk 0's typesize %lld does not divide the frame's chunksize\n", (long long)f->typesize);
+  if (rc) return -1;
+  if (box_nbytes(nitems, (long long)f->typesize, (unsigned long long)f->nbytes)) { free(f->off); return -1; }
+  return 0;
+}
+
+/* The next chunk of an N-d read, from *c on, that touched[] flags: 1 with *c, *h and *codec set, 0 past the last
+ * chunk, frame_chunk_header's failure, or -1 with a message when the chunk does not hold the frame's items there. */
+static int frame_next_chunk(b2_ws* w, const void* frame, const b2_frame* f, long long nitems, const int* touched,
+                            size_t* c, b2_hdr* h, int* codec) {
+  const long long ts = (long long)f->typesize, ipc = (long long)f->ipc;
+  for (; *c < f->nchunks; ++*c) {
+    const long long w0 = (long long)*c * ipc, w1 = w0 + ipc < nitems ? w0 + ipc : nitems;
+    int rc;
+    if (!touched[*c]) continue;
+    *codec = 0;
+    rc = frame_chunk_header(w, frame, f, *c, h, codec);
+    if (rc < 0) return rc;
+    if (rc || h->nbytes != (w1 - w0) * ts) {
+      fprintf(stderr, "blosc_b200: chunk %zu holds %d items of %d bytes, not the frame's %lld of %lld\n", *c,
+              h->nbytes / h->typesize, h->typesize, w1 - w0, ts);
+      return -1;
+    }
+    return 1;
+  }
+  return 0;
+}
+
 int blosc_b200_frame_info(const void* frame, size_t framesize, size_t* nbytes, size_t* cbytes, size_t* chunksize,
                           size_t* nchunks) {
   b2_frame f;
@@ -2438,49 +2471,40 @@ long long blosc_b200_frame_getslice_step(const void* frame, size_t framesize, in
   size_t c;
   b2_frame f;
   long long nitems = 0, ts, ipc, sum = 0, got = 0, result = -1;
-  int dest_dev, rc;
+  int dest_dev, codec, *touched = NULL;
   B2Box box;
+  b2_hdr h;
   b2_ws* w;
   uint8_t* d_dst;
   if (!backend_ready()) return -1;
   if (box_geometry(ndim, shape, start, stop, &nitems) || box_steps(ndim, step)) return -1;
-  rc = frame_open_items(frame, framesize, &f);
-  if (rc == -2)
-    fprintf(stderr, "blosc_b200: chunk 0's typesize %lld does not divide the frame's chunksize\n", (long long)f.typesize);
-  if (rc) return -1;
+  if (frame_open_nd(frame, framesize, nitems, &f)) return -1;
   ts = (long long)f.typesize; ipc = (long long)f.ipc;
   dest_dev = b2_ptr_is_device(dest);
-  if (box_nbytes(nitems, ts, (unsigned long long)f.nbytes)) { free(f.off); return -1; }
   if (box_empty(ndim, start, stop)) { free(f.off); return 0; }
   box_build(ndim, shape, start, stop, step, nitems, &box);
   if (!(w = ws_acquire())) { free(f.off); return -1; }
   do {
     if (!(d_dst = stage_dest(&w->fstage, dest, dest_dev, (size_t)(box.count * ts)))) break;
-    for (c = 0; c < f.nchunks; c++) {
+    if (!(touched = (int*)malloc(sizeof(int) * f.nchunks))) break;
+    for (c = 0; c < f.nchunks; c++) {                                    /* the chunks that hold a box item */
       const long long w0 = (long long)c * ipc, w1 = w0 + ipc < nitems ? w0 + ipc : nitems;
-      b2_hdr h;
-      int codec = 0;
-      if (b2_box_next(&box, w0, box.stepped) >= w1) continue;             /* no box item in this chunk */
-      got = frame_chunk_header(w, frame, &f, c, &h, &codec);
-      if (got < 0) break;
-      if (got || h.nbytes != (w1 - w0) * ts) {
-        fprintf(stderr, "blosc_b200: chunk %zu holds %d items of %d bytes, not the frame's %lld of %lld\n", c,
-                h.nbytes / h.typesize, h.typesize, w1 - w0, ts);
-        got = -1;
-        break;
-      }
+      touched[c] = b2_box_next(&box, w0, box.stepped) < w1;
+    }
+    for (c = 0; (got = frame_next_chunk(w, frame, &f, nitems, touched, &c, &h, &codec)) > 0; c++) {
+      const long long w0 = (long long)c * ipc;
       got = getslice_chunk(w, (const uint8_t*)frame + f.off[c], f.dev, &h, codec, &box, w0,
                            d_dst + b2_box_rank(&box, w0, box.stepped) * ts);
       if (got < 0) break;
       sum += got;
     }
-    if (c < f.nchunks) { result = got; break; }
+    if (got < 0) { result = got; break; }
     if (sum != box.count * ts) break;
     if (!dest_dev && d2h_any(w, dest, d_dst, (size_t)sum)) break;
     result = sum;
   } while (0);
   ws_release(w);
-  free(f.off);
+  free(touched); free(f.off);
   return result;
 }
 
@@ -2498,21 +2522,18 @@ long long blosc_b200_frame_getslices(const void* frame, size_t framesize, int nd
   size_t c;
   b2_frame f;
   long long nitems = 0, ts, ipc, nbytes, got = 0, result = -1;
-  int dest_dev, rc;
+  int dest_dev, codec;
   B2Box box;
   BoxCheckArgs ck;
+  b2_hdr h;
   b2_ws* w;
   uint8_t *d_dst, *head = NULL;
   long long* part = NULL;
   if (!backend_ready()) return -1;
   if (boxes_geometry(ndim, shape, extent, nboxes, frame, dest, starts, &nitems)) return -1;
-  rc = frame_open_items(frame, framesize, &f);
-  if (rc == -2)
-    fprintf(stderr, "blosc_b200: chunk 0's typesize %lld does not divide the frame's chunksize\n", (long long)f.typesize);
-  if (rc) return -1;
+  if (frame_open_nd(frame, framesize, nitems, &f)) return -1;
   ts = (long long)f.typesize; ipc = (long long)f.ipc;
   dest_dev = b2_ptr_is_device(dest);
-  if (box_nbytes(nitems, ts, (unsigned long long)f.nbytes)) { free(f.off); return -1; }
   if (nboxes == 0 || box_empty(ndim, g_box_origin, extent)) { free(f.off); return 0; }
   boxes_build(ndim, shape, extent, nitems, nboxes, &box, &ck);
   if (boxes_nbytes(nboxes, ndim, box.count, ts)) { free(f.off); return -1; }
@@ -2524,29 +2545,17 @@ long long blosc_b200_frame_getslices(const void* frame, size_t framesize, int nd
     if (boxes_scratch(w, starts, (long long)f.nchunks, &ck, &part) || b2_launch_box_check(&ck, w->stream)) break;
     if (!(head = (uint8_t*)malloc(16 + 4 * f.nchunks)) || d2h_any(w, head, ck.bad, 16 + 4 * f.nchunks)) break;
     if (*(unsigned long long*)head != ~0ull) { box_bad_corner(w, &ck, *(unsigned long long*)head); break; }
-    for (c = 0; c < f.nchunks; c++) {
-      const long long w0 = (long long)c * ipc, w1 = w0 + ipc < nitems ? w0 + ipc : nitems;
-      b2_hdr h;
-      int codec = 0;
-      if (!((int*)(head + 16))[c]) continue;                               /* no box item in this chunk */
-      got = frame_chunk_header(w, frame, &f, c, &h, &codec);
-      if (got < 0) break;
-      if (got || h.nbytes != (w1 - w0) * ts) {
-        fprintf(stderr, "blosc_b200: chunk %zu holds %d items of %d bytes, not the frame's %lld of %lld\n", c,
-                h.nbytes / h.typesize, h.typesize, w1 - w0, ts);
-        got = -1;
-        break;
-      }
-      got = boxes_read(w, (const uint8_t*)frame + f.off[c], f.dev, &h, codec, &ck, 0, w0, part, nbytes, d_dst);
+    for (c = 0; (got = frame_next_chunk(w, frame, &f, nitems, (const int*)(head + 16), &c, &h, &codec)) > 0; c++) {
+      got = boxes_read(w, (const uint8_t*)frame + f.off[c], f.dev, &h, codec, &ck, 0, (long long)c * ipc, part, nbytes,
+                       d_dst);
       if (got < 0) break;
     }
-    if (c < f.nchunks) { result = got; break; }
+    if (got < 0) { result = got; break; }
     if (!dest_dev && d2h_any(w, dest, d_dst, (size_t)nbytes)) break;
     result = nbytes;
   } while (0);
   ws_release(w);
-  free(head);
-  free(f.off);
+  free(head); free(f.off);
   return result;
 }
 
@@ -2576,21 +2585,19 @@ long long blosc_b200_frame_getoindex(const void* frame, size_t framesize, int nd
   size_t c;
   b2_frame f;
   long long nitems = 0, count = 0, ts, ipc, nbytes, got = 0, result = -1;
-  int dest_dev, rc;
+  int dest_dev, codec;
   B2OSel sel;
+  b2_hdr h;
   b2_ws* w;
   uint8_t *d_dst, *head = NULL;
   if (ndim < 1 || ndim > B2_BOX_MAXDIM || !osel_any(ndim, index))
     return blosc_b200_frame_getslice_step(frame, framesize, ndim, shape, start, stop, step, dest);
   if (!backend_ready()) return -1;
   if (osel_geometry(ndim, shape, start, stop, step, index, nindex, frame, dest, st, sp, t, &nitems, &count)) return -1;
-  rc = frame_open_items(frame, framesize, &f);
-  if (rc == -2)
-    fprintf(stderr, "blosc_b200: chunk 0's typesize %lld does not divide the frame's chunksize\n", (long long)f.typesize);
-  if (rc) return -1;
+  if (frame_open_nd(frame, framesize, nitems, &f)) return -1;
   ts = (long long)f.typesize; ipc = (long long)f.ipc;
   dest_dev = b2_ptr_is_device(dest);
-  if (box_nbytes(nitems, ts, (unsigned long long)f.nbytes) || osel_nbytes(count, ts)) { free(f.off); return -1; }
+  if (osel_nbytes(count, ts)) { free(f.off); return -1; }
   if (count == 0) { free(f.off); return 0; }
   nbytes = count * ts;
   if (!(w = ws_acquire())) { free(f.off); return -1; }
@@ -2609,31 +2616,19 @@ long long blosc_b200_frame_getoindex(const void* frame, size_t framesize, int nd
     if (b2_launch_oindex_plan(&fa, w->stream)) break;
     if (!(head = (uint8_t*)malloc(16 + 4 * f.nchunks)) || d2h_any(w, head, w->fplan.p, 16 + 4 * f.nchunks)) break;
     if (*(unsigned long long*)head != ~0ull) { osel_bad_entry(w, &sel, *(unsigned long long*)head); break; }
-    for (c = 0; c < f.nchunks; c++) {
+    for (c = 0; (got = frame_next_chunk(w, frame, &f, nitems, (const int*)(head + 16), &c, &h, &codec)) > 0; c++) {
       const long long w0 = (long long)c * ipc, w1 = w0 + ipc < nitems ? w0 + ipc : nitems;
       long long g0, g1;
-      b2_hdr h;
-      int codec = 0;
-      if (!((int*)(head + 16))[c]) continue;                               /* no selected item in this chunk */
-      got = frame_chunk_header(w, frame, &f, c, &h, &codec);
-      if (got < 0) break;
-      if (got || h.nbytes != (w1 - w0) * ts) {
-        fprintf(stderr, "blosc_b200: chunk %zu holds %d items of %d bytes, not the frame's %lld of %lld\n", c,
-                h.nbytes / h.typesize, h.typesize, w1 - w0, ts);
-        got = -1;
-        break;
-      }
       osel_slabs(&sel, w0, w1, ts, &g0, &g1);
       got = oindex_chunk(w, (const uint8_t*)frame + f.off[c], f.dev, &h, codec, &sel, 1, w0, g0, g1, d_dst);
       if (got < 0) break;
     }
-    if (c < f.nchunks) { result = got; break; }
+    if (got < 0) { result = got; break; }
     if (!dest_dev && d2h_any(w, dest, d_dst, (size_t)nbytes)) break;
     result = nbytes;
   } while (0);
   ws_release(w);
-  free(head);
-  free(f.off);
+  free(head); free(f.off);
   return result;
 }
 

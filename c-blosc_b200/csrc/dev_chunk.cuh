@@ -794,6 +794,42 @@ DEV void warp_copy_vec(u8* __restrict__ dst, const u8* __restrict__ src, int n) 
   }
 }
 
+/* The block-mapped copy of the N-d gathers: bytes [s, s + n) of a chunk (chunk offsets are below 2^31, blocks of bs
+ * bytes) to out.  With slot NULL the chunk is read in place at src; else only its touched blocks were decoded, into
+ * the compact scratch at src, block b at slot[b] * bs.  slot_copy_warp is the whole warp's copy, one warp_copy_vec per
+ * piece, each piece cut at block edges; slot_copy_lane is one lane's, bytewise, reading slot[] again only when it
+ * crosses a block edge. */
+DEV void slot_copy_warp(u8* out, const u8* src, const int* slot, unsigned bs, unsigned s, long long n) {
+  while (n > 0) {
+    int m = (int)n;
+    const u8* from = src + s;
+    if (slot) {
+      const unsigned blk = s / bs, left = (blk + 1) * bs - s;
+      if ((unsigned)m > left) m = (int)left;
+      from = src + (long long)slot[blk] * bs + (s - blk * bs);
+    }
+    warp_copy_vec(out, from, m);
+    out += m; s += (unsigned)m; n -= m;
+  }
+}
+
+DEV void slot_copy_lane(u8* out, const u8* src, const int* slot, unsigned bs, unsigned s, int n) {
+  if (!slot) {
+    for (int x = 0; x < n; x++) out[x] = src[s + x];
+    return;
+  }
+  unsigned bend = 0;
+  const u8* base = src;
+  for (int x = 0; x < n; x++, s++) {
+    if (s >= bend) {
+      const unsigned blk = s / bs;
+      bend = (blk + 1) * bs;
+      base = src + (long long)slot[blk] * bs - (long long)blk * bs;
+    }
+    out[x] = base[s];
+  }
+}
+
 __global__ void __launch_bounds__(GATHER_WARPS * 32) gather_kernel(GatherArgs a) {
   if (a.status && ld_cg_i32(a.status) < 0) return;       /* a stream failed to decode: dest stays untouched */
   const long long warps = (long long)gridDim.x * GATHER_WARPS;
@@ -819,13 +855,15 @@ __global__ void __launch_bounds__(GATHER_WARPS * 32) gather_kernel(GatherArgs a)
 /* The CPU emulator's launcher of gather_kernel (the other kernels are launched by tests/emu/backend_emu.cpp, which
  * includes this header): a few CTAs, so that every warp goes through several spans.  It counts its own launches. */
 static long long g_emu_gather_launches = 0;
+static unsigned emu_gather_ctas(long long total) {
+  const long long ctas = (total + (long long)GATHER_WARPS * GATHER_SPAN - 1) / ((long long)GATHER_WARPS * GATHER_SPAN);
+  return (unsigned)(ctas > 3 ? 3 : ctas);
+}
 extern "C" int b2_launch_gather(const GatherArgs* a, b2_stream_t) {
   if (a->total <= 0) return 0;
-  long long ctas = (a->total + (long long)GATHER_WARPS * GATHER_SPAN - 1) / ((long long)GATHER_WARPS * GATHER_SPAN);
-  if (ctas > 3) ctas = 3;
   g_emu_gather_launches++;
   GatherArgs args = *a;
-  simt::launch(simt::Dim3((unsigned)ctas), simt::Dim3(GATHER_WARPS * 32), 0, [&] { gather_kernel(args); });
+  simt::launch(simt::Dim3(emu_gather_ctas(a->total)), simt::Dim3(GATHER_WARPS * 32), 0, [&] { gather_kernel(args); });
   return 0;
 }
 #endif
@@ -1048,31 +1086,31 @@ __global__ void __launch_bounds__(PLAN_THREADS) plan_scan_kernel(A a, long long 
 /* The emulator's launcher of the plan kernels: a few CTAs for the per-range check, so that the grid-stride loop runs;
  * every tile of a scan is its own CTA, as on the GPU.  The emulator has one device. */
 static long long g_emu_plan_launches = 0;
+static unsigned emu_tiles(long long n) { return (unsigned)((n + PLAN_TILE - 1) / PLAN_TILE); }
+static unsigned emu_range_ctas(long long n) { return (unsigned)(n > 2 * PLAN_THREADS ? 3 : (n + PLAN_THREADS - 1) / PLAN_THREADS); }
+/* the PLAN_SLOT scan over a chunk plan's blocks, one plan launch */
+static void emu_slot_scan(const PlanArgs& plan) {
+  const long long nb = plan.nblocks;
+  simt::launch(simt::Dim3(emu_tiles(nb)), simt::Dim3(PLAN_THREADS), 0, [&] { plan_scan_kernel<PLAN_SLOT>(plan, nb); });
+  g_emu_plan_launches++;
+}
 extern "C" int b2_launch_plan(const PlanArgs* a, b2_stream_t) {
   if (a->nranges <= 0) return 0;
   PlanArgs args = *a;
-  long long ctas = ((long long)a->nranges + PLAN_THREADS - 1) / PLAN_THREADS;
-  if (ctas > 3) ctas = 3;
-  simt::launch(simt::Dim3((unsigned)ctas), simt::Dim3(PLAN_THREADS), 0, [&] { plan_check_kernel(args); });
+  const long long nb = a->nblocks, nr = a->nranges;
+  simt::launch(simt::Dim3(emu_range_ctas(nr)), simt::Dim3(PLAN_THREADS), 0, [&] { plan_check_kernel(args); });
   g_emu_plan_launches++;
   if (!a->in_place) {
-    const long long nb = a->nblocks;
-    simt::launch(simt::Dim3((unsigned)((nb + PLAN_TILE - 1) / PLAN_TILE)), simt::Dim3(PLAN_THREADS), 0,
-                 [&] { plan_scan_kernel<PLAN_COVER>(args, nb); });
-    simt::launch(simt::Dim3((unsigned)((nb + PLAN_TILE - 1) / PLAN_TILE)), simt::Dim3(PLAN_THREADS), 0,
-                 [&] { plan_scan_kernel<PLAN_SLOT>(args, nb); });
-    g_emu_plan_launches += 2;
+    simt::launch(simt::Dim3(emu_tiles(nb)), simt::Dim3(PLAN_THREADS), 0, [&] { plan_scan_kernel<PLAN_COVER>(args, nb); });
+    g_emu_plan_launches++;
+    emu_slot_scan(args);
   }
-  const long long nr = a->nranges;
-  simt::launch(simt::Dim3((unsigned)((nr + PLAN_TILE - 1) / PLAN_TILE)), simt::Dim3(PLAN_THREADS), 0,
-               [&] { plan_scan_kernel<PLAN_POS>(args, nr); });
+  simt::launch(simt::Dim3(emu_tiles(nr)), simt::Dim3(PLAN_THREADS), 0, [&] { plan_scan_kernel<PLAN_POS>(args, nr); });
   g_emu_plan_launches++;
   return 0;
 }
 
 /* ... and of the frame plan's kernels, the same way; they count as plan launches */
-static unsigned emu_tiles(long long n) { return (unsigned)((n + PLAN_TILE - 1) / PLAN_TILE); }
-static unsigned emu_range_ctas(long long n) { return (unsigned)(n > 2 * PLAN_THREADS ? 3 : (n + PLAN_THREADS - 1) / PLAN_THREADS); }
 extern "C" int b2_launch_fplan(const FramePlanArgs* a, b2_stream_t) {
   if (a->nranges <= 0) return 0;
   FramePlanArgs args = *a;
@@ -1115,8 +1153,8 @@ __global__ void __launch_bounds__(PLAN_THREADS) box_touch_kernel(BoxPlanArgs a) 
 }
 
 /* box_gather_kernel: output-driven like gather_kernel, warp job k covering output bytes [k * GATHER_SPAN, (k + 1) *
- * GATHER_SPAN).  Runs of BOX_SHORT_RUN bytes or more are copied by the whole warp, one run piece at a time, each piece
- * cut at block edges.  Shorter runs are copied by one lane each: lane l takes every 32nd run that starts in the job's
+ * GATHER_SPAN).  Runs of BOX_SHORT_RUN bytes or more are copied by the whole warp (slot_copy_warp).  Shorter runs are
+ * copied by one lane each (slot_copy_lane): lane l takes every 32nd run that starts in the job's
  * bytes (the job of byte 0 also takes the run that the chunk's part starts inside), so no run is split between two
  * lanes.  Either way a run's source is the unrank of its first item.  With a step in the innermost dimension every run
  * is one item. */
@@ -1135,40 +1173,16 @@ __global__ void __launch_bounds__(GATHER_WARPS * 32) box_gather_kernel(BoxGather
       for (long long o = lo; o < hi;) {
         const long long g = g0 + o, k = b2_box_div(g, runb), u = g - k * runb;
         unsigned s = (unsigned)((b2_box_unrank(&a.box, k * a.box.run, STEPPED) - a.window) * ts + u);
-        long long n = runb - u < hi - o ? runb - u : hi - o;
-        while (n > 0) {
-          int m = (int)n;
-          const u8* from = a.src + s;
-          if (a.slot) {
-            const unsigned blk = s / bs, left = (blk + 1) * bs - s;
-            if ((unsigned)m > left) m = (int)left;
-            from = a.src + (long long)a.slot[blk] * bs + (s - blk * bs);
-          }
-          warp_copy_vec(a.dst + o, from, m);
-          o += m; s += (unsigned)m; n -= m;
-        }
+        const long long n = runb - u < hi - o ? runb - u : hi - o;
+        slot_copy_warp(a.dst + o, a.src, a.slot, bs, s, n);
+        o += n;
       }
     } else {
       const long long ka = b2_box_div(lo == 0 ? g0 : g0 + lo + runb - 1, runb), kb = b2_box_div(g0 + hi + runb - 1, runb);
       for (long long k = ka + lane; k < kb; k += 32) {
         const long long gs = k * runb > g0 ? k * runb : g0, ge = (k + 1) * runb < end ? (k + 1) * runb : end;
         unsigned s = (unsigned)((b2_box_unrank(&a.box, k * a.box.run, STEPPED) - a.window) * ts + (gs - k * runb));
-        u8* out = a.dst + (gs - g0);
-        const int n = (int)(ge - gs);
-        if (!a.slot) {
-          for (int x = 0; x < n; x++) out[x] = a.src[s + x];
-        } else {
-          unsigned bend = 0;
-          const u8* base = a.src;
-          for (int x = 0; x < n; x++, s++) {
-            if (s >= bend) {
-              const unsigned blk = s / bs;
-              bend = (blk + 1) * bs;
-              base = a.src + (long long)a.slot[blk] * bs - (long long)blk * bs;
-            }
-            out[x] = base[s];
-          }
-        }
+        slot_copy_lane(a.dst + (gs - g0), a.src, a.slot, bs, s, (int)(ge - gs));
       }
     }
   }
@@ -1184,17 +1198,15 @@ extern "C" int b2_launch_box_plan(const BoxPlanArgs* a, b2_stream_t) {
   simt::launch(simt::Dim3(emu_range_ctas(nb)), simt::Dim3(PLAN_THREADS), 0, [&] {
     if (args.box.stepped) box_touch_kernel<true>(args); else box_touch_kernel<false>(args);
   });
-  simt::launch(simt::Dim3(emu_tiles(nb)), simt::Dim3(PLAN_THREADS), 0, [&] { plan_scan_kernel<PLAN_SLOT>(args.plan, nb); });
-  g_emu_plan_launches += 2;
+  g_emu_plan_launches++;
+  emu_slot_scan(args.plan);
   return 0;
 }
 extern "C" int b2_launch_box_gather(const BoxGatherArgs* a, b2_stream_t) {
   if (a->total <= 0) return 0;
-  long long ctas = (a->total + (long long)GATHER_WARPS * GATHER_SPAN - 1) / ((long long)GATHER_WARPS * GATHER_SPAN);
-  if (ctas > 3) ctas = 3;
   g_emu_gather_launches++;
   BoxGatherArgs args = *a;
-  simt::launch(simt::Dim3((unsigned)ctas), simt::Dim3(GATHER_WARPS * 32), 0, [&] {
+  simt::launch(simt::Dim3(emu_gather_ctas(a->total)), simt::Dim3(GATHER_WARPS * 32), 0, [&] {
     if (args.box.stepped) box_gather_kernel<true>(args); else box_gather_kernel<false>(args);
   });
   return 0;
@@ -1286,17 +1298,8 @@ __global__ void __launch_bounds__(GATHER_WARPS * 32) boxes_gather_kernel(BoxesGa
         unsigned s = (unsigned)((b2_box_unrank(&a.box, (k - i * rpb) * a.box.run, 0) + f0 - a.window) * ts + u);
         long long n = runb - u < hi - o ? runb - u : hi - o;
         if (n > phi - gb) n = phi - gb;
-        while (n > 0) {
-          int m = (int)n;
-          const u8* from = a.src + s;
-          if (a.slot) {
-            const unsigned blk = s / bs, left = (blk + 1) * bs - s;
-            if ((unsigned)m > left) m = (int)left;
-            from = a.src + (long long)a.slot[blk] * bs + (s - blk * bs);
-          }
-          warp_copy_vec(a.dst + o, from, m);
-          o += m; s += (unsigned)m; n -= m;
-        }
+        slot_copy_warp(a.dst + o, a.src, a.slot, bs, s, n);
+        o += n;
       }
     } else {
       const long long ka = b2_box_div(lo + runb - 1, runb), kb = b2_box_div(hi + runb - 1, runb);
@@ -1308,22 +1311,7 @@ __global__ void __launch_bounds__(GATHER_WARPS * 32) boxes_gather_kernel(BoxesGa
         if (ge > i * boxb + phi) ge = i * boxb + phi;
         if (gs >= ge) continue;
         unsigned s = (unsigned)((b2_box_unrank(&a.box, (k - i * rpb) * a.box.run, 0) + f0 - a.window) * ts + (gs - k * runb));
-        u8* out = a.dst + gs;
-        const int n = (int)(ge - gs);
-        if (!a.slot) {
-          for (int x = 0; x < n; x++) out[x] = a.src[s + x];
-        } else {
-          unsigned bend = 0;
-          const u8* base = a.src;
-          for (int x = 0; x < n; x++, s++) {
-            if (s >= bend) {
-              const unsigned blk = s / bs;
-              bend = (blk + 1) * bs;
-              base = a.src + (long long)a.slot[blk] * bs - (long long)blk * bs;
-            }
-            out[x] = base[s];
-          }
-        }
+        slot_copy_lane(a.dst + gs, a.src, a.slot, bs, s, (int)(ge - gs));
       }
     }
   }
@@ -1342,20 +1330,17 @@ extern "C" int b2_launch_box_check(const BoxCheckArgs* a, b2_stream_t) {
 extern "C" int b2_launch_boxes_plan(const BoxesPlanArgs* a, b2_stream_t) {
   if (a->plan.nblocks <= 0) return 0;
   BoxesPlanArgs args = *a;
-  const long long nb = a->plan.nblocks;
   simt::launch(simt::Dim3(emu_range_ctas(a->nboxes * a->per_box)), simt::Dim3(PLAN_THREADS), 0,
                [&] { boxes_touch_kernel(args); });
-  simt::launch(simt::Dim3(emu_tiles(nb)), simt::Dim3(PLAN_THREADS), 0, [&] { plan_scan_kernel<PLAN_SLOT>(args.plan, nb); });
-  g_emu_plan_launches += 2;
+  g_emu_plan_launches++;
+  emu_slot_scan(args.plan);
   return 0;
 }
 extern "C" int b2_launch_boxes_gather(const BoxesGatherArgs* a, b2_stream_t) {
   if (a->total <= 0) return 0;
-  long long ctas = (a->total + (long long)GATHER_WARPS * GATHER_SPAN - 1) / ((long long)GATHER_WARPS * GATHER_SPAN);
-  if (ctas > 3) ctas = 3;
   g_emu_gather_launches++;
   BoxesGatherArgs args = *a;
-  simt::launch(simt::Dim3((unsigned)ctas), simt::Dim3(GATHER_WARPS * 32), 0, [&] { boxes_gather_kernel(args); });
+  simt::launch(simt::Dim3(emu_gather_ctas(a->total)), simt::Dim3(GATHER_WARPS * 32), 0, [&] { boxes_gather_kernel(args); });
   return 0;
 }
 #endif
@@ -1429,18 +1414,8 @@ __global__ void __launch_bounds__(GATHER_WARPS * 32) oindex_gather_kernel(OIndex
           if (u >= ahi) { o += n; continue; }
           if (n > ahi - u) n = ahi - u;
         }
-        unsigned s = (unsigned)((f - a.window) * ts + u);
-        while (n > 0) {
-          int m = (int)n;
-          const u8* from = a.src + s;
-          if (a.slot) {
-            const unsigned blk = s / bs, left = (blk + 1) * bs - s;
-            if ((unsigned)m > left) m = (int)left;
-            from = a.src + (long long)a.slot[blk] * bs + (s - blk * bs);
-          }
-          warp_copy_vec(a.dst + a.g0 + o, from, m);
-          o += m; s += (unsigned)m; n -= m;
-        }
+        slot_copy_warp(a.dst + a.g0 + o, a.src, a.slot, bs, (unsigned)((f - a.window) * ts + u), n);
+        o += n;
       }
     } else {
       const long long ka = b2_box_div(a.g0 + lo + runb - 1, runb), kb = b2_box_div(a.g0 + hi + runb - 1, runb);
@@ -1452,23 +1427,8 @@ __global__ void __launch_bounds__(GATHER_WARPS * 32) oindex_gather_kernel(OIndex
           if (f < a.window) x0 = a.window - f;
           if (f + run > a.wend) x1 = a.wend - f;
         }
-        unsigned s = (unsigned)((f + x0 - a.window) * ts);
-        u8* out = a.dst + (k * run + x0) * ts;
-        const int n = (int)((x1 - x0) * ts);
-        if (!a.slot) {
-          for (int x = 0; x < n; x++) out[x] = a.src[s + x];
-        } else {
-          unsigned bend = 0;
-          const u8* base = a.src;
-          for (int x = 0; x < n; x++, s++) {
-            if (s >= bend) {
-              const unsigned blk = s / bs;
-              bend = (blk + 1) * bs;
-              base = a.src + (long long)a.slot[blk] * bs - (long long)blk * bs;
-            }
-            out[x] = base[s];
-          }
-        }
+        slot_copy_lane(a.dst + (k * run + x0) * ts, a.src, a.slot, bs, (unsigned)((f + x0 - a.window) * ts),
+                       (int)((x1 - x0) * ts));
       }
     }
   }
@@ -1484,20 +1444,15 @@ extern "C" int b2_launch_oindex_plan(const OIndexPlanArgs* a, b2_stream_t) {
     simt::launch(simt::Dim3(emu_range_ctas(n)), simt::Dim3(PLAN_THREADS), 0, [&] { oindex_touch_kernel(args); });
     g_emu_plan_launches++;
   }
-  if (!a->touched && a->r1 > a->r0 && nb > 0) {
-    simt::launch(simt::Dim3(emu_tiles(nb)), simt::Dim3(PLAN_THREADS), 0, [&] { plan_scan_kernel<PLAN_SLOT>(args.plan, nb); });
-    g_emu_plan_launches++;
-  }
+  if (!a->touched && a->r1 > a->r0 && nb > 0) emu_slot_scan(args.plan);
   return 0;
 }
 extern "C" int b2_launch_oindex_gather(const OIndexGatherArgs* a, b2_stream_t) {
   const long long total = a->g1 - a->g0;
   if (total <= 0) return 0;
-  long long ctas = (total + (long long)GATHER_WARPS * GATHER_SPAN - 1) / ((long long)GATHER_WARPS * GATHER_SPAN);
-  if (ctas > 3) ctas = 3;
   g_emu_gather_launches++;
   OIndexGatherArgs args = *a;
-  simt::launch(simt::Dim3((unsigned)ctas), simt::Dim3(GATHER_WARPS * 32), 0, [&] { oindex_gather_kernel(args); });
+  simt::launch(simt::Dim3(emu_gather_ctas(total)), simt::Dim3(GATHER_WARPS * 32), 0, [&] { oindex_gather_kernel(args); });
   return 0;
 }
 #endif
@@ -1507,7 +1462,7 @@ extern "C" int b2_launch_oindex_gather(const OIndexGatherArgs* a, b2_stream_t) {
  * The walk is box_gather_kernel's over the part's bytes [0, total), one warp job per GATHER_SPAN bytes, with the run's
  * source the chunk box's unrank and its destination the output box's.  The part starts at a run edge and holds whole
  * runs, so a lane-per-run job takes exactly the runs that start in its bytes.  STEPPED = the chunk box's `stepped`;
- * the output box has step 1.  A kernel of its own, so that the box kernels' code and registers stay as they are. */
+ * the output box has step 1. */
 template <bool STEPPED>
 __global__ void __launch_bounds__(GATHER_WARPS * 32) placed_gather_kernel(PlacedGatherArgs a) {
   if (a.status && ld_cg_i32(a.status) < 0) return;       /* a stream failed to decode: dest stays untouched */
@@ -1522,41 +1477,16 @@ __global__ void __launch_bounds__(GATHER_WARPS * 32) placed_gather_kernel(Placed
       for (long long o = lo; o < hi;) {
         const long long k = b2_box_div(o, runb), u = o - k * runb;
         u8* out = a.dst + b2_box_unrank(&a.out, k * a.run, 0) * ts + u;
-        unsigned s = (unsigned)(b2_box_unrank(&a.box, k * a.run, STEPPED) * ts + u);
-        long long n = runb - u < hi - o ? runb - u : hi - o;
-        while (n > 0) {
-          int m = (int)n;
-          const u8* from = a.src + s;
-          if (a.slot) {
-            const unsigned blk = s / bs, left = (blk + 1) * bs - s;
-            if ((unsigned)m > left) m = (int)left;
-            from = a.src + (long long)a.slot[blk] * bs + (s - blk * bs);
-          }
-          warp_copy_vec(out, from, m);
-          out += m; o += m; s += (unsigned)m; n -= m;
-        }
+        const unsigned s = (unsigned)(b2_box_unrank(&a.box, k * a.run, STEPPED) * ts + u);
+        const long long n = runb - u < hi - o ? runb - u : hi - o;
+        slot_copy_warp(out, a.src, a.slot, bs, s, n);
+        o += n;
       }
     } else {
       const long long ka = b2_box_div(lo + runb - 1, runb), kb = b2_box_div(hi + runb - 1, runb);
-      for (long long k = ka + lane; k < kb; k += 32) {
-        unsigned s = (unsigned)(b2_box_unrank(&a.box, k * a.run, STEPPED) * ts);
-        u8* out = a.dst + b2_box_unrank(&a.out, k * a.run, 0) * ts;
-        const int n = (int)runb;
-        if (!a.slot) {
-          for (int x = 0; x < n; x++) out[x] = a.src[s + x];
-        } else {
-          unsigned bend = 0;
-          const u8* base = a.src;
-          for (int x = 0; x < n; x++, s++) {
-            if (s >= bend) {
-              const unsigned blk = s / bs;
-              bend = (blk + 1) * bs;
-              base = a.src + (long long)a.slot[blk] * bs - (long long)blk * bs;
-            }
-            out[x] = base[s];
-          }
-        }
-      }
+      for (long long k = ka + lane; k < kb; k += 32)
+        slot_copy_lane(a.dst + b2_box_unrank(&a.out, k * a.run, 0) * ts, a.src, a.slot, bs,
+                       (unsigned)(b2_box_unrank(&a.box, k * a.run, STEPPED) * ts), (int)runb);
     }
   }
 }
@@ -1615,7 +1545,7 @@ DEV unsigned warp_copy_cmp(u8* __restrict__ dst, const u8* __restrict__ src, int
  * walk is placed_gather_kernel's over the part's bytes [0, total), with the run's source the array box's unrank and its
  * destination the chunk box's; both boxes have step 1.  Source offsets are 64-bit: the array may exceed 4 GiB.  CMP =
  * a.diff != NULL: each lane compares the bytes it stores with the fill pattern and sets *diff once at the end; without
- * it the kernel only copies.  A kernel of its own, so that the placed kernels keep their code and registers. */
+ * it the kernel only copies. */
 template <bool CMP>
 __global__ void __launch_bounds__(GATHER_WARPS * 32) grid_pack_kernel(GridPackArgs a) {
   const long long ts = a.itemsize, runb = a.run * ts;
@@ -1654,10 +1584,6 @@ __global__ void __launch_bounds__(GATHER_WARPS * 32) grid_pack_kernel(GridPackAr
 
 #ifdef SIMT_EMU
 /* The emulator's launchers of the placed kernels, as those of the box kernels; both count as gather launches */
-static unsigned emu_gather_ctas(long long total) {
-  const long long ctas = (total + (long long)GATHER_WARPS * GATHER_SPAN - 1) / ((long long)GATHER_WARPS * GATHER_SPAN);
-  return (unsigned)(ctas > 3 ? 3 : ctas);
-}
 extern "C" int b2_launch_placed_gather(const PlacedGatherArgs* a, b2_stream_t) {
   if (a->total <= 0) return 0;
   g_emu_gather_launches++;

@@ -3,8 +3,8 @@
   LD_PRELOAD=$(gcc -print-file-name=libasan.so) ASAN_OPTIONS=detect_leaks=0 python scripts/asan_emu_case.py
 exact / fast / lz4hc / BloscLZ paths, exact-size buffers, damaged chunks, crafted and damaged zstd frames and zlib streams,
 crafted, random and damaged LZ4 and BloscLZ streams, the snappy encoder (serial and pool maxout rules), crafted,
-random and damaged snappy streams, and item ranges, boxes and batches of boxes of whole and damaged chunks and frames,
-in host and in device memory."""
+random and damaged snappy streams, item ranges, boxes, batches of boxes and index selections of whole and damaged
+chunks and frames, and boxes of chunk grids with present, missing and damaged chunks, in host and in device memory."""
 import os, sys, ctypes as C, numpy as np
 sys.path.insert(0, os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), 'tests'))
 from datagen import gen, compress, decompress
@@ -151,7 +151,9 @@ for f,res,args in (("blosc_b200_getitems",ll,[vp,C.c_int,vp,vp,vp]),("blosc_b200
                    ("blosc_b200_frame_bound",sz,[sz,sz,sz]),("blosc_b200_frame_compress",ll,[C.c_int,C.c_int,sz,sz,vp,vp,sz,C.c_char_p,sz,sz,C.c_int]),
                    ("blosc_b200_frame_getitems",ll,[vp,sz,sz,vp,vp,vp]),("blosc_b200_frame_getslice",ll,[vp,sz,C.c_int,vp,vp,vp,vp]),
                    ("blosc_b200_getslices",ll,[vp,C.c_int,vp,vp,ll,vp,vp]),("blosc_b200_frame_getslices",ll,[vp,sz,C.c_int,vp,vp,ll,vp,vp]),
-                   ("blosc_b200_getslice_step",ll,[vp,C.c_int,vp,vp,vp,vp,vp]),("blosc_b200_frame_getslice_step",ll,[vp,sz,C.c_int,vp,vp,vp,vp,vp])):
+                   ("blosc_b200_getslice_step",ll,[vp,C.c_int,vp,vp,vp,vp,vp]),("blosc_b200_frame_getslice_step",ll,[vp,sz,C.c_int,vp,vp,vp,vp,vp]),
+                   ("blosc_b200_frame_getoindex",ll,[vp,sz,C.c_int,vp,vp,vp,vp,vp,vp,vp]),
+                   ("blosc_b200_grid_getslice",ll,[C.c_int,vp,vp,sz,vp,vp,vp,vp,vp,vp])):
     getattr(emu,f).restype=res; getattr(emu,f).argtypes=args
 emu.emu_set_all_device.argtypes=[C.c_int]
 irng=np.random.default_rng(11)
@@ -169,6 +171,13 @@ ext=np.array([9,31],np.int64)                 # a batch of boxes, overlapping an
 corners=np.array([[0,0],[291,219],[100,7],[100,7],[150,200]]+[[int(a),int(b)] for a,b in zip(irng.integers(0,292,40),irng.integers(0,220,40))],np.int64)
 want_boxes=b"".join(arr[a:a+9,b:b+31].tobytes() for a,b in corners)
 bad=corners.copy(); bad[30,1]=220
+rows=np.array([5,290,17,17,120,0,299],np.int64); cols=np.arange(30,200,3)      # an index selection: unsorted rows, a column slice
+want_osel=arr[np.ix_(rows,cols)].tobytes()
+badrows=rows.copy(); badrows[3]=300
+ozero=np.zeros(2,np.int64); ostop=np.array([0,200],np.int64); ostep=np.array([0,3],np.int64); ostart=np.array([0,30],np.int64)
+def frame_oindex(f,fb,r,out):
+    ptrs=(vp*2)(r.ctypes.data,None); ni=np.array([r.size,0],np.int64)
+    return emu.blosc_b200_frame_getoindex(P(f),fb,2,P(sh),P(ostart),P(ostop),P(ostep),C.cast(ptrs,vp),P(ni),P(out))
 for comp,shuf,cl in (("lz4",1,5),("blosclz",2,5),("lz4",1,0)):
     dest=np.zeros(n+16,np.uint8)
     r=emu.blosc_compress_ctx(C.c_int(cl),C.c_int(shuf),C.c_size_t(ts),C.c_size_t(n),P(src),P(dest),C.c_size_t(n+16),comp.encode(),C.c_size_t(4096),C.c_int(1))
@@ -212,7 +221,49 @@ for comp,shuf,cl in (("lz4",1,5),("blosclz",2,5),("lz4",1,0)):
                 g=emu.blosc_b200_frame_getslices(P(f),fb,2,P(sh),P(ext),len(corners),P(corners),P(out))
                 assert f is not frame or (g==len(want_boxes) and out.tobytes()==want_boxes)
                 assert emu.blosc_b200_frame_getslices(P(f),fb,2,P(sh),P(ext),len(bad),P(bad),P(out))<0
-                cases+=5
+                out=np.zeros(len(want_osel),np.uint8)
+                g=frame_oindex(f,fb,rows,out)
+                assert f is not frame or (g==len(want_osel) and out.tobytes()==want_osel)
+                assert frame_oindex(f,fb,badrows,out)<0
+                cases+=7
         finally:
             emu.emu_set_all_device(0)
+# boxes of the array stored as a grid of 64 x 96 chunks (edge chunks padded to full shape): every chunk present, some
+# missing (read as the fill pattern), and some damaged, with and without steps, chunks in host and in device memory
+cs=np.array([64,96],np.int64); grid=(5,3)
+fill=np.array([0xDEADBEEF],np.uint32)
+gstart=np.array([17,30],np.int64); gstop=np.array([290,240],np.int64); gstep=np.array([2,3],np.int64)
+gchunks=[]
+for gi in range(grid[0]):
+    for gj in range(grid[1]):
+        buf=np.zeros((64,96),np.uint32); part=arr[gi*64:(gi+1)*64,gj*96:(gj+1)*96]; buf[:part.shape[0],:part.shape[1]]=part
+        d=buf.view(np.uint8).reshape(-1); dest=np.zeros(d.size+16,np.uint8)
+        r=emu.blosc_compress_ctx(C.c_int(5),C.c_int(1),C.c_size_t(ts),C.c_size_t(d.size),P(d),P(dest),C.c_size_t(d.size+16),b"lz4",C.c_size_t(4096),C.c_int(1))
+        assert r>0
+        gchunks.append(dest[:r].copy())
+missing={1,7,14}
+filled=arr.copy()
+for i in missing:
+    gi,gj=divmod(i,grid[1]); filled[gi*64:(gi+1)*64,gj*96:(gj+1)*96]=fill[0]
+def grid_read(chunks,step,out):
+    table=(vp*len(chunks))(*[None if c is None else c.ctypes.data for c in chunks])
+    return emu.blosc_b200_grid_getslice(2,P(sh),P(cs),ts,table,P(fill),P(gstart),P(gstop),None if step is None else P(step),P(out))
+for dev in (0,1):
+    emu.emu_set_all_device(dev)
+    try:
+        for step in (None,gstep):
+            sl=tuple(slice(a,b,s) for a,b,s in zip(gstart,gstop,[1,1] if step is None else step))
+            for kind in ("present","missing","damaged"):
+                chunks=list(gchunks)
+                if kind=="missing": chunks=[None if i in missing else c for i,c in enumerate(chunks)]
+                if kind=="damaged":
+                    for i in (4,8):
+                        c=chunks[i].copy(); pos=irng.integers(16,len(c),6); c[pos]=irng.integers(0,256,6,dtype=np.uint8); chunks[i]=c
+                want=np.ascontiguousarray((filled if kind=="missing" else arr)[sl]).tobytes()
+                out=np.zeros(len(want),np.uint8)
+                g=grid_read(chunks,step,out)
+                assert kind=="damaged" or (g==len(want) and out.tobytes()==want)
+                cases+=1
+    finally:
+        emu.emu_set_all_device(0)
 print("asan workload ok, cases", cases)
