@@ -27,16 +27,19 @@
  * produces with its default block sizes) positions fit in 17 bits: 16 low bits in a u16 array plus
  * one bit in a bitmap = 34 KiB, i.e. six streams per SM.  Same contents, same replacement policy. */
 struct BlzTab32 {
+  enum { PACKED = 0 };
   u32* t;
   DEV int get(u32 h) const { return (int)t[h]; }
   DEV void put(u32 h, int pos) const { t[h] = (u32)pos; }
 };
 struct BlzTab16 {                              /* the entropy probe's 2^12 x u16 table (blosclz.c:321-322) */
+  enum { PACKED = 0 };
   u16* t;
   DEV int get(u32 h) const { return (int)t[h]; }
   DEV void put(u32 h, int pos) const { t[h] = (u16)pos; }
 };
 struct BlzTab17 {
+  enum { PACKED = 1 };
   u16* lo;
   u32* hi;
   DEV int get(u32 h) const { return (int)lo[h] | (int)(((hi[h >> 5] >> (h & 31u)) & 1u) << 16); }
@@ -48,6 +51,50 @@ struct BlzTab17 {
 };
 #define BLZ_TAB17_BYTES (32768 + 2048)
 #define BLZ_TAB17_MAXLEN 131072
+
+/* branch ids of the encoder (blz_encode_warp, blz_search_round, blz_probe_one, blz_probe_warp); emulator builds count
+ * them so that tests can tell which path a stream reached */
+enum {
+  /* entropy probe */
+  BLZE_H_PROBE_BELOW, BLZE_H_PROBE_EQUAL, BLZE_H_PROBE_ABOVE,   /* cratio below / equal to / above the clevel's threshold */
+  BLZE_H_PROBE_EXT,                          /* the probe's own match extension (m >= 12) */
+  BLZE_H_SHIFT3_NOSPLIT, BLZE_H_SHIFT3_LOWRATIO, BLZE_H_SHIFT4,   /* ipshift / minlen 3: split_block 0 / cratio < 4; else 4 */
+  /* refusals */
+  BLZE_H_REF_SHORT, BLZE_H_REF_MAXOUT,       /* length < 16 / maxout < 66 */
+  /* tables */
+  BLZE_H_TAB_HL12, BLZE_H_TAB_HL13, BLZE_H_TAB_HL14, BLZE_H_TAB_17, BLZE_H_TAB_32,
+  BLZE_H_TAB17_HI,                           /* a match whose candidate is at position >= 65536 (bit 16 of BlzTab17) */
+  /* search round */
+  BLZE_H_R_LANE0, BLZE_H_R_LANE31, BLZE_H_R_NONE,   /* the accepting lane is 0 / 31 / none (32 literals) */
+  BLZE_H_R_FWD,                              /* the accepting lane's candidate comes from a lower lane with its hash */
+  BLZE_H_R_PARTIAL,                          /* fewer than 32 valid lanes (ip_limit) */
+  BLZE_H_R_MINLEN3, BLZE_H_R_BELOW3, BLZE_H_R_MINLEN4, BLZE_H_R_BELOW4,   /* len == minlen (taken) / minlen - 1, per ipshift */
+  BLZE_H_EXT_MISMATCH, BLZE_H_EXT_BOUND,     /* m == 12, extended to a mismatch / to ip_bound */
+  /* distance rules (search round and blz_probe_one) */
+  BLZE_H_FAR5, BLZE_H_FAR6,                  /* equal bytes at a far distance, len 5 (refused) / 6 (taken) */
+  BLZE_H_MAXFAR_M1, BLZE_H_MAXFAR,           /* equal bytes at distance MAX_FARDISTANCE - 1 (taken) / MAX_FARDISTANCE (refused) */
+  /* blz_probe_one after a match */
+  BLZE_H_P1_HIT, BLZE_H_P1_DIST, BLZE_H_P1_BYTES, BLZE_H_P1_LEN,   /* a hit; misses: distance, bytes, length / far rule */
+  /* emission */
+  BLZE_H_NEAR8190, BLZE_H_FAR8191,           /* biased distance 8190 (the farthest near) / 8191 (the nearest far) */
+  BLZE_H_SHORT_NEAR, BLZE_H_SHORT_FAR,
+  BLZE_H_LONG_NEAR0, BLZE_H_LONG_NEAR1, BLZE_H_LONG_NEAR2,   /* MATCH_LONG with zero / one / two 255 bytes */
+  BLZE_H_LONG_FAR0, BLZE_H_LONG_FAR1, BLZE_H_LONG_FAR2,
+  BLZE_H_COPY0,                              /* a match right after a match: op-- */
+  BLZE_H_LIT_CROSS,                          /* a literal run that crosses a 32-byte control boundary */
+  BLZE_H_L9_STORE,                           /* clevel 9: the second table store */
+  /* BLZ_LIMIT: the check that refused the stream */
+  BLZE_H_LIM_LIT, BLZE_H_LIM_SHORT, BLZE_H_LIM_LONG, BLZE_H_LIM_CTRL, BLZE_H_LIM_LEFT,
+  BLZE_NHIT
+};
+#ifdef SIMT_EMU
+static long long g_blze_hit[BLZE_NHIT + 1];      /* [BLZE_NHIT]: "none of these", not counted */
+#define BLZE_HIT(id) do { if (lane_id() == 0) g_blze_hit[id]++; } while (0)         /* warp-uniform branch */
+#define BLZE_HITL(id, c) do { if (c) g_blze_hit[id]++; } while (0)                /* per lane */
+#else
+#define BLZE_HIT(id) do {} while (0)
+#define BLZE_HITL(id, c) do {} while (0)
+#endif
 
 DEV u32 blz_hash(u32 seq, u32 hashlog) { return (seq * 2654435761u) >> (32u - hashlog); }   /* blosclz.c:58-60 */
 
@@ -86,7 +133,14 @@ DEV int blz_search_round(const u8* __restrict__ b, int ip, int ip_limit, const T
       const int len = m + 1 - ipshift;
       const bool far = FARRULE && (dist - 1u >= BLZ_MAX_DISTANCE);
       acc = m >= 12 || (len >= minlen && !(len <= 5 && far));               /* :535 */
+      if (FARRULE) {
+        BLZE_HITL(ipshift == 3 ? BLZE_H_R_MINLEN3 : BLZE_H_R_MINLEN4, m < 12 && len == minlen && !far);
+        BLZE_HITL(ipshift == 3 ? BLZE_H_R_BELOW3 : BLZE_H_R_BELOW4, m < 12 && len == minlen - 1 && !far);
+        BLZE_HITL(len == 5 ? BLZE_H_FAR5 : BLZE_H_FAR6, far && m < 12 && (len == 5 || len == 6) && len >= minlen);
+        BLZE_HITL(BLZE_H_MAXFAR_M1, dist == BLZ_MAX_FARDISTANCE - 1);
+      }
     }
+    if (FARRULE) BLZE_HITL(BLZE_H_MAXFAR, dist == BLZ_MAX_FARDISTANCE && ld_u32(b + cand) == seq);
   }
   const unsigned found = __ballot_sync(FULLMASK, acc);
   const int nv = __popc(vmask);
@@ -99,6 +153,11 @@ DEV int blz_search_round(const u8* __restrict__ b, int ip, int ip_limit, const T
   }
   __syncwarp();
   *nvalid = nv;
+  if (FARRULE) {
+    BLZE_HIT(f == 0 ? BLZE_H_R_LANE0 : f == 31 ? BLZE_H_R_LANE31 : f == 32 && nv == 32 ? BLZE_H_R_NONE : BLZE_NHIT);
+    if (nv < 32) BLZE_HIT(BLZE_H_R_PARTIAL);
+    BLZE_HITL(BLZE_H_R_FWD, lane == f && lower != 0);
+  }
   if (found) {
     *cand_f = __shfl_sync(FULLMASK, cand, f);
     *m_f = __shfl_sync(FULLMASK, m, f);
@@ -119,14 +178,21 @@ DEV int blz_probe_one(const u8* __restrict__ b, int pos, const Tab tab, u32 hash
   if (lane_id() == 0) tab.put(h, pos);
   __syncwarp();                              /* ordered before lane 0's later inserts and everybody's next lookups */
   const u32 dist = (u32)(pos - cand);
-  if (dist == 0 || dist >= BLZ_MAX_FARDISTANCE || ld_u32(b + cand) != seq) return 32;
+  if (FARRULE) BLZE_HIT(dist == BLZ_MAX_FARDISTANCE && ld_u32(b + cand) == seq ? BLZE_H_MAXFAR : BLZE_NHIT);
+  if (dist == 0 || dist >= BLZ_MAX_FARDISTANCE) { BLZE_HIT(BLZE_H_P1_DIST); return 32; }
+  if (ld_u32(b + cand) != seq) { BLZE_HIT(BLZE_H_P1_BYTES); return 32; }
   int m;
   const u32 x1 = ld_u32(b + pos + 4) ^ ld_u32(b + cand + 4);
   if (x1) m = 4 + eq_bytes32(x1);
   else m = 8 + eq_bytes32(ld_u32(b + pos + 8) ^ ld_u32(b + cand + 8));
   const int len = m + 1 - ipshift;
   const bool far = FARRULE && (dist - 1u >= BLZ_MAX_DISTANCE);
-  if (!(m >= 12 || (len >= minlen && !(len <= 5 && far)))) return 32;
+  if (FARRULE) {
+    BLZE_HIT(far && m < 12 && len >= minlen && (len == 5 || len == 6) ? (len == 5 ? BLZE_H_FAR5 : BLZE_H_FAR6) : BLZE_NHIT);
+    BLZE_HIT(dist == BLZ_MAX_FARDISTANCE - 1 ? BLZE_H_MAXFAR_M1 : BLZE_NHIT);
+  }
+  if (!(m >= 12 || (len >= minlen && !(len <= 5 && far)))) { BLZE_HIT(BLZE_H_P1_LEN); return 32; }
+  BLZE_HIT(BLZE_H_P1_HIT);
   *cand_f = cand; *m_f = m;
   return 0;
 }
@@ -151,6 +217,7 @@ DEV double blz_probe_warp(const u8* __restrict__ b, int maxlen, void* tabmem) {
     ip += nlit;
     if (f == 32) continue;
     const int anchor = ip, dist = anchor - cand;
+    if (m >= 12) BLZE_HIT(BLZE_H_PROBE_EXT);
     const int e = m < 12 ? anchor + m + 1 : blz_match_end_warp(b, anchor + 12, dist, ip_bound);
     ip = e - 3;
     const int len = ip - anchor;
@@ -189,16 +256,20 @@ DEV int blz_encode_warp(const int clevel, const u8* __restrict__ b, const int le
     case 9: thr = 1.0; break;
     default: thr = 1.2; break;
   }
+  BLZE_HIT(cratio < thr ? BLZE_H_PROBE_BELOW : cratio == thr ? BLZE_H_PROBE_EQUAL : BLZE_H_PROBE_ABOVE);
   if (cratio < thr) return 0;
   int ipshift = 4, minlen = 4;
   if (!split_block || cratio < 4) { ipshift = 3; minlen = 3; }               /* :445-457 */
+  BLZE_HIT(!split_block ? BLZE_H_SHIFT3_NOSPLIT : cratio < 4 ? BLZE_H_SHIFT3_LOWRATIO : BLZE_H_SHIFT4);
   const u32 hashlog = clevel == 1 ? 12u : (clevel == 2 ? 13u : 14u);         /* :459-461 */
-  if (length < 16 || maxout < 66) return 0;                                  /* :473-475 */
+  if (length < 16 || maxout < 66) { BLZE_HIT(length < 16 ? BLZE_H_REF_SHORT : BLZE_H_REF_MAXOUT); return 0; }   /* :473-475 */
+  BLZE_HIT(BLZE_H_TAB_HL12 + (hashlog - 12));
 
   __syncwarp();
   if (hashlog == 14 && table_bytes < 65536) {                               /* packed 17-bit table (host guarantees length <= 128 KiB) */
     for (int i = lane; i < BLZ_TAB17_BYTES / 4; i += 32) ((u32*)tabmem)[i] = 0;
     __syncwarp();
+    BLZE_HIT(BLZE_H_TAB_17);
     BlzTab17 t;
     t.lo = (u16*)tabmem;
     t.hi = (u32*)((u8*)tabmem + 32768);
@@ -206,6 +277,7 @@ DEV int blz_encode_warp(const int clevel, const u8* __restrict__ b, const int le
   }
   for (int i = lane; i < (1 << hashlog); i += 32) ((u32*)tabmem)[i] = 0;
   __syncwarp();
+  if (hashlog == 14) BLZE_HIT(BLZE_H_TAB_32);
   BlzTab32 t;
   t.t = (u32*)tabmem;
   return blz_encode_main<BlzTab32>(clevel, b, length, out, maxout, ipshift, minlen, hashlog, t, need_out);
@@ -219,7 +291,7 @@ DEV int blz_encode_main(const int clevel, const u8* __restrict__ b, const int le
   const int ip_bound = length - 1, ip_limit = length - 12, op_limit = maxout;
   int ip = 4, op = 5, copy = 4;
   int need = 66;                                                            /* :473-475: maxout < 66 is refused */
-#define BLZ_LIMIT(v) do { const int v_ = (v); if (v_ > need) need = v_; if (v_ > op_limit) return 0; } while (0)
+#define BLZ_LIMIT(v, site) do { const int v_ = (v); if (v_ > need) need = v_; if (v_ > op_limit) { BLZE_HIT(site); return 0; } } while (0)
   if (lane == 0) { out[0] = BLZ_MAX_COPY - 1; out[1] = b[0]; out[2] = b[1]; out[3] = b[2]; out[4] = b[3]; }   /* :481-487 */
 
   bool post = false;                                                         /* a match was just emitted */
@@ -230,7 +302,8 @@ DEV int blz_encode_main(const int clevel, const u8* __restrict__ b, const int le
     post = f < 32;
     const int nlit = f < 32 ? f : nvalid;
     if (nlit > 0) {                                                          /* LITERAL x nlit, :246-256 */
-      BLZ_LIMIT(op + (nlit - 1) + ((copy + nlit - 1) >> 5) + 2);
+      BLZ_LIMIT(op + (nlit - 1) + ((copy + nlit - 1) >> 5) + 2, BLZE_H_LIM_LIT);
+      if ((copy + nlit) >> 5) BLZE_HIT(BLZE_H_LIT_CROSS);
       if (lane < nlit) {
         const int o = op + lane + ((copy + lane) >> 5);
         out[o] = b[ip + lane];
@@ -246,16 +319,20 @@ DEV int blz_encode_main(const int clevel, const u8* __restrict__ b, const int le
     const int anchor = ip;
     u32 distance = (u32)(anchor - cand) - 1u;                                /* biased, :524 */
     const int e = m < 12 ? anchor + m + 1 : blz_match_end_warp(b, anchor + 12, (int)distance + 1, ip_bound);
+    if (m >= 12) BLZE_HIT(e < ip_bound ? BLZE_H_EXT_MISMATCH : BLZE_H_EXT_BOUND);
+    if (Tab::PACKED && cand >= 65536) BLZE_HIT(BLZE_H_TAB17_HI);
+    BLZE_HIT(distance == 8190 ? BLZE_H_NEAR8190 : distance == 8191 ? BLZE_H_FAR8191 : BLZE_NHIT);
     ip = e - ipshift;                                                        /* :530 */
     u32 len = (u32)(ip - anchor);
 
     if (copy) { if (lane == 0) out[op - copy - 1] = (u8)(copy - 1); }        /* :541-546 */
-    else op--;
+    else { BLZE_HIT(BLZE_H_COPY0); op--; }
     copy = 0;
     const bool far = distance >= BLZ_MAX_DISTANCE;
     if (far) distance -= BLZ_MAX_DISTANCE;                                   /* :559 */
     if (len < 7) {                                                           /* MATCH_SHORT[_FAR] */
-      BLZ_LIMIT(op + (far ? 4 : 2));
+      BLZE_HIT(far ? BLZE_H_SHORT_FAR : BLZE_H_SHORT_NEAR);
+      BLZ_LIMIT(op + (far ? 4 : 2), BLZE_H_LIM_SHORT);
       if (lane == 0) {
         if (!far) { out[op] = (u8)((len << 5) + (distance >> 8)); out[op + 1] = (u8)(distance & 255); }
         else { out[op] = (u8)((len << 5) + 31); out[op + 1] = 255; out[op + 2] = (u8)(distance >> 8); out[op + 3] = (u8)(distance & 255); }
@@ -264,7 +341,8 @@ DEV int blz_encode_main(const int clevel, const u8* __restrict__ b, const int le
     } else {                                                                 /* MATCH_LONG[_FAR] */
       len -= 7;
       const int nff = (int)(len / 255);
-      BLZ_LIMIT(op + 1 + nff + (far ? 4 : 2));
+      BLZE_HIT((far ? BLZE_H_LONG_FAR0 : BLZE_H_LONG_NEAR0) + (nff < 2 ? nff : 2));
+      BLZ_LIMIT(op + 1 + nff + (far ? 4 : 2), BLZE_H_LIM_LONG);
       if (lane == 0) out[op] = (u8)((7u << 5) + (far ? 31u : (distance >> 8)));
       op++;
       warp_fill_bytes(out + op, nff, 255);
@@ -280,11 +358,11 @@ DEV int blz_encode_main(const int clevel, const u8* __restrict__ b, const int le
     u32 seq = ld_u32(b + ip);
     if (lane == 0) {
       tab.put(blz_hash(seq, hashlog), ip);
-      if (clevel == 9) { seq >>= 8; tab.put(blz_hash(seq, hashlog), ip + 1); }
+      if (clevel == 9) { BLZE_HIT(BLZE_H_L9_STORE); seq >>= 8; tab.put(blz_hash(seq, hashlog), ip + 1); }
     }
     __syncwarp();
     ip += 2;
-    BLZ_LIMIT(op + 1);                                                       /* :582-586 */
+    BLZ_LIMIT(op + 1, BLZE_H_LIM_CTRL);                                      /* :582-586 */
     if (lane == 0) out[op] = BLZ_MAX_COPY - 1;
     op++;
   }
@@ -293,7 +371,7 @@ DEV int blz_encode_main(const int clevel, const u8* __restrict__ b, const int le
   while (ip <= ip_bound) {
     int nlit = ip_bound - ip + 1;
     if (nlit > 32) nlit = 32;
-    BLZ_LIMIT(op + (nlit - 1) + ((copy + nlit - 1) >> 5) + 2);
+    BLZ_LIMIT(op + (nlit - 1) + ((copy + nlit - 1) >> 5) + 2, BLZE_H_LIM_LEFT);
     if (lane < nlit) {
       const int o = op + lane + ((copy + lane) >> 5);
       out[o] = b[ip + lane];

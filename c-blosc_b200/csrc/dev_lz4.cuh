@@ -534,6 +534,64 @@ DEV bool lz4t_search(Lz4Team* tm, smem_addr_t vda, void* tabmem, const StreamBas
   return false;
 }
 
+/* branch ids of lz4_encode_stream's one-warp paths and of the search, emission and last-literals code it shares with
+ * team mode; emulator builds count them so that tests can tell which parse path a stream reached */
+enum {
+  /* chained "test next position" on the lane-cached window */
+  LZ4E_H_WIN_PREFETCHED, LZ4E_H_WIN_BLOCKING,  /* the window refilled from the prefetched words / with a blocking load */
+  LZ4E_H_WIN_PB_OFF,                         /* no prefetch: the next window would reach past the stream */
+  LZ4E_H_WIN_FLUSH,                          /* parked records flushed at a refill (nrec >= 24) */
+  LZ4E_H_CH_MISS,
+  LZ4E_H_CH_D65535, LZ4E_H_CH_D65536,        /* 32-bit table: equal bytes at distance 65535 (taken) / 65536 (refused) */
+  LZ4E_H_CH_LEN_REG, LZ4E_H_CH_LEN_X3, LZ4E_H_CH_LEN_X4,   /* the match length from x1|x2 / x3 / x4 */
+  LZ4E_H_CH_TAIL_BALLOT, LZ4E_H_CH_TAIL_LOOP,  /* ... from lz4_count_tail: inside its 128-byte ballot / past it */
+  LZ4E_H_CH_HUGE,                            /* a 270+ match leaves the chain */
+  LZ4E_H_CH_EXT,                             /* a record with a length byte (mc 15..269) */
+  LZ4E_H_CH_END_LAST, LZ4E_H_CH_END_PROBE,   /* ip + 64 > n: then ip >= mfl1 / the scalar probe */
+  /* scalar post-match probe */
+  LZ4E_H_POST_WIDE, LZ4E_H_POST_NARROW, LZ4E_H_POST_HIT, LZ4E_H_POST_MISS,
+  LZ4E_H_POST_D65535, LZ4E_H_POST_D65536,
+  /* search */
+  LZ4E_H_SP_HIT0,                            /* + k: a hit at scalar probe k (0..3) */
+  LZ4E_H_SP_ENDED = LZ4E_H_SP_HIT0 + 4,      /* the scalar probes ran into mflimit */
+  LZ4E_H_SP_D65535, LZ4E_H_SP_D65536,
+  LZ4E_H_R_HIT,                              /* a hit in a 32-wide round */
+  LZ4E_H_R_FWD_HIT, LZ4E_H_R_FWD_MISS,       /* a lane's candidate forwarded from a lower lane with its hash hits / misses */
+  LZ4E_H_R_PARTIAL,                          /* a round with fewer than 32 valid lanes */
+  LZ4E_H_R_STEP64, LZ4E_H_R_STEP128, LZ4E_H_R_STEP192,   /* a probe past 64 / 128 / 192: the step grew */
+  /* catch-up */
+  LZ4E_H_CU_NONE, LZ4E_H_CU_SHORT, LZ4E_H_CU_LONG,   /* none / < 32 bytes / 32 or more (a second ballot round) */
+  LZ4E_H_CU_ANCHOR, LZ4E_H_CU_ZERO,          /* stopped by the anchor / by position 0 */
+  /* match length */
+  LZ4E_H_ML_NEXT,                            /* have_next with x != 0 */
+  LZ4E_H_ML_X0, LZ4E_H_ML_X1, LZ4E_H_ML_X2, LZ4E_H_ML_TAIL,   /* room > 20 */
+  LZ4E_H_ML_ROOM20, LZ4E_H_ML_ROOM4,         /* room <= 20 / room <= 4 */
+  LZ4E_H_ML_CLAMP,                           /* mc > room */
+  LZ4E_H_ML_NARROW,                          /* !have_next */
+  /* emission */
+  LZ4E_H_EM_COMPACT,                         /* lit < 15 and mc < 15: one predicated store */
+  LZ4E_H_EM_LIT_FF0, LZ4E_H_EM_LIT_FF1, LZ4E_H_EM_LIT_FF2,   /* lit >= 15 with zero / one / two 255 bytes */
+  LZ4E_H_EM_ML_FF0, LZ4E_H_EM_ML_FF1, LZ4E_H_EM_ML_FF2,      /* mc >= 15 ... */
+  LZ4E_H_EM_IMM, LZ4E_H_EM_LITS,             /* a sequence without literals (post-match) / from the search */
+  /* limitedOutput: the check that refused the stream */
+  LZ4E_H_LIM_FLUSH, LZ4E_H_LIM_FIRST, LZ4E_H_LIM_COMPACT, LZ4E_H_LIM_LONG, LZ4E_H_LIM_LAST,
+  /* last literals */
+  LZ4E_H_LAST_SHORT, LZ4E_H_LAST_FF0, LZ4E_H_LAST_FF1,   /* lastRun < 15 / 15..269 / 270 and more */
+  LZ4E_H_LAST_NOPARSE,                       /* n < 13: no parse at all */
+  /* tables */
+  LZ4E_H_TAB_U16, LZ4E_H_TAB_U32, LZ4E_H_TAB_PACK,
+  LZ4E_H_PACK_HI,                            /* PACK: a match whose candidate is at position >= 65536 (bit 16) */
+  LZ4E_NHIT
+};
+#ifdef SIMT_EMU
+static long long g_lz4e_hit[LZ4E_NHIT + 1];       /* [LZ4E_NHIT]: "none of these", not counted */
+#define LZ4E_HIT(id) do { if (lane_id() == 0) g_lz4e_hit[id]++; } while (0)          /* warp-uniform branch */
+#define LZ4E_HITL(id, c) do { if (c) g_lz4e_hit[id]++; } while (0)                 /* per lane */
+#else
+#define LZ4E_HIT(id) do {} while (0)
+#define LZ4E_HITL(id, c) do {} while (0)
+#endif
+
 /* Returns the compressed size, or 0 when the stream does not fit in `cap`
  * (LZ4_compress_fast's limitedOutput failure).  Uniform across the warp.
  * `tabmem` is LZ4_TABLE_BYTES of shared memory private to this warp.
@@ -565,6 +623,7 @@ DEV int lz4_encode_stream(const u8* __restrict__ s, const int n, u8* __restrict_
 
   for (int i = lane; i < (PACK ? LZ4_TAB17_BYTES : LZ4_TABLE_BYTES) / 4; i += 32) tab32[i] = 0;   /* LZ4_initStream, lz4.c:1384 */
   __syncwarp();
+  LZ4E_HIT(U16 ? LZ4E_H_TAB_U16 : PACK ? LZ4E_H_TAB_PACK : LZ4E_H_TAB_U32);
 
   const bool limited = (long long)cap < (long long)n + n / 255 + 16;   /* lz4.c:1388,1395 */
   const int olimit = cap;
@@ -572,7 +631,7 @@ DEV int lz4_encode_stream(const u8* __restrict__ s, const int n, u8* __restrict_
   const int matchlimit = n - LZ4_LASTLITERALS;
   int ip = 1, anchor = 0, op = 0;
   int need = 0;                               /* max left-hand side of the limitedOutput checks = smallest capacity that passes */
-#define LZ4_LIMIT(v) do { const int v_ = (v); if (v_ > need) need = v_; if (limited && v_ > olimit) return 0; } while (0)
+#define LZ4_LIMIT(v, site) do { const int v_ = (v); if (v_ > need) need = v_; if (limited && v_ > olimit) { LZ4E_HIT(site); return 0; } } while (0)
   /* first byte (lz4.c:1005-1010): table[hash(0)] = 0, which the zeroed table already says */
 
   /* Lane-cached window for the literal-free chains that dominate shuffled data: lane l keeps the
@@ -587,7 +646,7 @@ DEV int lz4_encode_stream(const u8* __restrict__ s, const int n, u8* __restrict_
   int nrec = 0, recop = 0;
   u32 rec = 0;
   int twt = 0, tvt = -1;                     /* TEAM: `wt` as last published, highest tile whose ready word was checked */
-#define LZ4_FLUSH_CHECKED() do { if (nrec) { LZ4_LIMIT(op + (1 + LZ4_LASTLITERALS)); } LZ4_FLUSH(); } while (0)
+#define LZ4_FLUSH_CHECKED() do { if (nrec) { LZ4_LIMIT(op + (1 + LZ4_LASTLITERALS), LZ4E_H_LIM_FLUSH); } LZ4_FLUSH(); } while (0)
 #define LZ4_FLUSH() do { if (lane < nrec) { d[recop] = (u8)rec; d[recop + 1] = (u8)(rec >> 8); d[recop + 2] = (u8)(rec >> 16); \
                                              if ((rec & 15u) == 15u) d[recop + 3] = (u8)(rec >> 24); } nrec = 0; } while (0)
 
@@ -776,16 +835,18 @@ DEV int lz4_encode_stream(const u8* __restrict__ s, const int n, u8* __restrict_
         bool room = true;
         for (;;) {
           if (ip - 2 < w0 || ip > w0 + 31) {
-            if (nrec >= 24) LZ4_FLUSH_CHECKED();                             /* a window serves at most 8 sequences */
+            if (nrec >= 24) { LZ4E_HIT(LZ4E_H_WIN_FLUSH); LZ4_FLUSH_CHECKED(); }   /* a window serves at most 8 sequences */
             /* The window that follows (base w0+30: the first ip past this window is >= w0+32) was
              * requested at the previous refill, so its bytes are here by now; only a long match
              * that jumps over it pays for a blocking load. */
-            if (ip - 2 >= pb && ip <= pb + 31) { w0 = pb; ldp_take12(sb, w0 + lane, pq0, pq1, pq2, pq3, wq0, wq1, wq2); }
-            else { w0 = ip - 2; ldp_win12(sb, w0 + lane, wq0, wq1, wq2); }   /* reaches byte w0+46 < ip+64 <= n */
+            if (ip - 2 >= pb && ip <= pb + 31) {
+              LZ4E_HIT(LZ4E_H_WIN_PREFETCHED);
+              w0 = pb; ldp_take12(sb, w0 + lane, pq0, pq1, pq2, pq3, wq0, wq1, wq2);
+            } else { LZ4E_HIT(LZ4E_H_WIN_BLOCKING); w0 = ip - 2; ldp_win12(sb, w0 + lane, wq0, wq1, wq2); }   /* reaches byte w0+46 < ip+64 <= n */
             wh = lz4_hash_seq<U16>(wq0, wq1);
             pb = w0 + 30;
             if (pb + 31 + 16 <= n) ldp_raw12(sb, pb + lane, pq0, pq1, pq2, pq3);   /* not waited for */
-            else pb = -(1 << 30);
+            else { LZ4E_HIT(LZ4E_H_WIN_PB_OFF); pb = -(1 << 30); }
             lz4d_prefetch(s, w0 + 192, lane == 0 ? n : 0);                   /* the line a few refills ahead */
           }
           const int li = ip - w0;                                            /* 2 .. 31 */
@@ -801,22 +862,28 @@ DEV int lz4_encode_stream(const u8* __restrict__ s, const int n, u8* __restrict_
           if (lane == 0) LZ4_TPUT(h, ip);
           u32 c0, c1, c2;
           ldp_win12(sb, cand, c0, c1, c2);   /* cand is a position < ip whatever the table holds: safe even when it is too far back */
-          if (!((U16 || cand + 65535 >= ip) && c0 == seq)) { ip++; break; }  /* lz4.c:1298; on to the search below */
+          LZ4E_HIT(U16 || c0 != seq ? LZ4E_NHIT : ip - cand == 65535 ? LZ4E_H_CH_D65535 : ip - cand == 65536 ? LZ4E_H_CH_D65536 : LZ4E_NHIT);
+          if (!((U16 || cand + 65535 >= ip) && c0 == seq)) { LZ4E_HIT(LZ4E_H_CH_MISS); ip++; break; }  /* lz4.c:1298; on to the search below */
           int mc;
           const u32 x1 = n4 ^ c1, x2 = n8 ^ c2;
           if (x1 | x2) {
             const u32 xx = x1 ? x1 : x2;
             mc = ((__ffs((int)xx) - 1) >> 3) + (x1 ? 0 : 4);
+            LZ4E_HIT(LZ4E_H_CH_LEN_REG);
           } else {                                                           /* >= 12 bytes: next 8 from memory */
             u32 p3, p4, q3, q4;
             ldp_win8(sb, ip + 12, p3, p4);
             ldp_win8(sb, cand + 12, q3, q4);
             const u32 x3 = p3 ^ q3, x4 = p4 ^ q4;
-            if (x3) mc = 8 + eq_bytes32(x3);
-            else if (x4) mc = 12 + eq_bytes32(x4);
-            else mc = 16 + lz4_count_tail(sb, s, ip + 20, cand + 20, matchlimit, n);   /* ip+64 <= n: far from matchlimit */
+            if (x3) { mc = 8 + eq_bytes32(x3); LZ4E_HIT(LZ4E_H_CH_LEN_X3); }
+            else if (x4) { mc = 12 + eq_bytes32(x4); LZ4E_HIT(LZ4E_H_CH_LEN_X4); }
+            else {
+              mc = 16 + lz4_count_tail(sb, s, ip + 20, cand + 20, matchlimit, n);   /* ip+64 <= n: far from matchlimit */
+              LZ4E_HIT(mc < 16 + 128 && ip + 20 + 136 <= n ? LZ4E_H_CH_TAIL_BALLOT : LZ4E_H_CH_TAIL_LOOP);
+            }
           }
           if (mc >= 15 + 255) {                                              /* very long match: general emission below */
+            LZ4E_HIT(LZ4E_H_CH_HUGE);
             hit = true; imm = true; match = cand;
             have_mc = true; mc_carry = mc;
             break;
@@ -826,6 +893,8 @@ DEV int lz4_encode_stream(const u8* __restrict__ s, const int n, u8* __restrict_
            * grows inside a chain, so the check is made once per parked batch, before anything is
            * written (LZ4_FLUSH_CHECKED) */
           const bool ext = mc >= 15;
+          if (ext) LZ4E_HIT(LZ4E_H_CH_EXT);
+          if (PACK && cand >= 65536) LZ4E_HIT(LZ4E_H_PACK_HI);
           const int off = ip - cand;
           if (lane == nrec) { rec = (ext ? 15u | ((u32)(mc - 15) << 24) : (u32)mc) | ((u32)off << 8); recop = op; }
           nrec++;
@@ -835,6 +904,7 @@ DEV int lz4_encode_stream(const u8* __restrict__ s, const int n, u8* __restrict_
           if (ip + 64 > n) { room = false; break; }
         }
         if (!room) {                                                         /* a match ended close to the end of the stream */
+          LZ4E_HIT(ip >= mfl1 ? LZ4E_H_CH_END_LAST : LZ4E_H_CH_END_PROBE);
           if (ip >= mfl1) break;                                             /* lz4.c:1230-1233 */
           continue;                                                          /* post stays true: the plain probe below takes over */
         }
@@ -844,6 +914,7 @@ DEV int lz4_encode_stream(const u8* __restrict__ s, const int n, u8* __restrict_
         LZ4C_TW(c_r);
         u32 b0, b1, b2 = 0;
         const bool wide = ip + 14 <= n;
+        LZ4E_HIT(wide ? LZ4E_H_POST_WIDE : LZ4E_H_POST_NARROW);
         if (wide) ldp_win12(sb, ip - 2, b0, b1, b2);
         else { b0 = ld_u32(s + ip - 2); b1 = ld_u32(s + ip + 2); }
         const u32 seq = __funnelshift_r(b0, b1, 16);                       /* bytes ip .. ip+3 */
@@ -854,6 +925,7 @@ DEV int lz4_encode_stream(const u8* __restrict__ s, const int n, u8* __restrict_
         const int cand = LZ4_TGET(h);
         __syncwarp();                      /* every lane has read the old entry before lane 0 overwrites it */
         if (lane == 0) LZ4_TPUT(h, ip);
+        LZ4E_HIT(U16 || ld_u32(s + cand) != seq ? LZ4E_NHIT : ip - cand == 65535 ? LZ4E_H_POST_D65535 : ip - cand == 65536 ? LZ4E_H_POST_D65536 : LZ4E_NHIT);
         if (U16 || cand + 65535 >= ip) {
           u32 c0, c1;
           ldp_win8(sb, cand, c0, c1);
@@ -862,6 +934,7 @@ DEV int lz4_encode_stream(const u8* __restrict__ s, const int n, u8* __restrict_
             ipn = __funnelshift_r(b1, b2, 16); cn = c1; have_next = wide;
           }
         }
+        LZ4E_HIT(hit ? LZ4E_H_POST_HIT : LZ4E_H_POST_MISS);
         if (!hit) ip++;                                                    /* lz4.c:1298 */
         if (TEAM) LZ4C_SPAN(LZ4C_REPROBE, c_r);
       }
@@ -872,7 +945,7 @@ DEV int lz4_encode_stream(const u8* __restrict__ s, const int n, u8* __restrict_
         bool ended = false;
         for (int it = TEAM ? lit : 0; it < LZ4_SCALAR_PROBES; it++) {   /* TEAM: lit = first probe lz4t_search left */
           const int pos = ip + (it ? 1 + (it - 1) * accel : 0);            /* probe offsets 0, 1, 1+accel, 1+2*accel (lz4.c:1043-1053) */
-          if (ip + 1 + it * accel > mfl1) { ended = true; break; }         /* `goto _last_literals` (lz4.c:1055) */
+          if (ip + 1 + it * accel > mfl1) { LZ4E_HIT(LZ4E_H_SP_ENDED); ended = true; break; }   /* `goto _last_literals` (lz4.c:1055) */
           u32 b0, b1 = 0, b2 = 0;
           const bool wide = pos + 16 <= n;
           if (wide) ldp_win12(sb, pos, b0, b1, b2);
@@ -882,10 +955,12 @@ DEV int lz4_encode_stream(const u8* __restrict__ s, const int n, u8* __restrict_
           const int cand = LZ4_TGET(h);
           __syncwarp();
           if (lane == 0) LZ4_TPUT(h, pos);
+          LZ4E_HIT(U16 || ld_u32(s + cand) != b0 ? LZ4E_NHIT : pos - cand == 65535 ? LZ4E_H_SP_D65535 : pos - cand == 65536 ? LZ4E_H_SP_D65536 : LZ4E_NHIT);
           if (U16 || cand + 65535 >= pos) {
             u32 c0, c1;
             ldp_win8(sb, cand, c0, c1);
             if (c0 == b0) {
+              LZ4E_HIT(LZ4E_H_SP_HIT0 + it);
               hit = true; ip = pos; match = cand;
               ipn = b1; cn = c1; have_next = wide;
               break;
@@ -908,6 +983,10 @@ DEV int lz4_encode_stream(const u8* __restrict__ s, const int n, u8* __restrict_
             if (valid) {
               cand = lower ? ip + (int)lz4_probe_offset(base_it + (31 - __clz((int)lower)), accel) : LZ4_TGET(h);
               if (U16 || cand + 65535 >= pos) lhit = ld_u32(s + cand) == seq;   /* lz4.c:1090-1101 */
+              LZ4E_HITL(lhit ? LZ4E_H_R_FWD_HIT : LZ4E_H_R_FWD_MISS, lower != 0);
+              LZ4E_HITL(LZ4E_H_R_STEP64, itl - 1 >= 64);
+              LZ4E_HITL(LZ4E_H_R_STEP128, itl - 1 >= 128);
+              LZ4E_HITL(LZ4E_H_R_STEP192, itl - 1 >= 192);
             }
             const unsigned found = __ballot_sync(FULLMASK, lhit);
             const int nvalid = __popc(vmask);                       /* valid lanes form a prefix */
@@ -920,18 +999,21 @@ DEV int lz4_encode_stream(const u8* __restrict__ s, const int n, u8* __restrict_
             }
             __syncwarp();
             if (found) {
+              LZ4E_HIT(LZ4E_H_R_HIT);
               ip = __shfl_sync(FULLMASK, pos, f);
               match = __shfl_sync(FULLMASK, cand, f);
               hit = true;
               break;
             }
-            if (nvalid < 32) break;                                  /* ran into the end: last literals */
+            if (nvalid < 32) { LZ4E_HIT(LZ4E_H_R_PARTIAL); break; }  /* ran into the end: last literals */
           }
         }
         if (!hit) { if (TEAM) LZ4C_SPAN(LZ4C_SEARCH, c_f); break; }  /* -> last literals */
 
         /* ---- catch up (lz4.c:1107-1109) ---- */
         if (ip > anchor && match > 0 && s[ip - 1] == s[match - 1]) back = lz4_catch_up(s, ip, match, anchor, 0);
+        LZ4E_HIT(back == 0 ? LZ4E_H_CU_NONE : back < 32 ? LZ4E_H_CU_SHORT : LZ4E_H_CU_LONG);
+        if (back) LZ4E_HIT(ip - back == anchor ? LZ4E_H_CU_ANCHOR : match - back == 0 ? LZ4E_H_CU_ZERO : LZ4E_NHIT);
         lit = ip - back - anchor;
         if (TEAM) LZ4C_SPAN(LZ4C_SEARCH, c_f);
       }
@@ -945,19 +1027,22 @@ DEV int lz4_encode_stream(const u8* __restrict__ s, const int n, u8* __restrict_
         const int room = matchlimit - (ip + 4);                      /* >= 3 because ip < mflimitPlusOne */
         if (have_next) {
           const u32 x = ipn ^ cn;
-          if (x) mc = eq_bytes32(x);
+          if (x) { mc = eq_bytes32(x); LZ4E_HIT(LZ4E_H_ML_NEXT); }
           else if (room > 20) {
             u32 p0, p1, p2, q0, q1, q2;                              /* bytes [ip+8, ip+20) vs [match+8, match+20) */
             ldp_win12(sb, ip + 8, p0, p1, p2);                        /* ip+8+16 <= n because room > 20 */
             ldp_win12(sb, match + 8, q0, q1, q2);
             const u32 x0 = p0 ^ q0, x1 = p1 ^ q1, x2 = p2 ^ q2;
-            if (x0) mc = 4 + eq_bytes32(x0);
-            else if (x1) mc = 8 + eq_bytes32(x1);
-            else if (x2) mc = 12 + eq_bytes32(x2);
-            else mc = 16 + lz4_count_tail(sb, s, ip + 20, match + 20, matchlimit, n);
-          } else mc = 4 + (room > 4 ? warp_count_match(s, ip + 8, match + 8, matchlimit) : 0);
-          if (mc > room) mc = room;
-        } else mc = warp_count_match(s, ip + 4, match + 4, matchlimit);
+            if (x0) { mc = 4 + eq_bytes32(x0); LZ4E_HIT(LZ4E_H_ML_X0); }
+            else if (x1) { mc = 8 + eq_bytes32(x1); LZ4E_HIT(LZ4E_H_ML_X1); }
+            else if (x2) { mc = 12 + eq_bytes32(x2); LZ4E_HIT(LZ4E_H_ML_X2); }
+            else { mc = 16 + lz4_count_tail(sb, s, ip + 20, match + 20, matchlimit, n); LZ4E_HIT(LZ4E_H_ML_TAIL); }
+          } else {
+            LZ4E_HIT(room > 4 ? LZ4E_H_ML_ROOM20 : LZ4E_H_ML_ROOM4);
+            mc = 4 + (room > 4 ? warp_count_match(s, ip + 8, match + 8, matchlimit) : 0);
+          }
+          if (mc > room) { LZ4E_HIT(LZ4E_H_ML_CLAMP); mc = room; }
+        } else { LZ4E_HIT(LZ4E_H_ML_NARROW); mc = warp_count_match(s, ip + 4, match + 4, matchlimit); }
       }
       const int off = ip - match;
       ip += mc + 4;
@@ -967,9 +1052,12 @@ DEV int lz4_encode_stream(const u8* __restrict__ s, const int n, u8* __restrict_
       if (TEAM) LZ4C_ADD(LZ4C_SEQS, 1);
       LZ4_FLUSH_CHECKED();
       const int token = op++;
-      if (!imm) LZ4_LIMIT(op + lit + (2 + 1 + LZ4_LASTLITERALS) + lit / 255);
+      LZ4E_HIT(imm ? LZ4E_H_EM_IMM : LZ4E_H_EM_LITS);
+      if (PACK && match >= 65536) LZ4E_HIT(LZ4E_H_PACK_HI);
+      if (!imm) LZ4_LIMIT(op + lit + (2 + 1 + LZ4_LASTLITERALS) + lit / 255, LZ4E_H_LIM_FIRST);
       if (lit < 15 && mc < 15) {
-        LZ4_LIMIT(op + lit + 2 + (1 + LZ4_LASTLITERALS));
+        LZ4E_HIT(LZ4E_H_EM_COMPACT);
+        LZ4_LIMIT(op + lit + 2 + (1 + LZ4_LASTLITERALS), LZ4E_H_LIM_COMPACT);
         u32 v;
         if (lane == 0) v = ((u32)lit << 4) | (u32)mc;
         else if (lane <= lit) v = s[anchor + lane - 1];
@@ -980,6 +1068,7 @@ DEV int lz4_encode_stream(const u8* __restrict__ s, const int n, u8* __restrict_
         u32 tokval;
         if (lit >= 15) {
           const int len = lit - 15, nff = len / 255;
+          LZ4E_HIT(LZ4E_H_EM_LIT_FF0 + (nff < 2 ? nff : 2));
           tokval = 15u << 4;
           warp_fill_bytes(d + op, nff, 255);
           if (lane == 0) d[op + nff] = (u8)(len - nff * 255);
@@ -989,10 +1078,11 @@ DEV int lz4_encode_stream(const u8* __restrict__ s, const int n, u8* __restrict_
         op += lit;
         if (lane == 0) { d[op] = (u8)off; d[op + 1] = (u8)(off >> 8); }
         op += 2;
-        LZ4_LIMIT(op + (1 + LZ4_LASTLITERALS) + (mc + 240) / 255);
+        LZ4_LIMIT(op + (1 + LZ4_LASTLITERALS) + (mc + 240) / 255, LZ4E_H_LIM_LONG);
         if (mc >= 15) {
           tokval += 15;
           const int rest = mc - 15, nff = rest / 255;
+          LZ4E_HIT(LZ4E_H_EM_ML_FF0 + (nff < 2 ? nff : 2));
           warp_fill_bytes(d + op, nff, 255);
           if (lane == 0) d[op + nff] = (u8)(rest - nff * 255);
           op += nff + 1;
@@ -1009,7 +1099,9 @@ DEV int lz4_encode_stream(const u8* __restrict__ s, const int n, u8* __restrict_
   /* ---- last literals (lz4.c:1302-1329) ---- */
   LZ4_FLUSH_CHECKED();
   const int lastRun = n - anchor;
-  LZ4_LIMIT(op + lastRun + 1 + (lastRun + 255 - 15) / 255);
+  if (n < LZ4_MFLIMIT + 1) LZ4E_HIT(LZ4E_H_LAST_NOPARSE);
+  LZ4E_HIT(lastRun < 15 ? LZ4E_H_LAST_SHORT : lastRun < 270 ? LZ4E_H_LAST_FF0 : LZ4E_H_LAST_FF1);
+  LZ4_LIMIT(op + lastRun + 1 + (lastRun + 255 - 15) / 255, LZ4E_H_LIM_LAST);
   if (lastRun >= 15) {
     const int acc = lastRun - 15, nff = acc / 255;
     if (lane == 0) d[op] = (u8)(15u << 4);

@@ -269,6 +269,9 @@ int emu_blz_fail_line(void) { return g_blz_fail_line; }
 /* branch counters of the LZ4 decoders (LZ4D_H_*) and of the BloscLZ decoder (BLZ_H_*): copied out and cleared */
 int emu_lz4d_hits(long long* h) { for (int i = 0; i < LZ4D_NHIT; i++) { h[i] = g_lz4d_hit[i]; g_lz4d_hit[i] = 0; } return LZ4D_NHIT; }
 int emu_blz_hits(long long* h) { for (int i = 0; i < BLZ_NHIT; i++) { h[i] = g_blz_hit[i]; g_blz_hit[i] = 0; } return BLZ_NHIT; }
+/* branch counters of the one-warp LZ4 encoder (LZ4E_H_*) and of the BloscLZ encoder (BLZE_H_*): copied out and cleared */
+int emu_lz4e_hits(long long* h) { for (int i = 0; i < LZ4E_NHIT; i++) { h[i] = g_lz4e_hit[i]; g_lz4e_hit[i] = 0; } return LZ4E_NHIT; }
+int emu_blze_hits(long long* h) { for (int i = 0; i < BLZE_NHIT; i++) { h[i] = g_blze_hit[i]; g_blze_hit[i] = 0; } return BLZE_NHIT; }
 
 int emu_zlib_fail_line(void) { return g_inf_fail_line; }
 int emu_zlib_decode(const unsigned char* src, int csize, unsigned char* dst, int cap) {
